@@ -84,6 +84,24 @@ int shifted_lopbicg_switching(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, IN
 int shifted_lopbicg_switching_noovlp(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set,
                                      double *r_loc, double *sigma, int sigma_len, int seed);
 
+/* shifted_solver.h:17-21 (shifted_solver.c:182-1085): the LOP shifted BiCGStab family for (A + sigma_j I) x_j = b.  Same arguments as
+ * shifted_lopbicg_switching, but the seed never changes and every shift is advanced until max_j |1/(zeta_j pi_j)|^2 (r,r) <=
+ * EPS^2 (b,b) or MAX_ITER; returns k, the iterations performed (not k + 1).  EPS / MAX_ITER: BICG_SHIFT_TOL / BICG_SHIFT_MAX_ITER.
+ * shifted_lopbicgstab_v2 and _nooverlap only move the reference's per-shift updates and MPI waits; their arithmetic is that of
+ * shifted_lopbicgstab, so all three are the same solve here (LOP).  shifted_pipe_lopbicgstab_nooverlap is likewise the same solve as
+ * shifted_pipe_lopbicgstab (PIPE-LOP: the pipelined seed recurrences of pipe_bicgstab).  The reference's test_shifted.c calls
+ * shifted_pipe_lopbicgstab_nooverlap.  shifted_bicgstab (:16) is not provided. */
+int shifted_lopbicgstab(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set, double *r_loc,
+                        double *sigma, int sigma_len, int seed);
+int shifted_lopbicgstab_v2(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set, double *r_loc,
+                           double *sigma, int sigma_len, int seed);
+int shifted_lopbicgstab_nooverlap(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set,
+                                  double *r_loc, double *sigma, int sigma_len, int seed);
+int shifted_pipe_lopbicgstab(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set, double *r_loc,
+                             double *sigma, int sigma_len, int seed);
+int shifted_pipe_lopbicgstab_nooverlap(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set,
+                                       double *r_loc, double *sigma, int sigma_len, int seed);
+
 /* vector.h:4-7 (vector.c:3-27) on HOST arrays: the shifted drivers build and copy their right-hand sides with these
  * (main_shifted.c:114-135, main_repeat.c:121, main_seed_diff.c:118-121), so they are exported for those programs to link
  * unchanged (csrc/hostvec.cpp).  The solvers do not use them: their vector work is fused into the device kernels. */
@@ -162,6 +180,12 @@ int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nr
  * iteration at which every shift stopped (returns sigma_len). */
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats);
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap);
+/* Any shifted solver on a resident matrix: BICG_SHIFTED_SWITCHING = shifted_lopbicg_switching (returns iterations + 1, like
+ * bicg_shifted_solve), BICG_SHIFTED_LOP = shifted_lopbicgstab, BICG_SHIFTED_PIPE_LOP = shifted_pipe_lopbicgstab (both return the
+ * iterations performed).  -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len). */
+enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP = 2 };
+int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                          bicg_stats *stats);
 
 /* y_loc = A x_loc on a resident matrix (host pointers) -- the kernel behind MPI_csr_spmv_ovlap. */
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc);

@@ -47,6 +47,11 @@ SYMBOLS = {
     "pipe_bicgstab_rr": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicg_switching": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicg_switching_noovlp": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_lopbicgstab": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_lopbicgstab_v2": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_lopbicgstab_nooverlap": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_pipe_lopbicgstab": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_pipe_lopbicgstab_nooverlap": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     # vector.h:4-7 on host arrays (csrc/hostvec.cpp): what the shifted drivers prepare their right-hand sides with
     "my_daxpy": (None, [C.c_int, C.c_double, _P(C.c_double), _P(C.c_double)]),
     "my_ddot": (C.c_double, [C.c_int, _P(C.c_double), _P(C.c_double)]),
@@ -65,6 +70,7 @@ SYMBOLS = {
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_shifted_solve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_last_shift_info": (C.c_int, [_P(C.c_int), _P(C.c_int), C.c_int]),
+    "bicg_shifted_solve_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_spmv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "bicg_spmv_time": (C.c_int, [C.c_void_p, C.c_int, _P(C.c_double), _P(C.c_double)]),
     "bicg_profile_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _P(C.c_double), _P(C.c_int)]),

@@ -16,6 +16,7 @@ import numpy as np
 from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_stats, lib
 
 METHODS = {"bicgstab": 0, "ca_bicgstab": 1, "pipe_bicgstab": 2, "pipe_bicgstab_rr": 3}
+SHIFTED_METHODS = {"shifted_lopbicg_switching": 0, "shifted_lopbicgstab": 1, "shifted_pipe_lopbicgstab": 2}
 GEN_KINDS = {"stencil15": 0, "laplace5": 1, "random": 2, "convdiff": 3}
 
 
@@ -234,6 +235,27 @@ def shifted_lopbicg_switching(blk, x_set, r_loc, sigma, seed):
                                          _dptr(sigma), int(sigma.size), int(seed))
 
 
+def _shifted_args(blk, x_set, r_loc, sigma):
+    sigma = np.ascontiguousarray(sigma, dtype=np.float64)
+    assert x_set.dtype == np.float64 and x_set.flags["C_CONTIGUOUS"] and x_set.shape == (sigma.size, blk.n_loc)
+    return _dptr(x_set), _vec(r_loc, blk.n_loc), sigma
+
+
+def shifted_lopbicgstab(blk, x_set, r_loc, sigma, seed):
+    """shifted_solver.h:17 (LOP; its _v2 / _nooverlap twins are the same solve).  x_set: (sigma_len, n_loc) C-contiguous;
+    returns the iterations performed."""
+    xp, rp, sigma = _shifted_args(blk, x_set, r_loc, sigma)
+    return lib.shifted_lopbicgstab(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info), xp, rp, _dptr(sigma), int(sigma.size), int(seed))
+
+
+def shifted_pipe_lopbicgstab(blk, x_set, r_loc, sigma, seed):
+    """shifted_solver.h:20 (PIPE-LOP; its _nooverlap twin is the same solve).  Same arguments and return value as
+    shifted_lopbicgstab."""
+    xp, rp, sigma = _shifted_args(blk, x_set, r_loc, sigma)
+    return lib.shifted_pipe_lopbicgstab(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info), xp, rp, _dptr(sigma), int(sigma.size),
+                                        int(seed))
+
+
 def last_shift_info(sigma_len):
     seed = C.c_int()
     stop = (C.c_int * sigma_len)()
@@ -281,6 +303,13 @@ class DeviceMatrix:
         st = bicg_stats()
         it = lib.bicg_solve(self.h, METHODS[method], _vec(x, self.blk.n_loc), _vec(r, self.blk.n_loc), krr, nrr, 0, C.byref(st))
         return it, _stats_dict(st)
+
+    def shifted_solve(self, method, x_set, r, sigma, seed):
+        """bicg_shifted_solve_ex: method is a key of SHIFTED_METHODS; returns (that solver's return value, stats)."""
+        xp, rp, sigma = _shifted_args(self.blk, x_set, r, sigma)
+        st = bicg_stats()
+        k = lib.bicg_shifted_solve_ex(self.h, SHIFTED_METHODS[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
+        return k, _stats_dict(st)
 
     def spmv(self, x_loc):
         y = np.empty(self.blk.n_loc)

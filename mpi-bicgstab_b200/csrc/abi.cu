@@ -18,6 +18,22 @@ static_assert(offsetof(INFO_Matrix, code) == 12 && offsetof(INFO_Matrix, recvcou
 
 namespace {
 
+// shifted_solver.h entry points of the LOP family (pipe = 0: LOP, 1: PIPE-LOP)
+int run_shifted_lop(int pipe, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+                    int sigma_len, int seed)
+{
+    if (info->cols != info->rows) {                      // shifted_solver.c:190-193, 711-714
+        printf("Error: matrix is not square.\n");
+        exit(1);
+    }
+    Context &c = ctx();
+    c.ensure();
+    bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
+    const int k = shifted_lop_solve(m, pipe, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    if (!c.cfg.cache) matrix_destroy(m);
+    return k;
+}
+
 int run_reference_entry(int method, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x, double *r, int krr, int nrr)
 {
     if (info->cols != info->rows) {                      // solver.c:43-46
@@ -93,6 +109,37 @@ int shifted_lopbicg_switching_noovlp(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *
     return shifted_lopbicg_switching(D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 
+// shifted_solver.h: the LOP family.  Same prototype and meaning as shifted_lopbicg_switching, but every shift is advanced until all
+// have converged (no seed switch) and the return value is k, the iterations performed.  The reference's _v2 and _nooverlap twins
+// differ from their first function only in where the per-shift updates and the MPI waits sit; the arithmetic is the same (x, r,
+// history and return value of the compiled reference functions are bit-identical on the golden cases:
+// tests/test_oracle_golden_shifted_lop.py), so each twin is the same solve here.
+int shifted_lopbicgstab(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma, int sigma_len,
+                        int seed)                                                         // shifted_solver.h:17
+{
+    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+int shifted_lopbicgstab_v2(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+                           int sigma_len, int seed)                                       // shifted_solver.h:18
+{
+    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+int shifted_lopbicgstab_nooverlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+                                  int sigma_len, int seed)                                // shifted_solver.h:19
+{
+    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+int shifted_pipe_lopbicgstab(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+                             int sigma_len, int seed)                                     // shifted_solver.h:20
+{
+    return run_shifted_lop(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+int shifted_pipe_lopbicgstab_nooverlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc,
+                                       double *sigma, int sigma_len, int seed)            // shifted_solver.h:21
+{
+    return run_shifted_lop(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+
 void MPI_csr_spmv_ovlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc, double *x, double *y_loc)
 {
     Context &c = ctx();
@@ -166,6 +213,23 @@ int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *s
 {
     Context &c = ctx();
     const int k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    if (stats) *stats = c.last_stats;
+    return k;
+}
+int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                          bicg_stats *stats)
+{
+    Context &c = ctx();
+    c.ensure();
+    int k;
+    switch (method) {
+    case BICG_SHIFTED_SWITCHING: k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter); break;
+    case BICG_SHIFTED_LOP:
+    case BICG_SHIFTED_PIPE_LOP:
+        k = shifted_lop_solve(m, method == BICG_SHIFTED_PIPE_LOP, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+        break;
+    default: return -1;
+    }
     if (stats) *stats = c.last_stats;
     return k;
 }

@@ -233,6 +233,9 @@ int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);
 // shifted.cu
 int  shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol, int max_iter);
+// shifted_lop.cu (pipe = 0: LOP, 1: PIPE-LOP); returns the iterations performed, -1 for a bad sigma_len / seed
+int  shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
+                       int max_iter);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, int prof_class = 0);

@@ -12,6 +12,7 @@
 // Element-wise operation order = the reference's call order with gcc's FMA contraction (y += a x -> fma(a, x, y)).
 // The host only enqueues batches of iterations and polls a done flag (as solve.cu does).
 #include "engine.hpp"
+#include "shifted_run.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -302,67 +303,11 @@ __global__ void __launch_bounds__(256) sh_vec_p(const __grid_constant__ ShVec a)
     }
 }
 
-inline TailDesc tail_none() { return TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0}; }
-inline TailDesc tail_store(int ndot) { return TailDesc{TAIL_ALLREDUCE, FIN_STORE_PEND, ndot, 0, 0, 0, 0}; }
-
-__global__ void sh_reset_scalars(Scalars *s)
-{
-    s->alpha = s->beta = s->omega = 0.0;
-    for (int k = 0; k < MAX_DOTS; ++k) s->pend[k] = 0.0;
-    s->k = 0; s->max_iter = 0; s->done = 0; s->converged = 0; s->error = 0; s->ticket = 0u;
-}
-
-struct ShRun {
-    bicg_matrix *m;
-    Context &c;
+struct ShRun : ShiftLaunch {
     ShiftDev *d_sd;
     ShVec base{};
-    int launches = 0;
-    explicit ShRun(bicg_matrix *mm) : m(mm), c(ctx()), d_sd(nullptr) {}
+    explicit ShRun(bicg_matrix *mm) : ShiftLaunch(mm), d_sd(nullptr) {}
 
-    PushDesc make_push(int id) const
-    {
-        PushDesc pd{};
-        if (m->world == 1) return pd;
-        pd.npeers = m->npush; pd.fence_writers = c.cfg.fence_writers;
-        pd.src = m->vec(id);
-        for (int s = 0; s < m->npush; ++s) {
-            const int d = m->push_peer[s];
-            pd.dst[s] = (double *)((char *)m->peer_base[d] + m->peer_vec_off[d]) + (long long)id * m->peer_vstride[d] + m->peer_ghost_off[d];
-            pd.runs[s] = m->d_push_runs[s]; pd.nruns[s] = m->push_nruns[s];
-        }
-        return pd;
-    }
-    VecArgs vec_args(TailDesc tail) const
-    {
-        VecArgs a{};
-        a.kc.sc = m->d_sc; a.kc.partials = m->d_partials; a.kc.hist = m->d_hist; a.kc.comm = m->comm; a.kc.tail = tail;
-        a.v.x = m->vec(V_X); a.v.r = m->vec(V_R); a.v.rh = m->vec(V_RH); a.v.p = m->vec(V_P); a.v.s = m->vec(V_S);
-        a.v.y = m->vec(V_Y); a.v.z = m->vec(V_Z); a.v.w = m->vec(V_W); a.v.v = m->vec(V_V); a.v.t = m->vec(V_T);
-        a.v.b = m->vec(V_B); a.v.ax = m->vec(V_AX);
-        a.n = m->n_loc; a.chunk = m->vchunk;
-        return a;
-    }
-    void push(int id)                             // halo of arena vector `id` for the next SpMV (kernel-per-phase protocol)
-    {
-        if (m->world == 1) return;
-        VecArgs a = vec_args(tail_none());
-        a.kc.tail.signal_halo = 1;
-        a.push = make_push(id);
-        int rc = launch_vec(PH_PUSH, m->vgrid, a, c.stream);
-        if (rc) fatal("bicgstab_b200: push kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        ++launches; ++c.launches;
-    }
-    void spmv(int x_id, int y_id, int ndot, const double *a0, const double *b0, const double *a1 = nullptr, const double *b1 = nullptr)
-    {
-        SpmvArgs a = make_spmv_args(m, m->plan, x_id, y_id);
-        a.kc.tail = tail_store(ndot);
-        a.shift_sigma = &d_sd->sigma_seed;
-        epi_add_dot(a.epi, a0, b0);
-        if (ndot > 1) epi_add_dot(a.epi, a1, b1);
-        launch_spmv_plan(m, m->plan, a, 0);
-        ++launches;
-    }
     ShVec vargs(TailDesc tail) const
     {
         ShVec v = base;
@@ -431,6 +376,7 @@ int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma,
 
     ShRun run(m);
     run.d_sd = d_sd;
+    run.shift_sigma = &d_sd->sigma_seed;
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);

@@ -1,0 +1,445 @@
+// shifted_lop.cu -- the LOP shifted BiCGStab solvers of shifted_solver.h for (A + sigma_j I) x_j = b, j = 0 .. sigma_len - 1:
+//   LOP      shifted_lopbicgstab (shifted_solver.c:182-354; _v2 :357-529 and _nooverlap :531-701 are the same arithmetic)
+//   PIPE-LOP shifted_pipe_lopbicgstab (:703-895; _nooverlap :897-1085 is the same arithmetic), the pipelined seed recurrences
+//            of pipe_bicgstab (s, z, w, v, t) with the same per-shift updates.
+// The seed never changes and no shift stops on its own: every non-seed shift is advanced in every iteration until
+// max_zeta_pi^2 dot_r <= tol^2 dot_zero (max_zeta_pi = max(1, max_j |1 / (zeta_j pi_j)|)) or MAX_ITER.
+//
+// Per iteration the seed runs on the arena vectors with the shifted SpMV epilogue (y = A x + sigma_seed x, shifted_run.cuh),
+// one scalar kernel derives every shift's coefficients (lop_scalar_shift), and ONE fused pass (lop_vec_update) updates the
+// seed's x and residual together with x_j and p_j of every shift, each read and written exactly once (32 B per row and
+// shift).  The reference scales p_j at the START of an iteration (p_j = beta_j p_j + r / (pi zeta), :264-269); that step is
+// moved into the same pass, where r of the iteration start is r_old, so the pass does
+//   p_j = beta_j p_j + c4 r_old ;  x_j += c1 q + alpha_j p_j ;  p_j += c2 q + c3 r_old
+// with the reference's operands and operation order.  Iteration 1 starts from p_j = 0, beta_j = 0, c4 = 1: p_j = r exactly.
+// Element-wise order = the reference's call order with gcc's FMA contraction (y += a x -> fma(a, x, y)).
+// Pinned undefined behaviour: PIPE-LOP reads omega[seed] and s, z, v before writing them in its first iteration (:795-803);
+// they start at 0 here, as with the oracle's zero-filling malloc (DESIGN.md section 1).
+#include "engine.hpp"
+#include "shifted_run.cuh"
+
+#include <algorithm>
+#include <cmath>
+
+namespace bicg {
+
+namespace {
+
+constexpr int LOP_COEF = 6;         // per non-seed shift: beta_j, c4, c1, alpha_j, c2, c3
+
+struct LopDev {
+    int L, max_iter, seed, k, done;
+    double tol;
+    double sigma_seed;                                  // read by the SpMV epilogue
+    double rTr, rTr_old, dot_r, dot_zero, max_zeta_pi;
+    double alpha, alpha_old, beta, omega;               // alpha_set[seed], alpha_old, beta_set[seed], omega_set[seed]
+    double *sigma, *eta, *zeta, *pi_old, *pi_new;       // [L]
+    double *coef;                                       // [L - 1][LOP_COEF]; slot t is shift t < seed ? t : t + 1
+    double *hist;                                       // [max_iter + 1]
+};
+
+__device__ __forceinline__ bool loop_go(const LopDev *sd)                      // :259 / :793
+{
+    return sd->max_zeta_pi * sd->max_zeta_pi * sd->dot_r > sd->tol * sd->tol * sd->dot_zero && sd->k < sd->max_iter;
+}
+
+// ---- scalar kernels ------------------------------------------------------------------------------------------------
+// (r,r) of b; LOP: alpha_set[seed] = 1 (:246); PIPE-LOP: alpha_old = 1, alpha is set by lop_scalar_pipe_init (:786-787)
+__global__ void lop_scalar_init(LopDev *sd, Scalars *sc, int pipe)
+{
+    const int t = threadIdx.x;
+    if (t == 0) {
+        sd->rTr = sc->pend[0]; sd->dot_r = sd->rTr; sd->dot_zero = sd->rTr;   // :255-256 / :788-789
+        sd->k = 0; sd->done = 0; sd->max_zeta_pi = 1.0;
+        sd->alpha = 1.0; sd->alpha_old = 1.0; sd->beta = 0.0; sd->omega = 0.0;
+        sd->hist[0] = 1.0;
+        if (!pipe && !loop_go(sd)) { sd->done = 1; sc->done = 1; }
+    }
+    for (int j = t; j < sd->L; j += blockDim.x) { sd->eta[j] = 0.0; sd->zeta[j] = 1.0; sd->pi_old[j] = 1.0; sd->pi_new[j] = 1.0; }   // :243-251
+}
+__global__ void lop_scalar_pipe_init(LopDev *sd, Scalars *sc)                  // alpha = (r,r) / (r,w)   :787
+{
+    sd->alpha = sd->rTr / sc->pend[0];
+    if (!loop_go(sd)) { sd->done = 1; sc->done = 1; }
+}
+__global__ void lop_scalar_alpha(LopDev *sd, Scalars *sc)                      // LOP :272-276
+{
+    if (sd->done) return;
+    sd->alpha_old = sd->alpha;
+    sd->alpha = sd->rTr / sc->pend[0];
+}
+// omega from the two pending dots, then every shift's coefficients and max |1/(zeta pi)|: one block
+//   LOP :264-270, 283-289, 293, 296-304, 313-318;  PIPE-LOP :804-809, 817-825, 829, 832-840, 860-865
+__global__ void __launch_bounds__(512) lop_scalar_shift(LopDev *sd, Scalars *sc)
+{
+    if (sd->done) return;
+    __shared__ double s_max[512 / 32];
+    const int t = threadIdx.x, T = blockDim.x;
+    const double om = sc->pend[0] / sc->pend[1];                                // (q,q)/(q,y) resp. (q,y)/(y,y)
+    const double al = sd->alpha, al_o = sd->alpha_old, be_o = sd->beta, sg_s = sd->sigma_seed;
+    const int seed = sd->seed;
+    double mx = 1.0;
+    for (int s = t; s < sd->L - 1; s += T) {
+        const int j = s < seed ? s : s + 1;
+        const double pi_oo = sd->pi_old[j], pi_o = sd->pi_new[j], zeta_o = sd->zeta[j], dsg = sg_s - sd->sigma[j];
+        const double be_j = (pi_oo / pi_o) * (pi_oo / pi_o) * be_o;              // :266 / :806
+        const double c4 = 1.0 / (pi_o * zeta_o);                                // :268 / :808
+        const double eta = (be_o / al_o) * al * sd->eta[j] - dsg * al * pi_o;    // :285 / :821 (pi_old <- pi_new, :270 / :817)
+        const double pi_n = eta + pi_o;                                         // :287 / :823
+        const double al_j = (pi_o / pi_n) * al;                                 // :288 / :824
+        const double om_j = om / (1.0 - om * dsg);                              // :298 / :834
+        const double c1 = om_j / (pi_n * zeta_o);                               // :299 / :835
+        const double c2 = om_j / (al_j * zeta_o * pi_n);                        // :301 / :837
+        const double c3 = -om_j / (al_j * zeta_o * pi_o);                       // :302 / :838
+        const double zeta_n = (1.0 - om * dsg) * zeta_o;                        // :303 / :839
+        sd->eta[j] = eta; sd->pi_old[j] = pi_o; sd->pi_new[j] = pi_n; sd->zeta[j] = zeta_n;
+        double *c = sd->coef + (size_t)s * LOP_COEF;
+        c[0] = be_j; c[1] = c4; c[2] = c1; c[3] = al_j; c[4] = c2; c[5] = c3;
+        const double azp = fabs(1.0 / (zeta_n * pi_n));                         // :316 / :863
+        if (azp > mx) mx = azp;
+    }
+    for (int o = 16; o > 0; o >>= 1) { const double v = __shfl_xor_sync(0xffffffffu, mx, o); if (v > mx) mx = v; }
+    if ((t & 31) == 0) s_max[t >> 5] = mx;
+    __syncthreads();
+    if (t == 0) {
+        for (int w = 1; w < (T + 31) / 32; ++w) if (s_max[w] > mx) mx = s_max[w];
+        sd->max_zeta_pi = mx;
+        sd->omega = om;
+    }
+}
+// beta, the loop test and the history once the fused pass's dots are known
+//   LOP      pend = (r,r), (r#,r)                               :306-312, 323
+//   PIPE-LOP pend = (r,r), (r#,r), (r#,w), (r#,s), (r#,z)       :842-859, 867
+__global__ void lop_scalar_end(LopDev *sd, Scalars *sc, int pipe)
+{
+    if (sd->done) return;
+    sd->dot_r = sc->pend[0];
+    sd->rTr_old = sd->rTr;
+    sd->rTr = sc->pend[1];
+    sd->beta = (sd->alpha / sd->omega) * (sd->rTr / sd->rTr_old);
+    if (pipe) {
+        const double rTw = sc->pend[2], rTs = sc->pend[3], rTz = sc->pend[4];
+        sd->alpha_old = sd->alpha;
+        sd->alpha = sd->rTr / (rTw + sd->beta * (rTs - sd->omega * rTz));
+    }
+    sd->k += 1;
+    sd->hist[sd->k] = sd->dot_r / sd->dot_zero;
+    if (!loop_go(sd)) { sd->done = 1; sc->done = 1; }
+}
+
+// ---- vector kernels -----------------------------------------------------------------------------------------------
+struct LopVec {
+    KernelCommon kc;
+    const LopDev *sd;
+    double *r, *rh, *p, *s, *y, *z, *w, *v, *t, *rold;  // arena vectors (own parts); y, z, w, v, t as the algorithm uses them
+    double *x_set, *p_set;
+    long long stride;                                   // doubles between consecutive shifts in x_set / p_set
+    int n, L;
+};
+
+__device__ __forceinline__ void ld2(const double *p, int i, bool two, double (&v)[2])
+{
+    if (two) { const double2 t = *reinterpret_cast<const double2 *>(p + i); v[0] = t.x; v[1] = t.y; }
+    else { v[0] = p[i]; v[1] = 0.0; }
+}
+__device__ __forceinline__ void st2(double *p, int i, bool two, const double (&v)[2])
+{
+    if (two) *reinterpret_cast<double2 *>(p + i) = make_double2(v[0], v[1]);
+    else p[i] = v[0];
+}
+
+// r# = r, p[seed] = r, (r,r); PIPE-LOP also zeroes s, z, v (pinned, see the top)          :240-252 / :763, 772-782
+__global__ void __launch_bounds__(256) lop_vec_init(const __grid_constant__ LopVec a, int pipe)
+{
+    __shared__ double scratch[32 * MAX_DOTS];
+    double dot[1] = {0.0};
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+        const double r = a.r[i];
+        a.rh[i] = r; a.p[i] = r;
+        if (pipe) { a.s[i] = 0.0; a.z[i] = 0.0; a.v[i] = 0.0; }
+        dot[0] = fma(r, r, dot[0]);
+    }
+    block_sum<1>(dot, scratch);
+    kernel_tail<1>(a.kc, dot, scratch);
+}
+// LOP: r_old = r; q = r - alpha s (in r)                                                   :271, 277
+__global__ void __launch_bounds__(256) lop_vec_q(const __grid_constant__ LopVec a)
+{
+    if (a.sd->done) return;
+    const double al = a.sd->alpha;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+        const double r = a.r[i];
+        a.rold[i] = r; a.r[i] = fma(-al, a.s[i], r);
+    }
+}
+// LOP: p[seed] = r + beta p[seed] - beta omega s                                           :319-321
+__global__ void __launch_bounds__(256) lop_vec_p(const __grid_constant__ LopVec a)
+{
+    if (a.sd->done) return;
+    const double be = a.sd->beta, nbo = -a.sd->beta * a.sd->omega;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+        double t = be * a.p[i];
+        t = fma(1.0, a.r[i], t);
+        a.p[i] = fma(nbo, a.s[i], t);
+    }
+}
+// PIPE-LOP: p, s, z recurrences; r_old = r; q = r - alpha s (in r); y = w - alpha z (in w); (q,y), (y,y)      :795-803, 810-814
+__global__ void __launch_bounds__(256) lop_vec_pipe1(const __grid_constant__ LopVec a)
+{
+    if (a.sd->done) return;
+    __shared__ double scratch[32 * MAX_DOTS];
+    const double al = a.sd->alpha, be = a.sd->beta, om = a.sd->omega;
+    double dot[2] = {0.0, 0.0};
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+        const double r = a.r[i], w = a.w[i], s0 = a.s[i], z0 = a.z[i];
+        double u = fma(-om, s0, a.p[i]);   u = be * u;  a.p[i] = fma(1.0, r, u);
+        double sv = fma(-om, z0, s0);      sv = be * sv; sv = fma(1.0, w, sv);
+        double zv = fma(-om, a.v[i], z0);  zv = be * zv; zv = fma(1.0, a.t[i], zv);
+        const double q = fma(-al, sv, r), y = fma(-al, zv, w);
+        a.s[i] = sv; a.z[i] = zv; a.rold[i] = r; a.r[i] = q; a.w[i] = y;
+        dot[0] = fma(q, y, dot[0]);
+        dot[1] = fma(y, y, dot[1]);
+    }
+    block_sum<2>(dot, scratch);
+    kernel_tail<2>(a.kc, dot, scratch);
+}
+// The seed's x and residual and every shift's x_j, p_j in one pass over the rows (two rows per thread, 16-byte accesses).
+//   seed   x[seed] += alpha p + omega q; r = q - omega y                                   :294-295, 305 / :830-831, 841
+//          PIPE-LOP: w = y - omega (t - alpha v)                                          :843-844
+//   shifts p_j = beta_j p_j + c4 r_old; x_j += c1 q + alpha_j p_j; p_j += c2 q + c3 r_old   :267-268, 299-302 / :807-808, 835-838
+//   dots   LOP (r,r), (r#,r)                                                               :306, 308
+//          PIPE-LOP (r,r), (r#,r), (r#,w), (r#,s), (r#,z)                                  :842, 846-849
+template <bool PIPE>
+__global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ LopVec a)
+{
+    const LopDev *sd = a.sd;
+    if (sd->done) return;
+    constexpr int ND = PIPE ? 5 : 2;
+    __shared__ double scratch[32 * MAX_DOTS];
+    extern __shared__ double s_coef[];                  // [L - 1][LOP_COEF]
+    const int na = a.L - 1, seed = sd->seed;
+    for (int t = threadIdx.x; t < na * LOP_COEF; t += blockDim.x) s_coef[t] = sd->coef[t];
+    __syncthreads();
+    const double al = sd->alpha, om = sd->omega;
+    double *xs = a.x_set + (size_t)seed * a.stride;
+    double dot[ND];
+#pragma unroll
+    for (int d = 0; d < ND; ++d) dot[d] = 0.0;
+    for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
+        const bool two = i + 1 < a.n;                   // stride and arena vectors are 16-byte aligned, i is even
+        const int ne = two ? 2 : 1;
+        double q[2], o[2], x[2], p[2], y[2], r[2], rh[2];
+        ld2(a.r, i, two, q); ld2(a.rold, i, two, o); ld2(xs, i, two, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
+        ld2(PIPE ? a.w : a.y, i, two, y);
+        for (int e = 0; e < ne; ++e) {
+            x[e] = fma(al, p[e], x[e]);
+            x[e] = fma(om, q[e], x[e]);
+            r[e] = fma(-om, y[e], q[e]);
+            dot[0] = fma(r[e], r[e], dot[0]);
+            dot[1] = fma(rh[e], r[e], dot[1]);
+        }
+        st2(xs, i, two, x); st2(a.r, i, two, r);
+        if constexpr (PIPE) {
+            double t[2], v[2], w[2], s[2], z[2];
+            ld2(a.t, i, two, t); ld2(a.v, i, two, v); ld2(a.s, i, two, s); ld2(a.z, i, two, z);
+            for (int e = 0; e < ne; ++e) {
+                t[e] = fma(-al, v[e], t[e]);            // t itself is overwritten by t = (A + sigma I) w next
+                w[e] = fma(-om, t[e], y[e]);
+                dot[2] = fma(rh[e], w[e], dot[2]);
+                dot[3] = fma(rh[e], s[e], dot[3]);
+                dot[4] = fma(rh[e], z[e], dot[4]);
+            }
+            st2(a.w, i, two, w);
+        }
+        if (!two) { q[1] = 0.0; o[1] = 0.0; }
+#pragma unroll 2
+        for (int t = 0; t < na; ++t) {
+            const double *c = s_coef + (size_t)t * LOP_COEF;
+            const size_t j = (size_t)(t < seed ? t : t + 1);
+            double *xj = a.x_set + j * a.stride + i, *pj = a.p_set + j * a.stride + i;
+            double xv[2], pv[2];
+            ld2(xj, 0, two, xv); ld2(pj, 0, two, pv);
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                pv[e] = c[0] * pv[e]; pv[e] = fma(c[1], o[e], pv[e]);
+                xv[e] = fma(c[2], q[e], xv[e]); xv[e] = fma(c[3], pv[e], xv[e]);
+                pv[e] = fma(c[4], q[e], pv[e]); pv[e] = fma(c[5], o[e], pv[e]);
+            }
+            st2(xj, 0, two, xv); st2(pj, 0, two, pv);
+        }
+    }
+    block_sum<ND>(dot, scratch);
+    kernel_tail<ND>(a.kc, dot, scratch);
+}
+
+struct LopRun : ShiftLaunch {
+    LopDev *d_sd = nullptr;
+    LopVec base{};
+    bool pipe = false;
+    int ugrid = 1;                                      // grid of lop_vec_update
+    size_t smem = 0;                                    // its coefficient table
+    explicit LopRun(bicg_matrix *mm) : ShiftLaunch(mm) {}
+
+    LopVec vargs(TailDesc tail) const
+    {
+        LopVec v = base;
+        v.kc.sc = m->d_sc; v.kc.partials = m->d_partials; v.kc.hist = m->d_hist; v.kc.comm = m->comm; v.kc.tail = tail;
+        return v;
+    }
+    void prologue()
+    {
+        const int G = m->vgrid;
+        lop_vec_init<<<G, 256, 0, c.stream>>>(vargs(tail_store(1)), pipe ? 1 : 0);
+        lop_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc, pipe ? 1 : 0);
+        c.launches += 2;
+        if (!pipe) { push(V_P); return; }
+        push(V_R);
+        spmv(V_R, V_W, 1, m->vec(V_R), nullptr);                                       // w = (A + sigma I) r, (r,w)  :765-767
+        lop_scalar_pipe_init<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                       :787
+        push(V_W);
+        spmv(V_W, V_T, 0);                                                             // t = (A + sigma I) w          :769-770
+        launches += 1; c.launches += 1;
+    }
+    void iteration()
+    {
+        const int G = m->vgrid;
+        if (!pipe) {
+            spmv(V_P, V_S, 1, m->vec(V_RH), nullptr);                                  // s = (A + sigma I) p, (r#,s)   :261-263
+            lop_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                        :276
+            lop_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // r_old, q                     :271, 277
+            push(V_R);
+            spmv(V_R, V_Y, 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);         // y = (A + sigma I) q, (q,q), (q,y)  :278-282
+            lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            lop_vec_update<false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
+            lop_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // p[seed]                      :319-321
+            push(V_P);
+            launches += 6; c.launches += 6;
+        } else {
+            lop_vec_pipe1<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));              // p, s, z, q, y, (q,y), (y,y)   :795-814
+            push(V_Z);
+            spmv(V_Z, V_V, 0);                                                         // v = (A + sigma I) z           :815-816
+            lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            lop_vec_update<true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            push(V_W);
+            spmv(V_W, V_T, 0);                                                         // t = (A + sigma I) w           :850-851
+            lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 1);                   // beta, alpha, loop test       :857-865
+            launches += 4; c.launches += 4;
+        }
+    }
+};
+
+} // namespace
+
+int shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
+                      int max_iter)
+{
+    Context &c = ctx();
+    c.ensure();
+    if (L <= 0 || seed < 0 || seed >= L) return -1;
+    const int n = m->n_loc;
+    const long long stride = ((long long)n + 15) / 16 * 16;
+
+    // ---- device state -------------------------------------------------------------------------------------------------
+    LopDev h{};
+    h.L = L; h.max_iter = max_iter; h.tol = tol; h.seed = seed; h.sigma_seed = sigma[seed];
+    auto dalloc = [&](size_t bytes) { return c.dev_alloc(std::max<size_t>(bytes, 16)); };
+    h.sigma = (double *)dalloc(L * sizeof(double));
+    h.eta = (double *)dalloc(L * sizeof(double)); h.zeta = (double *)dalloc(L * sizeof(double));
+    h.pi_old = (double *)dalloc(L * sizeof(double)); h.pi_new = (double *)dalloc(L * sizeof(double));
+    h.coef = (double *)dalloc((size_t)(L - 1) * LOP_COEF * sizeof(double));
+    h.hist = (double *)dalloc(((size_t)max_iter + 1) * sizeof(double));
+    LopDev *d_sd = (LopDev *)dalloc(sizeof(LopDev));
+    double *d_x = (double *)dalloc((size_t)L * stride * sizeof(double));
+    double *d_p = (double *)dalloc((size_t)L * stride * sizeof(double));
+    BICG_CUDA(cudaMemcpyAsync(d_sd, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
+    BICG_CUDA(cudaMemcpyAsync(h.sigma, sigma, L * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+    BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), c.stream));
+    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)L * stride * sizeof(double), c.stream));          // p_loc_set = calloc(...)  :226
+    BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
+                                cudaMemcpyHostToDevice, c.stream));
+    BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+    sh_reset_scalars<<<1, 1, 0, c.stream>>>(m->d_sc);
+
+    LopRun run(m);
+    run.pipe = pipe != 0;
+    run.d_sd = d_sd;
+    run.shift_sigma = &d_sd->sigma_seed;
+    run.base.sd = d_sd;
+    run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
+    run.base.y = m->vec(V_Y); run.base.z = m->vec(V_Z); run.base.w = m->vec(V_W); run.base.v = m->vec(V_V); run.base.t = m->vec(V_T);
+    run.base.rold = m->vec(run.pipe ? V_AX : V_V);
+    run.base.x_set = d_x; run.base.p_set = d_p; run.base.stride = stride; run.base.n = n; run.base.L = L;
+    run.ugrid = std::max(1, std::min(c.sm_count * 8, (n + 511) / 512));
+    run.smem = (size_t)(L - 1) * LOP_COEF * sizeof(double);
+    if (run.smem > 48 * 1024) {
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+    }
+
+    cudaEvent_t e0, e1;
+    BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
+    const int launches0 = c.launches;
+    BICG_CUDA(cudaEventRecord(e0, c.stream));                                         // the reference's timed region :237 / :759
+    run.prologue();
+
+    const int U = 8, DEPTH = 2, RING = 64;
+    std::vector<cudaEvent_t> ring((size_t)RING, nullptr);
+    const int batches = (max_iter + U - 1) / U;
+    for (int b = 0; b < batches; ++b) {
+        if (b >= DEPTH) {
+            const int o = (b - DEPTH) % RING;
+            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
+            if (c.h_flags[o * 4 + 0]) break;                                          // done was raised in batch b - DEPTH
+        }
+        for (int u = 0; u < U; ++u) run.iteration();
+        const int o = b % RING;
+        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o * 4], &d_sd->done, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
+        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
+    }
+    BICG_CUDA(cudaEventRecord(e1, c.stream));
+
+    // ---- results ------------------------------------------------------------------------------------------------------
+    BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
+                                cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+    LopDev out{};
+    BICG_CUDA(cudaMemcpyAsync(&out, d_sd, sizeof(LopDev), cudaMemcpyDeviceToHost, c.stream));
+    Scalars hs;
+    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);
+    if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted solver", m->rank);
+    float ms = 0.f;
+    BICG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+    cudaEventDestroy(e0); cudaEventDestroy(e1);
+
+    const int k = out.k;
+    c.last_hist.assign((size_t)k + 1, 0.0);
+    BICG_CUDA(cudaMemcpy(c.last_hist.data(), out.hist, ((size_t)k + 1) * sizeof(double), cudaMemcpyDeviceToHost));
+    bicg_stats st{};
+    const double res = sqrt(out.dot_r / out.dot_zero);
+    st.iters = k;
+    st.converged = out.max_zeta_pi * out.max_zeta_pi * out.dot_r <= out.tol * out.tol * out.dot_zero;      // false after a NaN
+    st.final_res = res; st.loop_ms = ms;
+    st.kernel_launches = c.launches - launches0;
+    st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
+    c.last_stats = st;
+
+    if (c.rank == 0 && !c.cfg.quiet) {                                                // :339-346 / :882-889
+        const double t = ms * 1e-3;
+        printf("Total iter   : %d\n", k);
+        printf("Final r      : %e\n", res);
+        printf("Total time   : %e [sec.] \n", t);
+        printf("Avg time/iter: %e [sec.] \n", t / k);
+        fflush(stdout);
+    }
+
+    for (void *p : {(void *)h.sigma, (void *)h.eta, (void *)h.zeta, (void *)h.pi_old, (void *)h.pi_new, (void *)h.coef,
+                    (void *)h.hist, (void *)d_sd, (void *)d_x, (void *)d_p})
+        c.dev_free(p);
+    return k;                                                                         // :352 / :894
+}
+
+} // namespace bicg
