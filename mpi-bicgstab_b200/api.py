@@ -320,6 +320,15 @@ class DeviceMatrix:
         """CTAs of the last persistent-kernel launch that kept their matrix slice in shared memory (BICG_RESIDENT)."""
         return int(lib.bicg_debug_resident_ctas(self.h))
 
+    def coded_ctas(self):
+        """CTAs of the last persistent-kernel launch that streamed 16-bit column codes instead of 32-bit columns."""
+        return int(lib.bicg_debug_coded_ctas(self.h))
+
+    def stream_codes(self, on):
+        """Test hook: on=False makes later persistent-kernel launches on this handle stream 32-bit columns everywhere
+        (the results are bit-identical); returns the previous setting."""
+        return bool(lib.bicg_debug_stream_codes(self.h, 1 if on else 0))
+
     def spmv_time(self, reps=20):
         ms, by = C.c_double(), C.c_double()
         lib.bicg_spmv_time(self.h, reps, C.byref(ms), C.byref(by))

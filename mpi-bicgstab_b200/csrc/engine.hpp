@@ -151,6 +151,8 @@ struct MegaPlan {
     unsigned *d_tile_nz = nullptr;
     int *d_cta_tile = nullptr;
     int4 *d_cta_dep = nullptr;
+    unsigned short *d_col16 = nullptr;   // nnz + 16: 16-bit column codes of the CTAs whose column window fits them (mega.cu)
+    bool stream_codes = true;    // streaming CTAs use d_col16 where they can (false: 32-bit columns; bicg_debug_stream_codes)
     int *d_tile_flag = nullptr;  // only when rows longer than a stage were cut into chunk tiles
     bool chunked = false;
     std::vector<int> cta_row;    // grid + 1: first row of every CTA

@@ -433,14 +433,26 @@ static void choose_spmv_plan(bicg_matrix *m, const unsigned *h_ptr)
     }
     if (cands.empty()) { if (!fixed(m->plan)) fatal("bicgstab_b200: no feasible SpMV configuration"); return; }
 
-    int best = -1;
+    int fastest = -1;
     for (size_t i = 0; i < cands.size(); ++i) {
         cands[i].ms = time_plan(m, cands[i], 5);
         if (cfg.verbose)
             fprintf(stderr, "[bicg autotune r%d] kind=%d lanes=%2d threads=%3d stages=%d ctas=%d cap=%5d grid=%4d smem=%6zu : %.4f ms\n",
                     m->rank, cands[i].kind, cands[i].lanes, cands[i].threads, cands[i].stages, cands[i].ctas_per_sm,
                     cands[i].cap, cands[i].grid, cands[i].smem, cands[i].ms);
-        if (best < 0 || cands[i].ms < cands[best].ms) best = (int)i;
+        if (fastest < 0 || cands[i].ms < cands[fastest].ms) fastest = (int)i;
+    }
+    // The lanes per row decide how a row's sum is associated (lane l adds entries l, l + LANES, ... in order, then a fixed
+    // butterfly), so they decide the bits of y; the kind, threads, stages and CTAs per SM do not.  Candidates within 3 % of
+    // the fastest are a tie that run-to-run timing noise would otherwise settle -- T': TMA with 1 and 2 lanes, 0.1138 and
+    // 0.1136 ms on an H100 80GB HBM3 at 700 W -- and y would change from run to run.  A tie goes to the most lanes (the
+    // shortest serial chain per thread), and among those to the fastest candidate.
+    const double tie = cands[(size_t)fastest].ms * 1.03;
+    int best = -1;
+    for (size_t i = 0; i < cands.size(); ++i) {
+        if (cands[i].ms > tie) continue;
+        if (best < 0 || cands[i].lanes > cands[best].lanes ||
+            (cands[i].lanes == cands[best].lanes && cands[i].ms < cands[best].ms)) best = (int)i;
     }
     for (size_t i = 0; i < cands.size(); ++i)
         if ((int)i != best) free_plan(cands[i]);
@@ -483,11 +495,12 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
         std::vector<int> tile_row, cta_tile, tile_flag;
         std::vector<unsigned> tile_nz;
         // a stage must hold one tile; at least two stages must fit.  Tiles (or single rows) with more entries than that
-        // are cut by the planner: greedy tiles + chunked long rows (plan.cpp)
-        const int cap_limit = (int)(((SMEM_MAX / 2 - (long long)(rpt + 8) * 4) / 12) / 32 * 32) - 64;   // cap = roundup(max + 8, 32) must still fit twice
+        // are cut by the planner: greedy tiles + chunked long rows (plan.cpp).  The producer loads a tile's entries from a
+        // window aligned to 8 entries at both ends (16-byte bulk copies of 2-byte column codes): up to 14 more than the tile.
+        const int cap_limit = (int)(((SMEM_MAX / 2 - (long long)(rpt + 8) * 4) / 12) / 32 * 32) - 64;   // cap = roundup(max + 16, 32) must still fit twice
         const unsigned max_tile_nnz = plan_cta_tiles(h_ptr, m->n_loc, G, rpt, row_extra.empty() ? nullptr : row_extra.data(),
                                                      c.cfg.boundary_weight, tile_row, cta_tile, cap_limit, &tile_nz, &tile_flag, c.cfg.row_weight);
-        const int cap = round_up((long long)max_tile_nnz + 8, 32);
+        const int cap = round_up((long long)max_tile_nnz + 16, 32);
         const long long stage = (long long)cap * 12 + (long long)(rpt + 8) * 4;
         int stages = (int)std::min<long long>(4, SMEM_MAX / stage);
         if (stages < 2) continue;                       // cannot happen with the cap-limited plan; kept as a guard
@@ -523,6 +536,12 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
         BICG_CUDA(cudaMemcpy(mp.d_tile_nz, tile_nz.data(), tile_nz.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
         BICG_CUDA(cudaMemcpy(mp.d_cta_tile, cta_tile.data(), cta_tile.size() * sizeof(int), cudaMemcpyHostToDevice));
         launch_mega_dep(m->d_col, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, G, m->ghost_off, mp.d_cta_dep, c.stream);   // behind the upload
+        BICG_CUDA(cudaGetLastError());
+        // 16-bit column codes (streamed by the CTAs whose column window fits them, copied by resident CTAs), padded like d_col
+        const size_t pad = 16;
+        mp.d_col16 = (unsigned short *)c.dev_alloc((m->nnz + pad) * sizeof(unsigned short));
+        BICG_CUDA(cudaMemsetAsync(mp.d_col16 + m->nnz, 0, pad * sizeof(unsigned short), c.stream));
+        launch_mega_code(m->d_col, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, G, m->ghost_off, mp.d_cta_dep, mp.d_col16, c.stream);
         BICG_CUDA(cudaGetLastError());
         mp.ok = true;
         if (c.cfg.verbose)
@@ -863,7 +882,7 @@ void matrix_destroy(bicg_matrix *m)
     free_plan(m->plan);
     c.dev_free(m->d_trace);
     c.dev_free(m->mega.d_tile_row); c.dev_free(m->mega.d_tile_nz); c.dev_free(m->mega.d_cta_tile); c.dev_free(m->mega.d_cta_dep);
-    c.dev_free(m->mega.d_tile_flag);
+    c.dev_free(m->mega.d_col16); c.dev_free(m->mega.d_tile_flag);
     if (m->hist_extra) cudaFree(m->hist_extra);
     c.dev_free(m->d_val); c.dev_free(m->d_col); c.dev_free(m->d_ptr);
     if (m->world > 1) c.arena_pool.emplace(m->arena_bytes, Context::ArenaRec{m->arena, m->arena_bytes, m->arena_id, m->arena_handle});

@@ -115,15 +115,42 @@ struct MegaShared {
     volatile int flags[4];                    // [1] producer stop, [2] consumed visits, [3] a wait timed out
 };
 
+// Column window of a CTA (mega_dep_kernel: the own columns [dep.x, dep.y] and the ghost slots [dep.z, dep.w] its rows
+// reference).  When both spans together fit 16 bits, every column of the CTA has a 16-bit code: own column c -> c - obase
+// (codes < ospan), ghost column c -> c - gbase (codes >= ospan).  The one place that decides this: the code kernel, the
+// resident loader, the producer thread and the consumer threads all call it with the same dep, so a CTA's choice is the
+// same everywhere.
+struct ColWindow { bool ok; unsigned ospan; int obase, gbase; };
+__device__ __forceinline__ ColWindow col_window(int4 dep, int ghost_off)
+{
+    ColWindow w;
+    const bool own = dep.x <= dep.y, gh = dep.z <= dep.w;
+    w.ospan = own ? (unsigned)(dep.y - dep.x + 1) : 0u;
+    const unsigned gspan = gh ? (unsigned)(dep.w - dep.z + 1) : 0u;
+    w.ok = w.ospan + gspan <= 65536u;
+    w.obase = own ? dep.x : 0;
+    w.gbase = ghost_off + (gh ? dep.z : 0) - (int)w.ospan;
+    return w;
+}
+__device__ __forceinline__ unsigned short col_encode(const ColWindow &w, int ghost_off, unsigned c)
+{
+    return (unsigned short)((int)c < ghost_off ? (int)c - w.obase : (int)c - w.gbase);
+}
+__device__ __forceinline__ unsigned col_decode(const ColWindow &w, unsigned code)
+{
+    return code + (unsigned)(code < w.ospan ? w.obase : w.gbase);
+}
+
 // Resident mode (MegaArgs::resident; strong scaling, e.g. T' over 8 GPUs x 132 CTAs = 21 k entries per CTA): a CTA whose whole
-// slice fits into its shared memory -- 8-byte values, columns as 16-bit offsets into the CTA's own / ghost column windows
-// (mega_dep_kernel), row pointers -- loads it ONCE per solve; its SpMV phases then touch neither L2 nor the TMA ring for
-// the matrix.  Decided per CTA, identically by the producer thread and by every consumer thread.
-struct ResidentPlan { bool on; int row_lo, rows; unsigned nz_lo, nnz, ospan; int obase, gbase; };
+// slice fits into its shared memory -- 8-byte values, the 16-bit column codes, row pointers -- loads it ONCE per solve; its
+// SpMV phases then touch neither L2 nor the TMA ring for the matrix.  Decided per CTA, identically by the producer thread
+// and by every consumer thread.
+struct ResidentPlan { bool on; int row_lo, rows; unsigned nz_lo, nnz; ColWindow w; };
 __device__ __forceinline__ ResidentPlan resident_plan(const MegaArgs &a, int t0, int t1, int lanes)
 {
     ResidentPlan p;
-    p.on = false; p.row_lo = 0; p.rows = 0; p.nz_lo = 0u; p.nnz = 0u; p.ospan = 0u; p.obase = 0; p.gbase = 0;
+    p.on = false; p.row_lo = 0; p.rows = 0; p.nz_lo = 0u; p.nnz = 0u;
+    p.w = col_window(a.cta_dep[blockIdx.x], a.ghost_off);
     if (!a.resident || lanes != 1 || t1 <= t0 || a.tile_flag != nullptr) return p;
     p.row_lo = a.tile_row[t0];
     p.rows = a.tile_row[t1] - p.row_lo;
@@ -131,15 +158,13 @@ __device__ __forceinline__ ResidentPlan resident_plan(const MegaArgs &a, int t0,
     p.nz_lo = a.ptr[p.row_lo];
     p.nnz = a.ptr[p.row_lo + p.rows] - p.nz_lo;
     if (mega_resident_bytes(p.nnz, p.rows) > (size_t)a.smem_bytes) return p;
-    const int4 dep = a.cta_dep[blockIdx.x];
-    const bool own = dep.x <= dep.y, gh = dep.z <= dep.w;
-    p.ospan = own ? (unsigned)(dep.y - dep.x + 1) : 0u;
-    const unsigned gspan = gh ? (unsigned)(dep.w - dep.z + 1) : 0u;
-    if (p.ospan + gspan > 65536u) return p;             // the columns of this CTA do not fit 16-bit offsets: it streams
-    p.obase = own ? dep.x : 0;
-    p.gbase = a.ghost_off + (gh ? dep.z : 0) - (int)p.ospan;   // column = gbase + code for codes >= ospan
-    p.on = true;
+    p.on = p.w.ok;                                      // columns that do not fit 16-bit codes: the CTA streams
     return p;
+}
+// a streaming CTA (not resident, owns tiles) streams the 16-bit codes instead of the 32-bit columns when its window fits
+__device__ __forceinline__ bool streams_codes(const MegaArgs &a, const ResidentPlan &rp, int my_tiles)
+{
+    return a.stream_codes && a.col16 != nullptr && my_tiles > 0 && !rp.on && rp.w.ok;
 }
 
 template <int CT, int LANES>
@@ -165,6 +190,7 @@ struct Mega {
     size_t stage_bytes;
     int trace_it, trace_who;
     bool resident;                // this CTA keeps its matrix slice in shared memory (ResidentPlan)
+    bool coded;                   // this CTA streams 16-bit column codes (streams_codes)
     ResidentPlan rp;
     const double *rs_val; const unsigned short *rs_col; const unsigned *rs_ptr;
 
@@ -418,7 +444,11 @@ struct Mega {
                 return;
             }
         }
-        if (a.gather_cg) spmv_impl<EPI, true>(x, y, dot); else spmv_impl<EPI, false>(x, y, dot);
+        if (coded) {
+            if (a.gather_cg) spmv_impl<EPI, true, true>(x, y, dot); else spmv_impl<EPI, false, true>(x, y, dot);
+        } else {
+            if (a.gather_cg) spmv_impl<EPI, true, false>(x, y, dot); else spmv_impl<EPI, false, false>(x, y, dot);
+        }
     }
     // one row's epilogue: y and the dots fused into the SpMV (same operations, same order as the streaming path)
     template <int EPI>
@@ -440,8 +470,8 @@ struct Mega {
     __device__ void spmv_res(const double *x, double *y, double (&dot)[4])
     {
         constexpr int U = 16;
-        const double *xo = x + rp.obase, *xg = x + rp.gbase;
-        const unsigned ospan = rp.ospan;
+        const double *xo = x + rp.w.obase, *xg = x + rp.w.gbase;
+        const unsigned ospan = rp.w.ospan;
         const int rows = rp.rows;
         const bool empty = rp.nnz == 0u;                      // a slice of empty rows: y = 0, the dots see acc = 0
         const unsigned last = empty ? 0u : rp.nnz - 1u;
@@ -473,11 +503,14 @@ struct Mega {
         }
     }
 
-    template <int EPI, bool CG>
+    // CODED: the stage's column area holds the CTA's 16-bit column codes (its first half; the stage layout is the same for
+    // both formats), each turned back into the column with one select and one add before its gather
+    template <int EPI, bool CG, bool CODED>
     __device__ void spmv_impl(const double *x, double *y, double (&dot)[4])
     {
         const int stages = a.stages, cap = a.cap;
         const int sub = tid % LANES, row_in_tile = tid / LANES;
+        const ColWindow w = rp.w;
         double carry = 0.0;
         for (int lt = 0; lt < my_tiles; ++lt, ++vis) {
             const int s = (int)(vis % (unsigned)stages);
@@ -485,7 +518,9 @@ struct Mega {
             const unsigned char *st = dyn + (size_t)s * stage_bytes;
             const double   *sval = reinterpret_cast<const double *>(st);
             const unsigned *scol = reinterpret_cast<const unsigned *>(sval + cap);
+            const unsigned short *scode = reinterpret_cast<const unsigned short *>(scol);
             const unsigned *sptr = scol + cap;
+            auto column = [&](unsigned idx) { return CODED ? col_decode(w, scode[idx]) : scol[idx]; };
             const StageHdr h = sh.hdr[s];
             if (h.flag != 0) {
                 // one chunk of a row longer than a stage: the whole CTA multiplies it, the row's partial sum is carried
@@ -496,7 +531,8 @@ struct Mega {
 #pragma unroll
                     for (int u = 0; u < 4; ++u) {
                         const unsigned idx = min(jj + (unsigned)(u * CT), h.hi - 1u);
-                        pv[u] = sval[idx]; px[u] = CG ? ld_l2(x + scol[idx]) : ld_coherent(x + scol[idx]);
+                        const double *src = x + column(idx);
+                        pv[u] = sval[idx]; px[u] = CG ? ld_l2(src) : ld_coherent(src);
                     }
 #pragma unroll
                     for (int u = 0; u < 4; ++u)
@@ -545,7 +581,7 @@ struct Mega {
 #pragma unroll
                 for (int u = 0; u < UNR; ++u) {
                     const int idx = min(j + u * LANES, e - 1);
-                    c[u] = scol[idx];
+                    c[u] = column((unsigned)idx);
                     v[u] = sval[idx];
                 }
 #pragma unroll
@@ -882,10 +918,16 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
 
     if (tid >= CT) {
         // ============================ producer warp: streams this CTA's tiles round and round ==============
-        if (tid == CT && my_tiles > 0 && !resident_plan(a, t0, t1, LANES).on) {
+        const ResidentPlan rp = tid == CT ? resident_plan(a, t0, t1, LANES) : ResidentPlan{};
+        if (tid == CT && my_tiles > 0 && !rp.on) {
             volatile int *flags = sh.flags;
             const unsigned long long pol = l2_evict_first_policy();
             const bool hint = a.l2_hint != 0;
+            // 16-bit codes: 2 bytes per entry; a bulk copy moves whole 16-byte units, so the entry window of a tile is
+            // aligned to 8 entries (4 suffice for 4-byte columns); the plan's stage capacity covers the wider window
+            const bool coded = streams_codes(a, rp, my_tiles);
+            const unsigned al = coded ? 7u : 3u, cbytes = coded ? 2u : 4u;
+            const void *cols = coded ? (const void *)a.col16 : (const void *)a.col;
             unsigned v = 0;
             bool stop = false;
             for (;; ++v) {
@@ -900,7 +942,7 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
                 const int t = t0 + (int)(v % (unsigned)my_tiles);
                 const int row0 = a.tile_row[t], row1 = a.tile_row[t + 1];
                 const unsigned p0 = a.tile_nz[t], p1 = a.tile_nz[t + 1];
-                const unsigned a0 = p0 & ~3u, cnt = ((p1 + 3u) & ~3u) - a0;
+                const unsigned a0 = p0 & ~al, cnt = ((p1 + al) & ~al) - a0;
                 const int rowa = row0 & ~3, cntp = ((row1 + 1 + 3) & ~3) - rowa;
                 unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
                 double   *sval = reinterpret_cast<double *>(st);
@@ -908,14 +950,15 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
                 unsigned *sptr = scol + cap;
                 sh.hdr[s] = StageHdr{row0, row1, a0, rowa, p0 - a0, p1 - a0, a.tile_flag ? a.tile_flag[t] : 0, 0};
                 const unsigned bar = smem_u32(&sh.full_bar[s]);
-                mbar_arrive_expect_tx(bar, cnt * 12u + (unsigned)cntp * 4u);
+                mbar_arrive_expect_tx(bar, cnt * (8u + cbytes) + (unsigned)cntp * 4u);
                 if (cnt) {
+                    const void *csrc = (const char *)cols + (size_t)a0 * cbytes;
                     if (hint) {
                         tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
-                        tma_load_1d_hint(smem_u32(scol), a.col + a0, cnt * 4u, bar, pol);
+                        tma_load_1d_hint(smem_u32(scol), csrc, cnt * cbytes, bar, pol);
                     } else {
                         tma_load_1d(smem_u32(sval), a.val + a0, cnt * 8u, bar);
-                        tma_load_1d(smem_u32(scol), a.col + a0, cnt * 4u, bar);
+                        tma_load_1d(smem_u32(scol), csrc, cnt * cbytes, bar);
                     }
                 }
                 tma_load_1d(smem_u32(sptr), a.ptr + rowa, (unsigned)cntp * 4u, bar);
@@ -972,21 +1015,21 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
         // resident mode: the slice goes into shared memory once (plain coalesced loads; the ring is not used by this CTA)
         m.rp = resident_plan(a, t0, t1, LANES);
         m.resident = m.rp.on;
+        m.coded = streams_codes(a, m.rp, my_tiles);
         if (m.resident) {
             const size_t nnzp = ((size_t)m.rp.nnz + 7u) & ~(size_t)7u;
             double *sv = reinterpret_cast<double *>(dyn_smem);
             unsigned short *sc16 = reinterpret_cast<unsigned short *>(sv + nnzp);
             unsigned *sp = reinterpret_cast<unsigned *>(sc16 + nnzp);
-            const int gh0 = a.ghost_off + (dep.z <= dep.w ? dep.z : 0);
             for (unsigned i = (unsigned)tid; i < m.rp.nnz; i += (unsigned)CT) {
                 sv[i] = a.val[m.rp.nz_lo + i];
-                const int cc = (int)a.col[m.rp.nz_lo + i];
-                sc16[i] = (unsigned short)(cc < a.ghost_off ? cc - m.rp.obase : cc - gh0 + (int)m.rp.ospan);
+                sc16[i] = a.col16[m.rp.nz_lo + i];
             }
             for (int r = tid; r <= m.rp.rows; r += CT) sp[r] = a.ptr[m.rp.row_lo + r] - m.rp.nz_lo;
             m.rs_val = sv; m.rs_col = sc16; m.rs_ptr = sp;
             if (tid == 0) atomicAdd(&a.sync->st.resident_ctas, 1);
         }
+        if (m.coded && tid == 0) atomicAdd(&a.sync->st.coded_ctas, 1);
         nbar(1, CT);
         if (a.comm.world > 1 && (m.reads_ghost || m.gs_hi > m.gs_lo)) {
             // the vectors the first phases read were pushed by the init kernels (kernel-per-phase protocol)
@@ -1031,6 +1074,20 @@ __global__ void __launch_bounds__(256) mega_dep_kernel(const unsigned *__restric
     atomicMin(&s[0], omin); atomicMax(&s[1], omax); atomicMin(&s[2], gmin); atomicMax(&s[3], gmax);
     __syncthreads();
     if (threadIdx.x == 0) dep[blockIdx.x] = make_int4(s[0], s[1], s[2], s[3]);
+}
+
+// the 16-bit column codes (col_encode) of every CTA whose column window fits them; the entries of the other CTAs are not
+// written (they stream, or keep resident, nothing but their 32-bit columns)
+__global__ void __launch_bounds__(256) mega_code_kernel(const unsigned *__restrict__ col, const unsigned *__restrict__ ptr,
+                                                        const int *__restrict__ tile_row, const int *__restrict__ cta_tile,
+                                                        int ghost_off, const int4 *__restrict__ dep, unsigned short *__restrict__ col16)
+{
+    const ColWindow w = col_window(dep[blockIdx.x], ghost_off);
+    if (!w.ok) return;
+    const int r0 = tile_row[cta_tile[blockIdx.x]], r1 = tile_row[cta_tile[blockIdx.x + 1]];
+    if (r1 <= r0) return;
+    const unsigned e0 = ptr[r0], e1 = ptr[r1];
+    for (unsigned j = e0 + threadIdx.x; j < e1; j += blockDim.x) col16[j] = col_encode(w, ghost_off, col[j]);
 }
 
 template <int CT, int LANES>
@@ -1090,6 +1147,12 @@ void launch_mega_dep(const unsigned *col, const unsigned *ptr, const int *tile_r
                      int ghost_off, int4 *dep, cudaStream_t st)
 {
     mega_dep_kernel<<<grid, 256, 0, st>>>(col, ptr, tile_row, cta_tile, ghost_off, dep);
+}
+
+void launch_mega_code(const unsigned *col, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
+                      int ghost_off, const int4 *dep, unsigned short *col16, cudaStream_t st)
+{
+    mega_code_kernel<<<grid, 256, 0, st>>>(col, ptr, tile_row, cta_tile, ghost_off, dep, col16);
 }
 
 } // namespace bicg

@@ -21,6 +21,7 @@ struct alignas(128) MegaState {
     unsigned long long halo_epoch;      // last halo exchange signalled
     int plan_ok[MAX_RANKS];             // written by rank p at plan time: its persistent-kernel plan is usable
     int resident_ctas;                  // CTAs of the last launch that kept their matrix slice in shared memory (test / trace aid)
+    int coded_ctas;                     // CTAs of the last launch that streamed 16-bit column codes (test / trace aid)
 };
 
 // Lives in the IPC-shared arena: `mail` and `st.plan_ok` are written by the peers.
@@ -55,6 +56,8 @@ struct MegaArgs {
     const int4 *cta_dep;        // [grid]: min / max own column, min / max ghost slot referenced by the CTA's rows
     const double   *val;
     const unsigned *col;
+    const unsigned short *col16;   // per entry: 16-bit code of the column in its CTA's column window (mega_code_kernel),
+                                   // filled for the CTAs whose window fits 16 bits; what the resident load copies
     const unsigned *ptr;
     const int      *tile_row;   // ntiles + 1
     const unsigned *tile_nz;    // ntiles + 1
@@ -67,6 +70,8 @@ struct MegaArgs {
     int resident;               // 1: a CTA whose whole matrix slice fits into its shared memory (strong scaling: 8 GPUs x one CTA per SM)
                                 //    loads it ONCE per solve (values + 16-bit CTA-relative columns + row pointers) instead of streaming it
                                 //    through the TMA ring in every SpMV
+    int stream_codes;           // 1: a streaming CTA whose column window fits 16 bits streams col16 (10 bytes per entry
+                                //    instead of 12); 0: every streaming CTA streams the 32-bit columns
     int smem_bytes;             // dynamic shared memory of this launch
     double *vec_base; long long vstride;   // arena vectors: vec(id) = vec_base + id * vstride
     VecPtrs v;
@@ -93,5 +98,8 @@ __host__ __device__ inline size_t mega_resident_bytes(unsigned nnz, int rows)
 // per-CTA column ranges of the plan (one launch at plan time)
 void   launch_mega_dep(const unsigned *col, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
                        int ghost_off, int4 *dep, cudaStream_t st);
+// 16-bit column codes of the CTAs whose column window fits them (one launch at plan time, behind launch_mega_dep)
+void   launch_mega_code(const unsigned *col, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
+                        int ghost_off, const int4 *dep, unsigned short *col16, cudaStream_t st);
 
 } // namespace bicg

@@ -88,7 +88,8 @@ struct Seq {
         a.sc = m->d_sc; a.hist = m->d_hist; a.comm = m->comm; a.sync = m->d_msync;
         for (int p = 0; p < MAX_RANKS; ++p) a.peer_mail[p] = &m->peer_msync[p]->mail[0][0];
         a.n_ghost = m->n_ghost; a.cta_dep = m->mega.d_cta_dep;
-        a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr;
+        a.val = m->d_val; a.col = m->d_col; a.col16 = m->mega.d_col16; a.ptr = m->d_ptr;
+        a.stream_codes = m->mega.stream_codes ? 1 : 0;
         a.tile_row = m->mega.d_tile_row; a.tile_nz = m->mega.d_tile_nz; a.cta_tile = m->mega.d_cta_tile;
         a.tile_flag = m->mega.d_tile_flag;
         a.cap = m->mega.cap; a.stages = m->mega.stages;
@@ -115,6 +116,7 @@ struct Seq {
         a.snap = m->d_trace ? m->d_trace + (size_t)2 * MEGA_TRACE_ITERS * MEGA_TRACE_SLOTS : nullptr;
         a.snap_iter = 50;
         BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.resident_ctas, 0, sizeof(int), c.stream));
+        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.coded_ctas, 0, sizeof(int), c.stream));
         int rc = launch_mega(m->mega.threads, m->mega.lanes, m->mega.grid, smem, a, c.stream);
         if (rc) {
             // e.g. the grid cannot be co-resident because something else holds SMs.  Single rank: not an error, the
@@ -614,6 +616,24 @@ extern "C" int bicg_debug_resident_ctas(bicg_matrix *m)
     BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.resident_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
     return n;
+}
+
+extern "C" int bicg_debug_coded_ctas(bicg_matrix *m)
+{
+    using namespace bicg;
+    Context &c = ctx();
+    c.ensure();
+    int n = 0;
+    BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.coded_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    return n;
+}
+
+extern "C" int bicg_debug_stream_codes(bicg_matrix *m, int on)
+{
+    const int was = m->mega.stream_codes ? 1 : 0;
+    m->mega.stream_codes = on != 0;
+    return was;
 }
 
 // ------------------------------------------------------------------------------------------------
