@@ -10,6 +10,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
+from loop_reference import reference_state
+
 pytestmark = pytest.mark.gpu
 
 V = dict(x=0, r=1, rh=2, p=3, s=4, y=5, z=5, w=6, v=7, t=8, b=9, ax=10)
@@ -131,36 +133,12 @@ def test_spmv_epilogue_dots(B, O, epi, kind, g, p0):
 
 
 def _one_iteration_reference(O, method, n, ptr, col, val, b):
-    """One pass of the reference loop with the oracle's primitives; returns the vectors and scalars it leaves."""
-    A = lambda x: O.spmv(n, ptr, col, val, x)
-    ax, sc, dot = O.daxpy, O.dscal, O.ddot
-    x = np.zeros(n); r = b.copy()
-    Ax = A(x); ax(-1.0, Ax, r); rh = r.copy()
-    if method == "bicgstab":                                          # solver.c:74-120
-        p = r.copy(); rTr = dot(r, r)
-        s = A(p); alpha = rTr / dot(rh, s); ax(-alpha, s, r)
-        y = A(r); omega = dot(r, y) / dot(y, y)
-        ax(alpha, p, x); ax(omega, r, x); ax(-omega, y, r)
-        dot_r, rTr_new = dot(r, r), dot(rh, r)
-        beta = (alpha / omega) * (rTr_new / rTr)
-        sc(beta, p); ax(1.0, r, p); ax(-beta * omega, s, p)
-        # p is not compared: the library evaluates the loop test of solver.c:86 right after beta, so on the LAST iteration it
-        # skips the p update whose result the reference computes and then discards
-        return dict(x=x, r=r, s=s, y=y), dict(alpha=alpha, omega=omega, beta=beta, dot_r=dot_r)
-    # ca_bicgstab solver.c:200-253 (pipe_bicgstab produces the same quantities in exact arithmetic, different roundings)
-    rTr = dot(r, r); w = A(r); alpha = rTr / dot(r, w); beta = 0.0; omega = 0.0
-    p = np.zeros(n); s = np.zeros(n); z = np.zeros(n)
-    ax(-omega, s, p); sc(beta, p); ax(1.0, r, p)
-    ax(-omega, z, s); sc(beta, s); ax(1.0, w, s)
-    z = A(s); ax(-alpha, s, r); ax(-alpha, z, w)
-    omega = dot(r, w) / dot(w, w)
-    ax(alpha, p, x); ax(omega, r, x); ax(-omega, w, r)
-    dot_r = dot(r, r)
-    w = A(r)
-    rTr_new, rTw, rTs, rTz = dot(rh, r), dot(rh, w), dot(rh, s), dot(rh, z)
-    beta = (alpha / omega) * (rTr_new / rTr)
-    alpha2 = rTr_new / (rTw + beta * (rTs - omega * rTz))
-    return dict(x=x, r=r, p=p, s=s, z=z, w=w), dict(alpha=alpha2, omega=omega, beta=beta, dot_r=dot_r)
+    """One pass of the reference loop (tests/loop_reference.py); returns the vectors and scalars it leaves.  p of bicgstab is
+    the direction the pass used: the library evaluates the loop test of solver.c:86 right after beta and skips the p update
+    whose result the reference computes and then discards."""
+    st = reference_state(O, method, ptr, col, val, b, 1)
+    names = ("x", "r", "p", "s", "y") if method == "bicgstab" else ("x", "r", "p", "s", "z", "w")
+    return {k: st[k] for k in names}, {k: st[k] for k in ("alpha", "omega", "beta", "dot_r")}
 
 
 @pytest.mark.parametrize("mega", [1, 0], ids=["mega", "multikernel"])
