@@ -83,6 +83,13 @@ int shifted_lopbicg_switching(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, IN
  * identical arithmetic, so the same function here. */
 int shifted_lopbicg_switching_noovlp(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set,
                                      double *r_loc, double *sigma, int sigma_len, int seed);
+/* shifted_switching_solver.h:11 (shifted_switching_solver.c:20-257): the fixed-seed variant the shifted drivers name as the
+ * alternative to the switching call (main_shifted.c:125, main_repeat.c:129, main_seed_diff.c:133).  Same arguments; until the seed
+ * converges it is the switching solve line for line.  The seed never switches: when it converges first it is counted as stopped
+ * but keeps iterating, since the other shifts still advance from its Krylov data, until every shift has stopped or MAX_ITER.
+ * Returns k, the iterations performed (not k + 1), and prints only the `Total time` / `Avg time/iter` lines (:241-242). */
+int shifted_lopbicg(CSR_Matrix *A_loc_diag, CSR_Matrix *A_loc_offd, INFO_Matrix *A_info, double *x_loc_set, double *r_loc,
+                    double *sigma, int sigma_len, int seed);
 
 /* shifted_solver.h:17-21 (shifted_solver.c:182-1085): the LOP shifted BiCGStab family for (A + sigma_j I) x_j = b.  Same arguments as
  * shifted_lopbicg_switching, but the seed never changes and every shift is advanced until max_j |1/(zeta_j pi_j)|^2 (r,r) <=
@@ -177,13 +184,15 @@ int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nr
                bicg_stats *stats);
 
 /* shifted_lopbicg_switching on a resident matrix; bicg_last_shift_info: the seed the last shifted solve ended with and the
- * iteration at which every shift stopped (returns sigma_len). */
+ * iteration at which every shift stopped (returns sigma_len).  The stop iteration is 1-based (the iteration after whose
+ * convergence test the shift stopped), 0 for a shift that never stopped; for shifted_lopbicg the seed is the one passed in. */
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats);
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap);
 /* Any shifted solver on a resident matrix: BICG_SHIFTED_SWITCHING = shifted_lopbicg_switching (returns iterations + 1, like
- * bicg_shifted_solve), BICG_SHIFTED_LOP = shifted_lopbicgstab, BICG_SHIFTED_PIPE_LOP = shifted_pipe_lopbicgstab (both return the
- * iterations performed).  -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len). */
-enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP = 2 };
+ * bicg_shifted_solve), BICG_SHIFTED_LOP = shifted_lopbicgstab, BICG_SHIFTED_PIPE_LOP = shifted_pipe_lopbicgstab,
+ * BICG_SHIFTED_LOPBICG = shifted_lopbicg (these three return the iterations performed).  -1 for an unknown method,
+ * sigma_len <= 0 or seed outside [0, sigma_len). */
+enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP = 2, BICG_SHIFTED_LOPBICG = 3 };
 int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
                           bicg_stats *stats);
 

@@ -47,6 +47,7 @@ SYMBOLS = {
     "pipe_bicgstab_rr": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicg_switching": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicg_switching_noovlp": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
+    "shifted_lopbicg": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicgstab": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicgstab_v2": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),
     "shifted_lopbicgstab_nooverlap": (C.c_int, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]),

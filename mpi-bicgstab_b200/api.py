@@ -17,6 +17,8 @@ from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_stats, lib
 
 METHODS = {"bicgstab": 0, "ca_bicgstab": 1, "pipe_bicgstab": 2, "pipe_bicgstab_rr": 3}
 SHIFTED_METHODS = {"shifted_lopbicg_switching": 0, "shifted_lopbicgstab": 1, "shifted_pipe_lopbicgstab": 2}
+# every method bicg_shifted_solve_ex accepts: SHIFTED_METHODS plus the fixed-seed shifted_lopbicg
+SHIFTED_SOLVE_EX = dict(SHIFTED_METHODS, shifted_lopbicg=3)
 GEN_KINDS = {"stencil15": 0, "laplace5": 1, "random": 2, "convdiff": 3}
 
 
@@ -241,6 +243,13 @@ def _shifted_args(blk, x_set, r_loc, sigma):
     return _dptr(x_set), _vec(r_loc, blk.n_loc), sigma
 
 
+def shifted_lopbicg(blk, x_set, r_loc, sigma, seed):
+    """shifted_switching_solver.h:11, the fixed-seed variant of shifted_lopbicg_switching (same arguments).  Returns the
+    iterations performed (not + 1)."""
+    xp, rp, sigma = _shifted_args(blk, x_set, r_loc, sigma)
+    return lib.shifted_lopbicg(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info), xp, rp, _dptr(sigma), int(sigma.size), int(seed))
+
+
 def shifted_lopbicgstab(blk, x_set, r_loc, sigma, seed):
     """shifted_solver.h:17 (LOP; its _v2 / _nooverlap twins are the same solve).  x_set: (sigma_len, n_loc) C-contiguous;
     returns the iterations performed."""
@@ -305,10 +314,10 @@ class DeviceMatrix:
         return it, _stats_dict(st)
 
     def shifted_solve(self, method, x_set, r, sigma, seed):
-        """bicg_shifted_solve_ex: method is a key of SHIFTED_METHODS; returns (that solver's return value, stats)."""
+        """bicg_shifted_solve_ex: method is a key of SHIFTED_SOLVE_EX; returns (that solver's return value, stats)."""
         xp, rp, sigma = _shifted_args(self.blk, x_set, r, sigma)
         st = bicg_stats()
-        k = lib.bicg_shifted_solve_ex(self.h, SHIFTED_METHODS[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
+        k = lib.bicg_shifted_solve_ex(self.h, SHIFTED_SOLVE_EX[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
         return k, _stats_dict(st)
 
     def spmv(self, x_loc):

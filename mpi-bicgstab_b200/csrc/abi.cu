@@ -18,6 +18,22 @@ static_assert(offsetof(INFO_Matrix, code) == 12 && offsetof(INFO_Matrix, recvcou
 
 namespace {
 
+// shifted_switching_solver.h entry points (fixed = 0: shifted_lopbicg_switching, 1: shifted_lopbicg)
+int run_shifted(int fixed, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+                int sigma_len, int seed)
+{
+    if (info->cols != info->rows) {                      // shifted_switching_solver.c:28-31, 268-271
+        printf("Error: matrix is not square.\n");
+        exit(1);
+    }
+    Context &c = ctx();
+    c.ensure();
+    bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
+    const int k = shifted_solve(m, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, fixed);
+    if (!c.cfg.cache) matrix_destroy(m);
+    return k;
+}
+
 // shifted_solver.h entry points of the LOP family (pipe = 0: LOP, 1: PIPE-LOP)
 int run_shifted_lop(int pipe, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                     int sigma_len, int seed)
@@ -87,16 +103,15 @@ int pipe_bicgstab_rr(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_
 int shifted_lopbicg_switching(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                               int sigma_len, int seed)
 {
-    if (info->cols != info->rows) {                      // shifted_switching_solver.c:268-271
-        printf("Error: matrix is not square.\n");
-        exit(1);
-    }
-    Context &c = ctx();
-    c.ensure();
-    bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
-    const int k = shifted_solve(m, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
-    if (!c.cfg.cache) matrix_destroy(m);
-    return k;
+    return run_shifted(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+}
+
+// shifted_switching_solver.h:11 -- the fixed-seed variant: same prototype and meaning, but the seed never switches (when it
+// converges first it keeps iterating until every shift has stopped) and the return value is k, the iterations performed.
+int shifted_lopbicg(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma, int sigma_len,
+                    int seed)
+{
+    return run_shifted(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 
 // shifted_switching_solver.c:611 -- the reference's twin of the function above with the halo exchange NOT overlapped with the
@@ -212,7 +227,7 @@ int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();
-    const int k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    const int k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, 0);
     if (stats) *stats = c.last_stats;
     return k;
 }
@@ -223,7 +238,10 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
     c.ensure();
     int k;
     switch (method) {
-    case BICG_SHIFTED_SWITCHING: k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter); break;
+    case BICG_SHIFTED_SWITCHING:
+    case BICG_SHIFTED_LOPBICG:
+        k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, method == BICG_SHIFTED_LOPBICG);
+        break;
     case BICG_SHIFTED_LOP:
     case BICG_SHIFTED_PIPE_LOP:
         k = shifted_lop_solve(m, method == BICG_SHIFTED_PIPE_LOP, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);

@@ -233,8 +233,10 @@ int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, i
 int  spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full_or_null);
 int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);
-// shifted.cu
-int  shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol, int max_iter);
+// shifted.cu (fixed = 0: shifted_lopbicg_switching, returns iterations + 1; 1: shifted_lopbicg, returns the iterations performed);
+// -1 for a bad sigma_len / seed
+int  shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol, int max_iter,
+                   int fixed);
 // shifted_lop.cu (pipe = 0: LOP, 1: PIPE-LOP); returns the iterations performed, -1 for a bad sigma_len / seed
 int  shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
                        int max_iter);

@@ -11,6 +11,12 @@
 //     p_j of every active shift are read and written exactly once -- 32 B per row and shift, the HBM floor of the method.
 // Element-wise operation order = the reference's call order with gcc's FMA contraction (y += a x -> fma(a, x, y)).
 // The host only enqueues batches of iterations and polls a done flag (as solve.cu does).
+//
+// The same solve also runs shifted_lopbicg (shifted_switching_solver.c:20-257; prototype :11), the fixed-seed variant: until the
+// seed converges its arithmetic is the switching solver's line for line.  With ShiftDev::fixed set, sh_scalar_iter skips the
+// seed switch, so a seed that converges first is counted as stopped but its BiCGStab keeps running (the other shifts still
+// advance from its Krylov data) until every shift has stopped or MAX_ITER.  It returns the iterations performed, not + 1,
+// and prints only the two MEASURE_TIME lines (:241-242).
 #include "engine.hpp"
 #include "shifted_run.cuh"
 
@@ -27,6 +33,7 @@ constexpr int SH_EVENTS = 16;       // seed switches remembered for the referenc
 
 struct ShiftDev {
     int L, max_iter;                // sigma_len, MAX_ITER + 1                                    (:291-293)
+    int fixed;                      // 1: shifted_lopbicg, the seed never switches               (:20-257)
     double tol;                     // EPS                                                       (:292)
     int seed, k, stop_count, done, live, switched, max_sigma, n_active, n_events;
     double rTr, rTs, qTq, qTy, dot_r, dot_zero, rTr_old, r_scale;
@@ -136,7 +143,7 @@ __global__ void __launch_bounds__(512) sh_scalar_iter(ShiftDev *sd, Scalars *sc)
         }
     }
     __syncthreads();
-    const bool sw = sd->stop_flag[seed] && sd->stop_count < L;                      // :490
+    const bool sw = !sd->fixed && sd->stop_flag[seed] && sd->stop_count < L;        // :490 (shifted_lopbicg: never)
     if (sw) {
         const int ms = sd->max_sigma;
         const double dsg = sg_s - sd->sigma[ms];
@@ -336,18 +343,19 @@ struct ShRun : ShiftLaunch {
 
 } // namespace
 
-int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter_opt)
+int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter_opt,
+                  int fixed)
 {
     Context &c = ctx();
     c.ensure();
     if (L <= 0 || seed < 0 || seed >= L) return -1;
     const int n = m->n_loc;
-    const int max_iter = max_iter_opt + 1;                                            // :293
+    const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
     const long long stride = ((long long)n + 15) / 16 * 16;
 
     // ---- device state -------------------------------------------------------------------------------------------------
     ShiftDev h{};
-    h.L = L; h.max_iter = max_iter; h.tol = tol; h.seed = seed;
+    h.L = L; h.max_iter = max_iter; h.fixed = fixed; h.tol = tol; h.seed = seed;
     auto dalloc = [&](size_t bytes) { return c.dev_alloc(std::max<size_t>(bytes, 16)); };
     h.sigma = (double *)dalloc(L * sizeof(double));
     h.alpha_set = (double *)dalloc(L * sizeof(double)); h.beta_set = (double *)dalloc(L * sizeof(double));
@@ -437,7 +445,13 @@ int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma,
     st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
     c.last_stats = st;
 
-    if (c.rank == 0 && !c.cfg.quiet) {
+    if (c.rank == 0 && !c.cfg.quiet && fixed) {
+        // shifted_lopbicg prints the MEASURE_TIME lines only, its average over the iterations performed (:241-242)
+        const double t = ms * 1e-3;
+        printf("Total time   : %e [sec.] \n", t);
+        printf("Avg time/iter: %e [sec.] \n", t / (double)(k - 1));
+        fflush(stdout);
+    } else if (c.rank == 0 && !c.cfg.quiet) {
         // what the reference prints: the seed switches (:518-526), then the MEASURE_TIME lines (:557-561)
         std::vector<int> ek(SH_EVENTS), es(SH_EVENTS), er(SH_EVENTS);
         std::vector<double> ev((size_t)SH_EVENTS * L * 3);
@@ -464,7 +478,7 @@ int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma,
                     (void *)h.pi_arch, (void *)h.coef, (void *)h.active, (void *)h.hist, (void *)h.ev_k, (void *)h.ev_seed,
                     (void *)h.ev_remain, (void *)h.ev_vals, (void *)d_sd, (void *)d_x, (void *)d_p})
         c.dev_free(p);
-    return k;                                                                         // :600
+    return fixed ? k - 1 : k;                                                         // :255 / :600
 }
 
 } // namespace bicg

@@ -1,15 +1,17 @@
 """Throughput of the shifted solvers on the T' matrix (1 GPU): iterations/s and effective GB/s on each method's algorithmic bytes
 per iteration (DESIGN.md section 3.4 / 3.5):
     switching  24 nnz + 32 n (active shifts) + 200 n (seed BiCGStab: two SpMVs + its vector phases)
+    fixed      the same (shifted_lopbicg runs the switching solver's kernels without the seed switch)
     lop        24 nnz + 32 n (L - 1) + 168 n
     pipe_lop   24 nnz + 32 n (L - 1) + 240 n
-usage: shifted_perf.py [--method switching|lop|pipe_lop] [L ...]   env: SP_G (grid size, default 117)"""
+usage: shifted_perf.py [--method switching|fixed|lop|pipe_lop] [L ...]   env: SP_G (grid size, default 117)"""
 import argparse, os, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import mpi_bicgstab_b200 as B
-METHODS = {"switching": "shifted_lopbicg_switching", "lop": "shifted_lopbicgstab", "pipe_lop": "shifted_pipe_lopbicgstab"}
+METHODS = {"switching": "shifted_lopbicg_switching", "fixed": "shifted_lopbicg", "lop": "shifted_lopbicgstab",
+           "pipe_lop": "shifted_pipe_lopbicgstab"}
 ap = argparse.ArgumentParser()
 ap.add_argument("--method", choices=sorted(METHODS), default="switching")
 ap.add_argument("L", nargs="*", type=int, default=[16, 64])
@@ -27,8 +29,8 @@ for L in args.L:
     for rep in range(2):
         x = np.zeros((L, n)); r = b.copy()
         k, st = dm.shifted_solve(METHODS[args.method], x, r, sigma, 0)
-    if args.method == "switching":
-        it = k - 1
+    if args.method in ("switching", "fixed"):
+        it = k - 1 if args.method == "switching" else k
         seed, stop = B.last_shift_info(L)
         active = sum(min(int(s) if s else it, it) for j, s in enumerate(stop) if j != 0) / max(it, 1)      # average active shifts per iteration
         bytes_it = 24.0 * nnz + 32.0 * n * active + 200.0 * n
