@@ -18,34 +18,18 @@ static_assert(offsetof(INFO_Matrix, code) == 12 && offsetof(INFO_Matrix, recvcou
 
 namespace {
 
-// shifted_switching_solver.h entry points (fixed = 0: shifted_lopbicg_switching, 1: shifted_lopbicg)
-int run_shifted(int fixed, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
+// the shifted entry points of shifted_switching_solver.h and shifted_solver.h (method = BICG_SHIFTED_*)
+int run_shifted(int method, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                 int sigma_len, int seed)
 {
-    if (info->cols != info->rows) {                      // shifted_switching_solver.c:28-31, 268-271
+    if (info->cols != info->rows) {   // shifted_switching_solver.c:28-31, 268-271; shifted_solver.c:190-193, 711-714
         printf("Error: matrix is not square.\n");
         exit(1);
     }
     Context &c = ctx();
     c.ensure();
     bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
-    const int k = shifted_solve(m, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, fixed);
-    if (!c.cfg.cache) matrix_destroy(m);
-    return k;
-}
-
-// shifted_solver.h entry points of the LOP family (pipe = 0: LOP, 1: PIPE-LOP)
-int run_shifted_lop(int pipe, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
-                    int sigma_len, int seed)
-{
-    if (info->cols != info->rows) {                      // shifted_solver.c:190-193, 711-714
-        printf("Error: matrix is not square.\n");
-        exit(1);
-    }
-    Context &c = ctx();
-    c.ensure();
-    bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
-    const int k = shifted_lop_solve(m, pipe, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    const int k = shifted_solve(m, method, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
     if (!c.cfg.cache) matrix_destroy(m);
     return k;
 }
@@ -103,7 +87,7 @@ int pipe_bicgstab_rr(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_
 int shifted_lopbicg_switching(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                               int sigma_len, int seed)
 {
-    return run_shifted(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_SWITCHING, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 
 // shifted_switching_solver.h:11 -- the fixed-seed variant: same prototype and meaning, but the seed never switches (when it
@@ -111,7 +95,7 @@ int shifted_lopbicg_switching(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, d
 int shifted_lopbicg(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma, int sigma_len,
                     int seed)
 {
-    return run_shifted(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_LOPBICG, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 
 // shifted_switching_solver.c:611 -- the reference's twin of the function above with the halo exchange NOT overlapped with the
@@ -132,27 +116,27 @@ int shifted_lopbicg_switching_noovlp(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *
 int shifted_lopbicgstab(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma, int sigma_len,
                         int seed)                                                         // shifted_solver.h:17
 {
-    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_LOP, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 int shifted_lopbicgstab_v2(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                            int sigma_len, int seed)                                       // shifted_solver.h:18
 {
-    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_LOP, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 int shifted_lopbicgstab_nooverlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                                   int sigma_len, int seed)                                // shifted_solver.h:19
 {
-    return run_shifted_lop(0, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_LOP, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 int shifted_pipe_lopbicgstab(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc, double *sigma,
                              int sigma_len, int seed)                                     // shifted_solver.h:20
 {
-    return run_shifted_lop(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_PIPE_LOP, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 int shifted_pipe_lopbicgstab_nooverlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc_set, double *r_loc,
                                        double *sigma, int sigma_len, int seed)            // shifted_solver.h:21
 {
-    return run_shifted_lop(1, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
+    return run_shifted(BICG_SHIFTED_PIPE_LOP, D, O, info, x_loc_set, r_loc, sigma, sigma_len, seed);
 }
 
 void MPI_csr_spmv_ovlap(CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, double *x_loc, double *x, double *y_loc)
@@ -227,7 +211,7 @@ int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();
-    const int k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, 0);
+    const int k = shifted_solve(m, BICG_SHIFTED_SWITCHING, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
     if (stats) *stats = c.last_stats;
     return k;
 }
@@ -235,19 +219,7 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
                           bicg_stats *stats)
 {
     Context &c = ctx();
-    c.ensure();
-    int k;
-    switch (method) {
-    case BICG_SHIFTED_SWITCHING:
-    case BICG_SHIFTED_LOPBICG:
-        k = shifted_solve(m, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, method == BICG_SHIFTED_LOPBICG);
-        break;
-    case BICG_SHIFTED_LOP:
-    case BICG_SHIFTED_PIPE_LOP:
-        k = shifted_lop_solve(m, method == BICG_SHIFTED_PIPE_LOP, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
-        break;
-    default: return -1;
-    }
+    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
     if (stats) *stats = c.last_stats;
     return k;
 }

@@ -9,6 +9,7 @@
 
 #include <cstdio>
 #include <cstdlib>
+#include <functional>
 #include <initializer_list>
 #include <map>
 #include <string>
@@ -90,7 +91,8 @@ struct Context {
     std::map<const void *, bicg_matrix *> cache;
     std::map<TuneKey, TuneVal> tuned;     // SpMV autotune winners by matrix shape
     // pinned scratch
-    int *h_flags = nullptr;      // ring of {k, max_iter, done, converged}
+    static constexpr int FLAG_RING = 64;
+    int *h_flags = nullptr;      // ring of FLAG_RING done flags, one per batch of iterations in flight (run_batches)
     // profiling of individual launches
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_ev;
@@ -233,15 +235,46 @@ int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, i
 int  spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full_or_null);
 int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);
-// shifted.cu (fixed = 0: shifted_lopbicg_switching, returns iterations + 1; 1: shifted_lopbicg, returns the iterations performed);
-// -1 for a bad sigma_len / seed
-int  shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol, int max_iter,
-                   int fixed);
-// shifted_lop.cu (pipe = 0: LOP, 1: PIPE-LOP); returns the iterations performed, -1 for a bad sigma_len / seed
-int  shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
-                       int max_iter);
+void print_times(double seconds, double iters);          // "Total time" / "Avg time/iter" (= seconds / iters), then flush
+void reset_scalars(bicg_matrix *m, double tol, int max_iter);   // Scalars of a new solve (enqueued on the stream)
+// The host side of every kernel-per-phase loop: enqueues batch b = 0, 1, ... of U iterations (max_iter / U rounded up)
+// and reads the device's done flag *d_done after each; from batch `depth` on it first waits for batch b - depth and
+// stops once the flag was raised by its end.  The loop test runs on the device, which returns from every kernel after it.
+void run_batches(int max_iter, int U, int depth, const int *d_done, const std::function<void(int)> &enqueue_batch);
+// shifted.cu: method = BICG_SHIFTED_*; returns what that solver returns (shifted_lopbicg_switching: iterations + 1, the others:
+// the iterations performed), -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len)
+int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
+                   int max_iter);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, int prof_class = 0);
+
+// reduction tails of the kernel-per-phase kernels
+inline TailDesc tail_none() { return TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0}; }
+inline TailDesc tail_allreduce(int fin, int ndot, int npend = 0) { return TailDesc{TAIL_ALLREDUCE, fin, ndot, npend, 0, 0, 0}; }
+inline TailDesc tail_post(int ndot) { return TailDesc{TAIL_POST, FIN_NONE, ndot, 0, 0, 0, 0}; }
+inline TailDesc tail_complete(int fin, int nred) { return TailDesc{TAIL_COMPLETE, fin, 0, 0, 0, nred, 0}; }
+inline TailDesc tail_pend(int ndot, int off) { return TailDesc{TAIL_PEND, FIN_NONE, ndot, 0, off, 0, 0}; }
+inline TailDesc tail_store(int ndot) { return TailDesc{TAIL_ALLREDUCE, FIN_STORE_PEND, ndot, 0, 0, 0, 0}; }   // -> Scalars::pend[]
+
+// Kernel-per-phase launcher (solve.cu): one fused vector kernel or one SpMV on the arena vectors per call, each with its
+// reduction tail.  The un-shifted loops of solve.cu and the shifted solvers (shifted.cu, shifted_lop.cu) share it.
+struct PhaseLauncher {
+    bicg_matrix *m;
+    Context &c;
+    const double *shift_sigma = nullptr;   // device scalar sigma: every SpMV computes y = (A + sigma I) x; null: y = A x
+    int launches = 0;                      // kernels launched through vec / spmv (a graph capture takes them back out)
+
+    explicit PhaseLauncher(bicg_matrix *mm) : m(mm), c(ctx()) {}
+    VecPtrs ptrs() const;
+    KernelCommon common(TailDesc tail) const;
+    PushDesc make_push(int id) const;
+    // one fused vector kernel; push_vec >= 0: that vector is the next SpMV's input (PH_PUSH: the push alone)
+    void vec(int phase, TailDesc tail, int push_vec = -1);
+    // y = A x (+ sigma x) with ndot (0..4) epilogue dots (a_k, b_k); a null b_k is the y just computed
+    void spmv(int x_id, int y_id, TailDesc tail, int ndot = 0, const double *a0 = nullptr, const double *b0 = nullptr,
+              const double *a1 = nullptr, const double *b1 = nullptr, const double *a2 = nullptr, const double *b2 = nullptr,
+              const double *a3 = nullptr, const double *b3 = nullptr);
+};
 
 } // namespace bicg

@@ -120,7 +120,7 @@ void Context::ensure()
     int rc = spmv_setup_attributes();
     if (rc == 0) rc = mega_setup_attributes();
     if (rc != 0) fatal("bicgstab_b200: cudaFuncSetAttribute failed: %s", cudaGetErrorString((cudaError_t)rc));
-    BICG_CUDA(cudaHostAlloc((void **)&h_flags, 64 * 4 * sizeof(int), cudaHostAllocDefault));
+    BICG_CUDA(cudaHostAlloc((void **)&h_flags, FLAG_RING * sizeof(int), cudaHostAllocDefault));
     ready = true;
 }
 

@@ -310,77 +310,77 @@ __global__ void __launch_bounds__(256) sh_vec_p(const __grid_constant__ ShVec a)
     }
 }
 
-struct ShRun : ShiftLaunch {
-    ShiftDev *d_sd;
+struct ShRun : PhaseLauncher {
+    ShiftDev *d_sd = nullptr;
     ShVec base{};
-    explicit ShRun(bicg_matrix *mm) : ShiftLaunch(mm), d_sd(nullptr) {}
+    using PhaseLauncher::PhaseLauncher;
 
     ShVec vargs(TailDesc tail) const
     {
         ShVec v = base;
-        v.kc.sc = m->d_sc; v.kc.partials = m->d_partials; v.kc.hist = m->d_hist; v.kc.comm = m->comm; v.kc.tail = tail;
+        v.kc = common(tail);
         return v;
+    }
+    void prologue()
+    {
+        sh_vec_init<<<m->vgrid, 256, 0, c.stream>>>(vargs(tail_store(1)));          // :342-354
+        sh_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc);
+        vec(PH_PUSH, tail_none(), V_P);
+        c.launches += 2;
     }
     void iteration()
     {
         const int G = m->vgrid;
         const double *Y = nullptr;
-        spmv(V_P, V_S, 1, m->vec(V_RH), Y);                                           // s = (A + sigma I) p, (r#,s)   :377-387
+        spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), Y);                            // s = (A + sigma I) p, (r#,s)   :377-387
         sh_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
         sh_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // q, r_old, q_copy            :374, 391-392
-        push(V_R);
-        spmv(V_R, V_Y, 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), Y);                  // y = (A + sigma I) q, (q,q), (q,y)  :395-406
+        vec(PH_PUSH, tail_none(), V_R);
+        spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), Y);   // y = (A + sigma I) q, (q,q), (q,y)  :395-406
         sh_scalar_omega<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
         sh_vec_xr<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));                     // x[seed], r, (r,r), (r#,r)   :411-416
         sh_scalar_iter<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                       // beta ... loop test          :420, 429-537
         const size_t smem = (size_t)base.L * (SH_COEF * sizeof(double) + sizeof(int));
         sh_vec_shift<<<std::max(1, std::min(c.sm_count * 8, (m->n_loc + 511) / 512)), 256, smem, c.stream>>>(vargs(tail_none()));
         sh_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // p[seed] (or the switch)     :421-423 / :499
-        push(V_P);
-        launches += 7; c.launches += 7;
+        vec(PH_PUSH, tail_none(), V_P);
+        c.launches += 7;
     }
 };
 
 } // namespace
 
-int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter_opt,
-                  int fixed)
+int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
+                    int max_iter_opt)
 {
-    Context &c = ctx();
-    c.ensure();
-    if (L <= 0 || seed < 0 || seed >= L) return -1;
-    const int n = m->n_loc;
+    ShiftedSolve s(m, L);
+    Context &c = s.c;
+    const int n = s.n;
     const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
-    const long long stride = ((long long)n + 15) / 16 * 16;
 
     // ---- device state -------------------------------------------------------------------------------------------------
     ShiftDev h{};
-    h.L = L; h.max_iter = max_iter; h.fixed = fixed; h.tol = tol; h.seed = seed;
-    auto dalloc = [&](size_t bytes) { return c.dev_alloc(std::max<size_t>(bytes, 16)); };
-    h.sigma = (double *)dalloc(L * sizeof(double));
-    h.alpha_set = (double *)dalloc(L * sizeof(double)); h.beta_set = (double *)dalloc(L * sizeof(double));
-    h.omega_set = (double *)dalloc(L * sizeof(double)); h.eta_set = (double *)dalloc(L * sizeof(double));
-    h.zeta_set = (double *)dalloc(L * sizeof(double));
-    h.stop_flag = (unsigned char *)dalloc(L); h.stop_iter = (int *)dalloc(L * sizeof(int));
-    h.alpha_arch = (double *)dalloc(max_iter * sizeof(double)); h.beta_arch = (double *)dalloc(max_iter * sizeof(double));
-    h.omega_arch = (double *)dalloc(max_iter * sizeof(double));
-    h.pi_arch = (double *)dalloc((size_t)L * max_iter * sizeof(double));
-    h.coef = (double *)dalloc((size_t)L * SH_COEF * sizeof(double)); h.active = (int *)dalloc(L * sizeof(int));
-    h.hist = (double *)dalloc(((size_t)max_iter + 1) * sizeof(double));
-    h.ev_k = (int *)dalloc(SH_EVENTS * sizeof(int)); h.ev_seed = (int *)dalloc(SH_EVENTS * sizeof(int));
-    h.ev_remain = (int *)dalloc(SH_EVENTS * sizeof(int));
-    h.ev_vals = (double *)dalloc((size_t)SH_EVENTS * L * 3 * sizeof(double));
-    ShiftDev *d_sd = (ShiftDev *)dalloc(sizeof(ShiftDev));
-    double *d_x = (double *)dalloc((size_t)L * stride * sizeof(double));
-    double *d_p = (double *)dalloc((size_t)L * stride * sizeof(double));
+    h.L = L; h.max_iter = max_iter; h.fixed = fixed ? 1 : 0; h.tol = tol; h.seed = seed;
+    h.sigma = s.alloc<double>(L);
+    h.alpha_set = s.alloc<double>(L); h.beta_set = s.alloc<double>(L);
+    h.omega_set = s.alloc<double>(L); h.eta_set = s.alloc<double>(L);
+    h.zeta_set = s.alloc<double>(L);
+    h.stop_flag = s.alloc<unsigned char>(L); h.stop_iter = s.alloc<int>(L);
+    h.alpha_arch = s.alloc<double>(max_iter); h.beta_arch = s.alloc<double>(max_iter);
+    h.omega_arch = s.alloc<double>(max_iter);
+    h.pi_arch = s.alloc<double>((size_t)L * max_iter);
+    h.coef = s.alloc<double>((size_t)L * SH_COEF); h.active = s.alloc<int>(L);
+    h.hist = s.alloc<double>((size_t)max_iter + 1);
+    h.ev_k = s.alloc<int>(SH_EVENTS); h.ev_seed = s.alloc<int>(SH_EVENTS);
+    h.ev_remain = s.alloc<int>(SH_EVENTS);
+    h.ev_vals = s.alloc<double>((size_t)SH_EVENTS * L * 3);
+    ShiftDev *d_sd = s.alloc<ShiftDev>(1);
+    double *d_p = s.alloc<double>((size_t)L * s.stride);
     BICG_CUDA(cudaMemcpyAsync(d_sd, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
     BICG_CUDA(cudaMemcpyAsync(h.sigma, sigma, L * sizeof(double), cudaMemcpyHostToDevice, c.stream));
     BICG_CUDA(cudaMemsetAsync(h.pi_arch, 0, (size_t)L * max_iter * sizeof(double), c.stream));
     BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), c.stream));
-    BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
-                                cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
-    sh_reset_scalars<<<1, 1, 0, c.stream>>>(m->d_sc);
+    s.upload(x_set, r);
 
     ShRun run(m);
     run.d_sd = d_sd;
@@ -388,69 +388,27 @@ int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma,
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);
-    run.base.x_set = d_x; run.base.p_set = d_p; run.base.stride = stride; run.base.n = n; run.base.L = L;
+    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.stride = s.stride; run.base.n = n; run.base.L = L;
     const size_t smem = (size_t)L * (SH_COEF * sizeof(double) + sizeof(int));
     if (smem > 48 * 1024) BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
 
-    cudaEvent_t e0, e1;
-    BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
-    const int launches0 = c.launches;
-    BICG_CUDA(cudaEventRecord(e0, c.stream));                                         // the reference's timed region :364
-    sh_vec_init<<<m->vgrid, 256, 0, c.stream>>>(run.vargs(tail_store(1)));            // :342-354
-    sh_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc);
-    run.push(V_P);
-    c.launches += 2;
-
-    const int U = 8, DEPTH = 2, RING = 64;
-    std::vector<cudaEvent_t> ring((size_t)RING, nullptr);
-    const int batches = (max_iter + U - 1) / U;
-    for (int b = 0; b < batches; ++b) {
-        if (b >= DEPTH) {
-            const int o = (b - DEPTH) % RING;
-            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
-            if (c.h_flags[o * 4 + 0]) break;                                          // done was raised in batch b - DEPTH
-        }
-        for (int u = 0; u < U; ++u) run.iteration();
-        const int o = b % RING;
-        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o * 4], &d_sd->done, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
-    }
-    BICG_CUDA(cudaEventRecord(e1, c.stream));
+    s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :364
+    const ShiftDev out = s.finish(x_set, r, d_sd);
 
     // ---- results ------------------------------------------------------------------------------------------------------
-    BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
-                                cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
-    ShiftDev out{};
-    BICG_CUDA(cudaMemcpyAsync(&out, d_sd, sizeof(ShiftDev), cudaMemcpyDeviceToHost, c.stream));
-    Scalars hs;
-    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);
-    if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted solver", m->rank);
-    float ms = 0.f;
-    BICG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-
     const int k = out.k;
     c.last_hist.assign((size_t)std::max(k, 1), 0.0);
     BICG_CUDA(cudaMemcpy(c.last_hist.data(), out.hist, (size_t)std::max(k, 1) * sizeof(double), cudaMemcpyDeviceToHost));
     c.last_shift_stop.assign((size_t)L, 0);
     BICG_CUDA(cudaMemcpy(c.last_shift_stop.data(), out.stop_iter, (size_t)L * sizeof(int), cudaMemcpyDeviceToHost));
     c.last_shift_seed = out.seed;
-    bicg_stats st{};
-    st.iters = k - 1; st.converged = out.stop_count >= L; st.final_res = sqrt(out.dot_r / out.dot_zero); st.loop_ms = ms;
-    st.kernel_launches = c.launches - launches0;
-    st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
+    bicg_stats st = s.stats();
+    st.iters = k - 1; st.converged = out.stop_count >= L; st.final_res = sqrt(out.dot_r / out.dot_zero);
     c.last_stats = st;
 
     if (c.rank == 0 && !c.cfg.quiet && fixed) {
         // shifted_lopbicg prints the MEASURE_TIME lines only, its average over the iterations performed (:241-242)
-        const double t = ms * 1e-3;
-        printf("Total time   : %e [sec.] \n", t);
-        printf("Avg time/iter: %e [sec.] \n", t / (double)(k - 1));
-        fflush(stdout);
+        print_times(s.ms * 1e-3, k - 1);
     } else if (c.rank == 0 && !c.cfg.quiet) {
         // what the reference prints: the seed switches (:518-526), then the MEASURE_TIME lines (:557-561)
         std::vector<int> ek(SH_EVENTS), es(SH_EVENTS), er(SH_EVENTS);
@@ -466,19 +424,24 @@ int shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma,
             }
             printf("k: %d, seed: %d, remain: %d\n", ek[(size_t)e], es[(size_t)e], er[(size_t)e]);
         }
-        const double t = ms * 1e-3;
         printf("Total iter   : %d\n", k - 1);
-        printf("Total time   : %e [sec.] \n", t);
-        printf("Avg time/iter: %e [sec.] \n", t / k);
-        fflush(stdout);
+        print_times(s.ms * 1e-3, k);
     }
-
-    for (void *p : {(void *)h.sigma, (void *)h.alpha_set, (void *)h.beta_set, (void *)h.omega_set, (void *)h.eta_set, (void *)h.zeta_set,
-                    (void *)h.stop_flag, (void *)h.stop_iter, (void *)h.alpha_arch, (void *)h.beta_arch, (void *)h.omega_arch,
-                    (void *)h.pi_arch, (void *)h.coef, (void *)h.active, (void *)h.hist, (void *)h.ev_k, (void *)h.ev_seed,
-                    (void *)h.ev_remain, (void *)h.ev_vals, (void *)d_sd, (void *)d_x, (void *)d_p})
-        c.dev_free(p);
     return fixed ? k - 1 : k;                                                         // :255 / :600
+}
+
+// the one mapping from a BICG_SHIFTED_* method to its solver
+int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter)
+{
+    ctx().ensure();
+    if (L <= 0 || seed < 0 || seed >= L) return -1;
+    switch (method) {
+    case BICG_SHIFTED_SWITCHING: return switching_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter);
+    case BICG_SHIFTED_LOPBICG:   return switching_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter);
+    case BICG_SHIFTED_LOP:       return lop_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter);
+    case BICG_SHIFTED_PIPE_LOP:  return lop_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter);
+    default: return -1;
+    }
 }
 
 } // namespace bicg

@@ -5,7 +5,7 @@
 // The seed never changes and no shift stops on its own: every non-seed shift is advanced in every iteration until
 // max_zeta_pi^2 dot_r <= tol^2 dot_zero (max_zeta_pi = max(1, max_j |1 / (zeta_j pi_j)|)) or MAX_ITER.
 //
-// Per iteration the seed runs on the arena vectors with the shifted SpMV epilogue (y = A x + sigma_seed x, shifted_run.cuh),
+// Per iteration the seed runs on the arena vectors with the shifted SpMV epilogue (y = A x + sigma_seed x, PhaseLauncher),
 // one scalar kernel derives every shift's coefficients (lop_scalar_shift), and ONE fused pass (lop_vec_update) updates the
 // seed's x and residual together with x_j and p_j of every shift, each read and written exactly once (32 B per row and
 // shift).  The reference scales p_j at the START of an iteration (p_j = beta_j p_j + r / (pi zeta), :264-269); that step is
@@ -272,18 +272,18 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
     kernel_tail<ND>(a.kc, dot, scratch);
 }
 
-struct LopRun : ShiftLaunch {
+struct LopRun : PhaseLauncher {
     LopDev *d_sd = nullptr;
     LopVec base{};
     bool pipe = false;
     int ugrid = 1;                                      // grid of lop_vec_update
     size_t smem = 0;                                    // its coefficient table
-    explicit LopRun(bicg_matrix *mm) : ShiftLaunch(mm) {}
+    using PhaseLauncher::PhaseLauncher;
 
     LopVec vargs(TailDesc tail) const
     {
         LopVec v = base;
-        v.kc.sc = m->d_sc; v.kc.partials = m->d_partials; v.kc.hist = m->d_hist; v.kc.comm = m->comm; v.kc.tail = tail;
+        v.kc = common(tail);
         return v;
     }
     void prologue()
@@ -292,84 +292,76 @@ struct LopRun : ShiftLaunch {
         lop_vec_init<<<G, 256, 0, c.stream>>>(vargs(tail_store(1)), pipe ? 1 : 0);
         lop_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc, pipe ? 1 : 0);
         c.launches += 2;
-        if (!pipe) { push(V_P); return; }
-        push(V_R);
-        spmv(V_R, V_W, 1, m->vec(V_R), nullptr);                                       // w = (A + sigma I) r, (r,w)  :765-767
+        if (!pipe) { vec(PH_PUSH, tail_none(), V_P); return; }
+        vec(PH_PUSH, tail_none(), V_R);
+        spmv(V_R, V_W, tail_store(1), 1, m->vec(V_R), nullptr);                         // w = (A + sigma I) r, (r,w)  :765-767
         lop_scalar_pipe_init<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                       :787
-        push(V_W);
-        spmv(V_W, V_T, 0);                                                             // t = (A + sigma I) w          :769-770
-        launches += 1; c.launches += 1;
+        vec(PH_PUSH, tail_none(), V_W);
+        spmv(V_W, V_T, tail_none());                                                   // t = (A + sigma I) w          :769-770
+        c.launches += 1;
     }
     void iteration()
     {
         const int G = m->vgrid;
         if (!pipe) {
-            spmv(V_P, V_S, 1, m->vec(V_RH), nullptr);                                  // s = (A + sigma I) p, (r#,s)   :261-263
+            spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), nullptr);                    // s = (A + sigma I) p, (r#,s)   :261-263
             lop_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                        :276
             lop_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // r_old, q                     :271, 277
-            push(V_R);
-            spmv(V_R, V_Y, 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);         // y = (A + sigma I) q, (q,q), (q,y)  :278-282
+            vec(PH_PUSH, tail_none(), V_R);
+            spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);   // y = (A + sigma I) q, (q,q), (q,y)  :278-282
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
             lop_vec_update<false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
             lop_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // p[seed]                      :319-321
-            push(V_P);
-            launches += 6; c.launches += 6;
+            vec(PH_PUSH, tail_none(), V_P);
+            c.launches += 6;
         } else {
             lop_vec_pipe1<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));              // p, s, z, q, y, (q,y), (y,y)   :795-814
-            push(V_Z);
-            spmv(V_Z, V_V, 0);                                                         // v = (A + sigma I) z           :815-816
+            vec(PH_PUSH, tail_none(), V_Z);
+            spmv(V_Z, V_V, tail_none());                                               // v = (A + sigma I) z           :815-816
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
             lop_vec_update<true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
-            push(V_W);
-            spmv(V_W, V_T, 0);                                                         // t = (A + sigma I) w           :850-851
+            vec(PH_PUSH, tail_none(), V_W);
+            spmv(V_W, V_T, tail_none());                                               // t = (A + sigma I) w           :850-851
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 1);                   // beta, alpha, loop test       :857-865
-            launches += 4; c.launches += 4;
+            c.launches += 4;
         }
     }
 };
 
 } // namespace
 
-int shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
-                      int max_iter)
+int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter)
 {
-    Context &c = ctx();
-    c.ensure();
-    if (L <= 0 || seed < 0 || seed >= L) return -1;
-    const int n = m->n_loc;
-    const long long stride = ((long long)n + 15) / 16 * 16;
+    ShiftedSolve s(m, L);
+    Context &c = s.c;
+    const int n = s.n;
 
     // ---- device state -------------------------------------------------------------------------------------------------
     LopDev h{};
     h.L = L; h.max_iter = max_iter; h.tol = tol; h.seed = seed; h.sigma_seed = sigma[seed];
-    auto dalloc = [&](size_t bytes) { return c.dev_alloc(std::max<size_t>(bytes, 16)); };
-    h.sigma = (double *)dalloc(L * sizeof(double));
-    h.eta = (double *)dalloc(L * sizeof(double)); h.zeta = (double *)dalloc(L * sizeof(double));
-    h.pi_old = (double *)dalloc(L * sizeof(double)); h.pi_new = (double *)dalloc(L * sizeof(double));
-    h.coef = (double *)dalloc((size_t)(L - 1) * LOP_COEF * sizeof(double));
-    h.hist = (double *)dalloc(((size_t)max_iter + 1) * sizeof(double));
-    LopDev *d_sd = (LopDev *)dalloc(sizeof(LopDev));
-    double *d_x = (double *)dalloc((size_t)L * stride * sizeof(double));
-    double *d_p = (double *)dalloc((size_t)L * stride * sizeof(double));
+    h.sigma = s.alloc<double>(L);
+    h.eta = s.alloc<double>(L); h.zeta = s.alloc<double>(L);
+    h.pi_old = s.alloc<double>(L); h.pi_new = s.alloc<double>(L);
+    h.coef = s.alloc<double>((size_t)(L - 1) * LOP_COEF);
+    h.hist = s.alloc<double>((size_t)max_iter + 1);
+    LopDev *d_sd = s.alloc<LopDev>(1);
+    double *d_p = s.alloc<double>((size_t)L * s.stride);
     BICG_CUDA(cudaMemcpyAsync(d_sd, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
     BICG_CUDA(cudaMemcpyAsync(h.sigma, sigma, L * sizeof(double), cudaMemcpyHostToDevice, c.stream));
     BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), c.stream));
-    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)L * stride * sizeof(double), c.stream));          // p_loc_set = calloc(...)  :226
-    BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
-                                cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
-    sh_reset_scalars<<<1, 1, 0, c.stream>>>(m->d_sc);
+    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)L * s.stride * sizeof(double), c.stream));        // p_loc_set = calloc(...)  :226
+    s.upload(x_set, r);
 
     LopRun run(m);
-    run.pipe = pipe != 0;
+    run.pipe = pipe;
     run.d_sd = d_sd;
     run.shift_sigma = &d_sd->sigma_seed;
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.z = m->vec(V_Z); run.base.w = m->vec(V_W); run.base.v = m->vec(V_V); run.base.t = m->vec(V_T);
-    run.base.rold = m->vec(run.pipe ? V_AX : V_V);
-    run.base.x_set = d_x; run.base.p_set = d_p; run.base.stride = stride; run.base.n = n; run.base.L = L;
+    run.base.rold = m->vec(pipe ? V_AX : V_V);
+    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.stride = s.stride; run.base.n = n; run.base.L = L;
     run.ugrid = std::max(1, std::min(c.sm_count * 8, (n + 511) / 512));
     run.smem = (size_t)(L - 1) * LOP_COEF * sizeof(double);
     if (run.smem > 48 * 1024) {
@@ -377,68 +369,25 @@ int shifted_lop_solve(bicg_matrix *m, int pipe, double *x_set, double *r, const 
         BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
     }
 
-    cudaEvent_t e0, e1;
-    BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
-    const int launches0 = c.launches;
-    BICG_CUDA(cudaEventRecord(e0, c.stream));                                         // the reference's timed region :237 / :759
-    run.prologue();
-
-    const int U = 8, DEPTH = 2, RING = 64;
-    std::vector<cudaEvent_t> ring((size_t)RING, nullptr);
-    const int batches = (max_iter + U - 1) / U;
-    for (int b = 0; b < batches; ++b) {
-        if (b >= DEPTH) {
-            const int o = (b - DEPTH) % RING;
-            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
-            if (c.h_flags[o * 4 + 0]) break;                                          // done was raised in batch b - DEPTH
-        }
-        for (int u = 0; u < U; ++u) run.iteration();
-        const int o = b % RING;
-        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o * 4], &d_sd->done, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
-    }
-    BICG_CUDA(cudaEventRecord(e1, c.stream));
+    s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :237 / :759
+    const LopDev out = s.finish(x_set, r, d_sd);
 
     // ---- results ------------------------------------------------------------------------------------------------------
-    BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
-                                cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
-    LopDev out{};
-    BICG_CUDA(cudaMemcpyAsync(&out, d_sd, sizeof(LopDev), cudaMemcpyDeviceToHost, c.stream));
-    Scalars hs;
-    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);
-    if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted solver", m->rank);
-    float ms = 0.f;
-    BICG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
-    cudaEventDestroy(e0); cudaEventDestroy(e1);
-
     const int k = out.k;
     c.last_hist.assign((size_t)k + 1, 0.0);
     BICG_CUDA(cudaMemcpy(c.last_hist.data(), out.hist, ((size_t)k + 1) * sizeof(double), cudaMemcpyDeviceToHost));
-    bicg_stats st{};
+    bicg_stats st = s.stats();
     const double res = sqrt(out.dot_r / out.dot_zero);
     st.iters = k;
     st.converged = out.max_zeta_pi * out.max_zeta_pi * out.dot_r <= out.tol * out.tol * out.dot_zero;      // false after a NaN
-    st.final_res = res; st.loop_ms = ms;
-    st.kernel_launches = c.launches - launches0;
-    st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
+    st.final_res = res;
     c.last_stats = st;
 
     if (c.rank == 0 && !c.cfg.quiet) {                                                // :339-346 / :882-889
-        const double t = ms * 1e-3;
         printf("Total iter   : %d\n", k);
         printf("Final r      : %e\n", res);
-        printf("Total time   : %e [sec.] \n", t);
-        printf("Avg time/iter: %e [sec.] \n", t / k);
-        fflush(stdout);
+        print_times(s.ms * 1e-3, k);
     }
-
-    for (void *p : {(void *)h.sigma, (void *)h.eta, (void *)h.zeta, (void *)h.pi_old, (void *)h.pi_new, (void *)h.coef,
-                    (void *)h.hist, (void *)d_sd, (void *)d_x, (void *)d_p})
-        c.dev_free(p);
     return k;                                                                         // :352 / :894
 }
 

@@ -1,75 +1,93 @@
-// shifted_run.cuh -- host-side launch helpers shared by the shifted solvers (shifted.cu, shifted_lop.cu): the halo push of an
-// arena vector before an SpMV (kernel-per-phase protocol) and the SpMV y = (A + sigma_seed I) x with up to two epilogue dots
-// whose totals land in Scalars::pend[] for the solver's own scalar kernels.
+// shifted_run.cuh -- the host side every shifted solver shares (shifted.cu, shifted_lop.cu).  The seed system runs on the
+// arena vectors through PhaseLauncher (engine.hpp) with shift_sigma set, so its SpMVs compute y = (A + sigma_seed I) x, and
+// tail_store puts the reduced epilogue dots into Scalars::pend[] for the solver's own scalar kernels.  ShiftedSolve holds
+// everything around a solver's own device state and kernel sequence: the device memory the solve owns, the sigma_len
+// solutions x_j in one strided device buffer, b in / the seed residual out through the arena's r, the timed loop and the
+// statistics every shifted solver reports alike.
 #pragma once
 #include "engine.hpp"
 
+#include <algorithm>
+#include <vector>
+
 namespace bicg {
-namespace {
 
-inline TailDesc tail_none() { return TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0}; }
-inline TailDesc tail_store(int ndot) { return TailDesc{TAIL_ALLREDUCE, FIN_STORE_PEND, ndot, 0, 0, 0, 0}; }
+// the two families behind shifted_solve, which has checked sigma_len and seed: shifted.cu (fixed: shifted_lopbicg, else
+// shifted_lopbicg_switching) and shifted_lop.cu (pipe: PIPE-LOP, else LOP)
+int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
+                    int max_iter);
+int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter);
 
-__global__ void sh_reset_scalars(Scalars *s)
-{
-    s->alpha = s->beta = s->omega = 0.0;
-    for (int k = 0; k < MAX_DOTS; ++k) s->pend[k] = 0.0;
-    s->k = 0; s->max_iter = 0; s->done = 0; s->converged = 0; s->error = 0; s->ticket = 0u;
-}
-
-struct ShiftLaunch {
+struct ShiftedSolve {
+    static constexpr int U = 8, DEPTH = 2;   // iterations per batch; batches enqueued ahead of the done flag the host reads
     bicg_matrix *m;
     Context &c;
-    const double *shift_sigma = nullptr;          // device scalar the SpMV epilogue adds as sigma x
-    int launches = 0;
-    explicit ShiftLaunch(bicg_matrix *mm) : m(mm), c(ctx()) {}
+    const int n, L;
+    const long long stride;                  // doubles between consecutive shifts in x_set / p_set (16-byte aligned blocks)
+    double *d_x = nullptr;                   // [L][stride] the solutions x_j
+    float ms = 0.f;                          // length of the timed region
+    int launches0 = 0;
+    std::vector<void *> owned;
 
-    PushDesc make_push(int id) const
+    ShiftedSolve(bicg_matrix *mm, int sigma_len)
+        : m(mm), c(ctx()), n(mm->n_loc), L(sigma_len), stride(((long long)mm->n_loc + 15) / 16 * 16) {}
+    ~ShiftedSolve() { for (void *p : owned) c.dev_free(p); }
+    ShiftedSolve(const ShiftedSolve &) = delete;
+    ShiftedSolve &operator=(const ShiftedSolve &) = delete;
+
+    template <class T> T *alloc(size_t count)       // device memory freed when the solve ends
     {
-        PushDesc pd{};
-        if (m->world == 1) return pd;
-        pd.npeers = m->npush; pd.fence_writers = c.cfg.fence_writers;
-        pd.src = m->vec(id);
-        for (int s = 0; s < m->npush; ++s) {
-            const int d = m->push_peer[s];
-            pd.dst[s] = (double *)((char *)m->peer_base[d] + m->peer_vec_off[d]) + (long long)id * m->peer_vstride[d] + m->peer_ghost_off[d];
-            pd.runs[s] = m->d_push_runs[s]; pd.nruns[s] = m->push_nruns[s];
-        }
-        return pd;
+        void *p = c.dev_alloc(std::max<size_t>(count * sizeof(T), 16));
+        owned.push_back(p);
+        return (T *)p;
     }
-    VecArgs vec_args(TailDesc tail) const
+    // x_set (L blocks of n) -> d_x, b -> the arena's r, fresh solver scalars
+    void upload(const double *x_set, const double *r)
     {
-        VecArgs a{};
-        a.kc.sc = m->d_sc; a.kc.partials = m->d_partials; a.kc.hist = m->d_hist; a.kc.comm = m->comm; a.kc.tail = tail;
-        a.v.x = m->vec(V_X); a.v.r = m->vec(V_R); a.v.rh = m->vec(V_RH); a.v.p = m->vec(V_P); a.v.s = m->vec(V_S);
-        a.v.y = m->vec(V_Y); a.v.z = m->vec(V_Z); a.v.w = m->vec(V_W); a.v.v = m->vec(V_V); a.v.t = m->vec(V_T);
-        a.v.b = m->vec(V_B); a.v.ax = m->vec(V_AX);
-        a.n = m->n_loc; a.chunk = m->vchunk;
-        return a;
+        d_x = alloc<double>((size_t)L * stride);
+        BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
+                                    cudaMemcpyHostToDevice, c.stream));
+        BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+        reset_scalars(m, 0.0, 0);
     }
-    void push(int id)                             // halo of arena vector `id` for the next SpMV (kernel-per-phase protocol)
+    // the reference's timed region: run.prologue(), then batches of U run.iteration() until the device raises *d_done
+    template <class Run> void run(Run &run, int max_iter, const int *d_done)
     {
-        if (m->world == 1) return;
-        VecArgs a = vec_args(tail_none());
-        a.kc.tail.signal_halo = 1;
-        a.push = make_push(id);
-        int rc = launch_vec(PH_PUSH, m->vgrid, a, c.stream);
-        if (rc) fatal("bicgstab_b200: push kernel launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        ++launches; ++c.launches;
+        BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
+        launches0 = c.launches;
+        BICG_CUDA(cudaEventRecord(e0, c.stream));
+        run.prologue();
+        run_batches(max_iter, U, DEPTH, d_done, [&](int) { for (int u = 0; u < U; ++u) run.iteration(); });
+        BICG_CUDA(cudaEventRecord(e1, c.stream));
     }
-    // y = (A + sigma I) x; ndot (0..2) epilogue dots, a null b = the y just computed
-    void spmv(int x_id, int y_id, int ndot, const double *a0 = nullptr, const double *b0 = nullptr, const double *a1 = nullptr,
-              const double *b1 = nullptr)
+    // after run(): x_set, the seed residual r and the solver's device state *d_state back to the host
+    template <class State> State finish(double *x_set, double *r, const State *d_state)
     {
-        SpmvArgs a = make_spmv_args(m, m->plan, x_id, y_id);
-        a.kc.tail = ndot > 0 ? tail_store(ndot) : tail_none();
-        a.shift_sigma = shift_sigma;
-        if (ndot > 0) epi_add_dot(a.epi, a0, b0);
-        if (ndot > 1) epi_add_dot(a.epi, a1, b1);
-        launch_spmv_plan(m, m->plan, a, 0);
-        ++launches;
+        BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
+                                    cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+        State out{};
+        BICG_CUDA(cudaMemcpyAsync(&out, d_state, sizeof(State), cudaMemcpyDeviceToHost, c.stream));
+        Scalars hs;
+        BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+        if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted solver", m->rank);
+        BICG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
+        cudaEventDestroy(e0); cudaEventDestroy(e1);
+        return out;
     }
+    // after finish(): the statistics every shifted solver fills alike (the solver adds iters, converged, final_res)
+    bicg_stats stats() const
+    {
+        bicg_stats st{};
+        st.loop_ms = ms;
+        st.kernel_launches = c.launches - launches0;
+        st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
+        return st;
+    }
+
+private:
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
 };
 
-} // namespace
 } // namespace bicg

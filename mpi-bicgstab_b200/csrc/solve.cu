@@ -41,45 +41,115 @@ __global__ void fill_kernel(double *p, int n, double v)
 
 __global__ void set_coef_kernel(Scalars *s, double al, double be, double om) { s->alpha = al; s->beta = be; s->omega = om; }
 
-inline TailDesc tail_none() { return TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0}; }
-inline TailDesc tail_allreduce(int fin, int ndot, int npend = 0) { return TailDesc{TAIL_ALLREDUCE, fin, ndot, npend, 0, 0, 0}; }
-inline TailDesc tail_post(int ndot) { return TailDesc{TAIL_POST, FIN_NONE, ndot, 0, 0, 0, 0}; }
-inline TailDesc tail_complete(int fin, int nred) { return TailDesc{TAIL_COMPLETE, fin, 0, 0, 0, nred, 0}; }
-inline TailDesc tail_pend(int ndot, int off) { return TailDesc{TAIL_PEND, FIN_NONE, ndot, 0, off, 0, 0}; }
+} // namespace
 
-struct Seq {
-    bicg_matrix *m;
-    Context &c;
-    int launches = 0;
+void reset_scalars(bicg_matrix *m, double tol, int max_iter)
+{
+    reset_state_kernel<<<1, 1, 0, ctx().stream>>>(m->d_sc, tol, max_iter);
+}
 
-    explicit Seq(bicg_matrix *mm) : m(mm), c(ctx()) {}
+VecPtrs PhaseLauncher::ptrs() const
+{
+    VecPtrs v;
+    v.x = m->vec(V_X); v.r = m->vec(V_R); v.rh = m->vec(V_RH); v.p = m->vec(V_P); v.s = m->vec(V_S);
+    v.y = m->vec(V_Y); v.z = m->vec(V_Z); v.w = m->vec(V_W); v.v = m->vec(V_V); v.t = m->vec(V_T);
+    v.b = m->vec(V_B); v.ax = m->vec(V_AX);
+    return v;
+}
 
-    VecPtrs ptrs() const
-    {
-        VecPtrs v;
-        v.x = m->vec(V_X); v.r = m->vec(V_R); v.rh = m->vec(V_RH); v.p = m->vec(V_P); v.s = m->vec(V_S);
-        v.y = m->vec(V_Y); v.z = m->vec(V_Z); v.w = m->vec(V_W); v.v = m->vec(V_V); v.t = m->vec(V_T);
-        v.b = m->vec(V_B); v.ax = m->vec(V_AX);
-        return v;
+KernelCommon PhaseLauncher::common(TailDesc tail) const
+{
+    KernelCommon kc{};
+    kc.sc = m->d_sc; kc.partials = m->d_partials; kc.hist = m->d_hist; kc.comm = m->comm;
+    kc.tail = tail;
+    return kc;
+}
+
+// where the runs of vector `id` that peers need go: their ghost slots, addressed through the IPC mappings
+PushDesc PhaseLauncher::make_push(int id) const
+{
+    PushDesc pd{};
+    if (m->world == 1) return pd;
+    pd.npeers = m->npush;
+    pd.fence_writers = c.cfg.fence_writers;
+    pd.src = m->vec(id);
+    for (int s = 0; s < m->npush; ++s) {
+        const int d = m->push_peer[s];
+        pd.dst[s] = (double *)((char *)m->peer_base[d] + m->peer_vec_off[d]) + (long long)id * m->peer_vstride[d] +
+                    m->peer_ghost_off[d];
+        pd.runs[s] = m->d_push_runs[s];
+        pd.nruns[s] = m->push_nruns[s];
     }
+    return pd;
+}
 
-    // where the runs of vector `id` that peers need go: their ghost slots, addressed through the IPC mappings
-    PushDesc make_push(int id) const
-    {
-        PushDesc pd{};
-        if (m->world == 1) return pd;
-        pd.npeers = m->npush;
-        pd.fence_writers = c.cfg.fence_writers;
-        pd.src = m->vec(id);
-        for (int s = 0; s < m->npush; ++s) {
-            const int d = m->push_peer[s];
-            pd.dst[s] = (double *)((char *)m->peer_base[d] + m->peer_vec_off[d]) + (long long)id * m->peer_vstride[d] +
-                        m->peer_ghost_off[d];
-            pd.runs[s] = m->d_push_runs[s];
-            pd.nruns[s] = m->push_nruns[s];
+void PhaseLauncher::vec(int phase, TailDesc tail, int push_vec)
+{
+    VecArgs a{};
+    a.kc = common(tail);
+    a.v = ptrs(); a.n = m->n_loc; a.chunk = m->vchunk;
+    a.push.npeers = 0; a.push.src = nullptr;
+    if (push_vec >= 0 && m->world > 1) {
+        a.kc.tail.signal_halo = 1;               // every rank advances its halo epoch, senders also signal
+        a.push = make_push(push_vec);
+    } else if (phase == PH_PUSH) {
+        return;                                   // single rank: nothing to exchange
+    }
+    cudaEvent_t e0 = nullptr, e1 = nullptr;
+    if (c.prof_on) { BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1)); BICG_CUDA(cudaEventRecord(e0, c.stream)); }
+    int rc = launch_vec(phase, m->vgrid, a, c.stream);
+    if (rc) fatal("bicgstab_b200: vector kernel launch failed (phase %d): %s", phase, cudaGetErrorString((cudaError_t)rc));
+    if (c.prof_on) {
+        BICG_CUDA(cudaEventRecord(e1, c.stream));
+        c.prof_ev.push_back(e0); c.prof_ev.push_back(e1); c.prof_class.push_back(phase == PH_PUSH ? 2 : 1);
+    }
+    ++launches; ++c.launches;
+}
+
+void PhaseLauncher::spmv(int x_id, int y_id, TailDesc tail, int ndot, const double *a0, const double *b0, const double *a1,
+                         const double *b1, const double *a2, const double *b2, const double *a3, const double *b3)
+{
+    SpmvArgs a = make_spmv_args(m, m->plan, x_id, y_id);
+    a.kc.tail = tail;
+    a.shift_sigma = shift_sigma;
+    const double *as[4] = {a0, a1, a2, a3}, *bs[4] = {b0, b1, b2, b3};
+    for (int k = 0; k < ndot; ++k) epi_add_dot(a.epi, as[k], bs[k]);
+    launch_spmv_plan(m, m->plan, a, 0);
+    ++launches;
+}
+
+void run_batches(int max_iter, int U, int depth, const int *d_done, const std::function<void(int)> &enqueue_batch)
+{
+    Context &c = ctx();
+    std::vector<cudaEvent_t> ring((size_t)Context::FLAG_RING, nullptr);
+    const int batches = (max_iter + U - 1) / U;
+    for (int b = 0; b < batches; ++b) {
+        if (b >= depth) {
+            const int o = (b - depth) % Context::FLAG_RING;
+            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
+            if (c.h_flags[o]) break;                             // done was raised in batch b - depth
         }
-        return pd;
+        enqueue_batch(b);
+        const int o = b % Context::FLAG_RING;
+        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o], d_done, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
+        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
     }
+    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);       // released by the driver once the stream has passed them
+}
+
+void print_times(double seconds, double iters)
+{
+    printf("Total time   : %e [sec.] \n", seconds);                                         // solver.c:138
+    printf("Avg time/iter: %e [sec.] \n", seconds / iters);                                 // solver.c:139
+    fflush(stdout);
+}
+
+namespace {
+
+// the un-shifted loops: the reference's iteration bodies on the launcher, or the persistent kernel for the whole loop
+struct Seq : PhaseLauncher {
+    using PhaseLauncher::PhaseLauncher;
 
     // the persistent kernel runs the whole loop (mega.cu); false: it could not be launched
     bool mega(int method, int krr, int nrr)
@@ -132,43 +202,6 @@ struct Seq {
         }
         ++launches; ++c.launches;
         return true;
-    }
-
-    // one fused vector kernel; push_vec >= 0: that vector is the next SpMV's input
-    void vec(int phase, TailDesc tail, int push_vec = -1)
-    {
-        VecArgs a{};
-        a.kc.sc = m->d_sc; a.kc.partials = m->d_partials; a.kc.hist = m->d_hist; a.kc.comm = m->comm;
-        a.kc.tail = tail;
-        a.v = ptrs(); a.n = m->n_loc; a.chunk = m->vchunk;
-        a.push.npeers = 0; a.push.src = nullptr;
-        if (push_vec >= 0 && m->world > 1) {
-            a.kc.tail.signal_halo = 1;               // every rank advances its halo epoch, senders also signal
-            a.push = make_push(push_vec);
-        } else if (phase == PH_PUSH) {
-            return;                                   // single rank: nothing to exchange
-        }
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        if (c.prof_on) { BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1)); BICG_CUDA(cudaEventRecord(e0, c.stream)); }
-        int rc = launch_vec(phase, m->vgrid, a, c.stream);
-        if (rc) fatal("bicgstab_b200: vector kernel launch failed (phase %d): %s", phase, cudaGetErrorString((cudaError_t)rc));
-        if (c.prof_on) {
-            BICG_CUDA(cudaEventRecord(e1, c.stream));
-            c.prof_ev.push_back(e0); c.prof_ev.push_back(e1); c.prof_class.push_back(phase == PH_PUSH ? 2 : 1);
-        }
-        ++launches; ++c.launches;
-    }
-
-    void spmv(int x_id, int y_id, TailDesc tail, int ndot = 0, const double *a0 = nullptr, const double *b0 = nullptr,
-              const double *a1 = nullptr, const double *b1 = nullptr, const double *a2 = nullptr, const double *b2 = nullptr,
-              const double *a3 = nullptr, const double *b3 = nullptr)
-    {
-        SpmvArgs a = make_spmv_args(m, m->plan, x_id, y_id);
-        a.kc.tail = tail;
-        const double *as[4] = {a0, a1, a2, a3}, *bs[4] = {b0, b1, b2, b3};
-        for (int k = 0; k < ndot; ++k) epi_add_dot(a.epi, as[k], bs[k]);
-        launch_spmv_plan(m, m->plan, a, 0);
-        ++launches;
     }
 
     // ---- solver.c:74-83 --------------------------------------------------------------------------------
@@ -283,9 +316,7 @@ void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist
     const double t = st.loop_ms * 1e-3;
     printf("Total iter   : %d\n", st.iters);                                                // solver.c:135
     printf("Final r      : %e\n", st.final_res);                                            // solver.c:136
-    printf("Total time   : %e [sec.] \n", t);                                               // solver.c:138
-    printf("Avg time/iter: %e [sec.] \n", t / st.iters);                                    // solver.c:139
-    fflush(stdout);
+    print_times(t, st.iters);
 }
 
 int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *out)
@@ -317,7 +348,7 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     BICG_CUDA(cudaEventRecord(e_in0, c.stream));
     BICG_CUDA(cudaMemcpyAsync(m->vec(V_X), x, vbytes, in_kind, c.stream));
     BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, vbytes, in_kind, c.stream));
-    reset_state_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, cfg.tol, max_iter);
+    reset_scalars(m, cfg.tol, max_iter);
     if (method != BICG_METHOD_BICGSTAB) {
         // p, s, z, v, t start at zero: the defined version of the reference's uninitialised reads (SURVEY 5)
         const int zero_ids[5] = {(int)V_P, (int)V_S, (int)V_Z, (int)V_V, (int)V_T};
@@ -339,39 +370,25 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     if (use_mega) use_mega = seq.mega(method, krr, nrr);
     const bool use_graph = cfg.graph && !c.prof_on && method != BICG_METHOD_PIPE_RR;   // replacement iterations are host-scheduled
     const int U = std::max(1, cfg.unroll);
-    const int batches = (max_iter + U - 1) / U;
-    const int DEPTH = 3, RING = 64;
-    std::vector<cudaEvent_t> ring((size_t)RING, nullptr);
     if (use_graph && !use_mega) ensure_graph(m, method, U);
-    int launched_batches = 0;
-    for (int b = 0; b < batches && !use_mega; ++b) {
-        if (b >= DEPTH) {
-            const int o = (b - DEPTH) % RING;
-            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
-            if (c.h_flags[o * 4 + 2]) break;                     // done was raised in batch b - DEPTH
-        }
+    if (!use_mega) run_batches(max_iter, U, 3, &m->d_sc->done, [&](int b) {
         if (use_graph) {
             BICG_CUDA(cudaGraphLaunch(m->graph[method], c.stream));
             c.launches += U * kernels_per_iter(method, m->world);
-        } else {
-            for (int u = 0; u < U; ++u) {
-                const int k = b * U + u;
-                if (k >= max_iter) break;
-                if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_iter();
-                else if (method == BICG_METHOD_CA) seq.ca_iter();
-                else if (method == BICG_METHOD_PIPE) seq.pipe_iter();
-                else {
-                    const bool replace = (k % krr == 0) && k > 0 && k <= krr * nrr;       // solver.c:498, 522
-                    if (replace) seq.rr_replace_iter(); else seq.pipe_iter();
-                }
+            return;
+        }
+        for (int u = 0; u < U; ++u) {
+            const int k = b * U + u;
+            if (k >= max_iter) break;
+            if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_iter();
+            else if (method == BICG_METHOD_CA) seq.ca_iter();
+            else if (method == BICG_METHOD_PIPE) seq.pipe_iter();
+            else {
+                const bool replace = (k % krr == 0) && k > 0 && k <= krr * nrr;       // solver.c:498, 522
+                if (replace) seq.rr_replace_iter(); else seq.pipe_iter();
             }
         }
-        const int o = b % RING;
-        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o * 4], &m->d_sc->k, 4 * sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
-        ++launched_batches;
-    }
+    });
     BICG_CUDA(cudaEventRecord(e_loop1, c.stream));
 
     // ---- outputs ---------------------------------------------------------------------------------------
@@ -381,8 +398,6 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     Scalars hs;
     BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
-    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);
-    (void)launched_batches;
 
     if (hs.error) fatal("bicgstab_b200: rank %d timed out after %d s waiting for a peer GPU / another CTA (halo flag or reduction "
                         "mailbox; BICG_PEER_TIMEOUT_S raises the bound)", m->rank, cfg.peer_timeout_s);
@@ -466,7 +481,7 @@ int spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full
     c.ensure();
     const size_t vbytes = (size_t)m->n_loc * sizeof(double);
     BICG_CUDA(cudaMemcpyAsync(m->vec(V_X), x_loc, vbytes, cudaMemcpyHostToDevice, c.stream));
-    reset_state_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, c.cfg.tol, c.cfg.max_iter);
+    reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
     Seq seq(m);
     seq.vec(PH_PUSH, tail_none(), V_X);
     // With peers the SpMV ends in an (empty) cross-GPU reduction = a barrier: nobody may push the next x into a
@@ -499,7 +514,7 @@ int spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
 {
     Context &c = ctx();
     c.ensure();
-    reset_state_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, c.cfg.tol, c.cfg.max_iter);
+    reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
     fill_kernel<<<256, 256, 0, c.stream>>>(m->vec(V_P), (int)m->vstride, 1.0);
     fill_kernel<<<256, 256, 0, c.stream>>>(m->vec(V_RH), m->n_loc, 1.0);
     SpmvArgs a = make_spmv_args(m, m->plan, V_P, V_S);
@@ -536,7 +551,7 @@ extern "C" int bicg_debug_vec_phase(bicg_matrix *m, int phase, const double coef
     const size_t vb = (size_t)m->n_loc * sizeof(double);
     for (int id = 0; id < V_COUNT; ++id)
         BICG_CUDA(cudaMemcpyAsync(m->vec(id), vecs + (size_t)id * m->n_loc, vb, cudaMemcpyHostToDevice, c.stream));
-    reset_state_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, c.cfg.tol, c.cfg.max_iter);
+    reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
     set_coef_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, coef[0], coef[1], coef[2]);
     static const int ndots[PH_PUSH] = {phase_ndot(PH_BICG_INIT), phase_ndot(PH_BICG_Q), phase_ndot(PH_BICG_XR), phase_ndot(PH_BICG_P),
                                        phase_ndot(PH_INIT_R), phase_ndot(PH_CA_PS), phase_ndot(PH_QY), phase_ndot(PH_CA_XR),
@@ -565,7 +580,7 @@ extern "C" int bicg_debug_spmv_epi(bicg_matrix *m, int epi, double *vecs, double
     const size_t vb = (size_t)m->n_loc * sizeof(double);
     for (int id = 0; id < V_COUNT; ++id)
         BICG_CUDA(cudaMemcpyAsync(m->vec(id), vecs + (size_t)id * m->n_loc, vb, cudaMemcpyHostToDevice, c.stream));
-    reset_state_kernel<<<1, 1, 0, c.stream>>>(m->d_sc, c.cfg.tol, c.cfg.max_iter);
+    reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
     Seq seq(m);
     const double *Y = nullptr;
     int nd = 0;
