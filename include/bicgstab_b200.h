@@ -196,6 +196,17 @@ enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP =
 int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
                           bicg_stats *stats);
 
+/* out[j] = ||(A + sigma_j I) x_j - b|| / ||b||, j < sigma_len; x_set: sigma_len blocks of n_loc doubles, b: n_loc doubles, both
+ * host pointers, or device pointers when device_vectors != 0.  Collective over the ranks, which pass the same sigma_len: every rank
+ * returns -1 when any rank passed sigma_len <= 0 or a null pointer, or the ranks' sigma_len differ.  Any sigma_len > 0 works.
+ * One fused pass over the matrix serves a batch of shifts (csrc/shift_check.cu). */
+int bicg_shift_residuals(bicg_matrix *m, const double *x_set, const double *b, const double *sigma, int sigma_len,
+                         int device_vectors, double *out);
+/* With the option SHIFT_ERROR = 1 (BICG_SHIFT_ERROR; the reference's DISPLAY_ERROR) every shifted solver computes, after its timed
+ * region, the relative error above for each of its solutions, against the b it was given, and rank 0 prints it in the reference's
+ * format.  This returns those errors of the last shifted solve: sigma_len, or 0 if the option was off. */
+int bicg_last_shift_error(double *out, int cap);
+
 /* y_loc = A x_loc on a resident matrix (host pointers) -- the kernel behind MPI_csr_spmv_ovlap. */
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc);
 

@@ -1,6 +1,7 @@
 /*
- * compat/mpi.h -- the seven MPI calls the reference's main.c makes (main.c:14-28, 90-92, 150), mapped onto
- * libbicgstab_b200.so so that main.c compiles and links UNCHANGED on a box without MPI:
+ * compat/mpi.h -- the seven MPI calls the reference's main.c makes (main.c:14-28, 90-92, 150), plus the MPI_Allreduce of
+ * test_shifted.c's DISPLAY_ERROR check, mapped onto libbicgstab_b200.so so that main.c compiles and links UNCHANGED on a box
+ * without MPI:
  *
  *     gcc -O2 -Iinclude/compat -I<reference>/src <reference>/src/main.c -Lmpi-bicgstab_b200 -lbicgstab_b200 -o solver
  *
@@ -43,6 +44,7 @@ typedef struct { int MPI_SOURCE, MPI_TAG, MPI_ERROR; } MPI_Status;
 #define MPI_Wtime              bicg_shim_MPI_Wtime
 #define MPI_Gather             bicg_shim_MPI_Gather
 #define MPI_Barrier            bicg_shim_MPI_Barrier
+#define MPI_Allreduce          bicg_shim_MPI_Allreduce
 
 int    MPI_Init(int *argc, char ***argv);
 int    MPI_Finalize(void);
@@ -53,6 +55,9 @@ double MPI_Wtime(void);
 int    MPI_Gather(const void *sbuf, int scount, MPI_Datatype st, void *rbuf, int rcount, MPI_Datatype rt,
                   int root, MPI_Comm comm);
 int    MPI_Barrier(MPI_Comm comm);
+/* MPI_DOUBLE + MPI_SUM only (sendbuf may be MPI_IN_PLACE): the sums are added in rank order, so every rank gets the same
+ * bits.  The DISPLAY_ERROR block of test_shifted.c uses it.  Any other type or op: message + exit(1). */
+int    MPI_Allreduce(const void *sendbuf, void *recvbuf, int count, MPI_Datatype type, MPI_Op op, MPI_Comm comm);
 
 #ifdef __cplusplus
 }

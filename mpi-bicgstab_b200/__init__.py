@@ -10,6 +10,6 @@ from .api import *                                   # noqa: F401,F403
 from .api import (METHODS, GEN_KINDS, MatrixBlock, DeviceMatrix, blocks_from_csr, block_to_global_csr, gen_block,
                   load_matrix_block, plan_partition, spmv_ovlap, bicgstab, ca_bicgstab, pipe_bicgstab,
                   pipe_bicgstab_rr, solve, SHIFTED_METHODS, SHIFTED_SOLVE_EX, shifted_lopbicg_switching, shifted_lopbicg,
-                  shifted_lopbicgstab, shifted_pipe_lopbicgstab, last_shift_info, set_option, set_options, last_history, last_stats, comm_init,
+                  shifted_lopbicgstab, shifted_pipe_lopbicgstab, last_shift_info, last_shift_error, set_option, set_options, last_history, last_stats, comm_init,
                   comm_init_torch, comm_finalize)
 from ._lib import lib, CSR_Matrix, INFO_Matrix, bicg_stats, SYMBOLS, LIB_PATH

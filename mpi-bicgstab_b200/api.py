@@ -272,6 +272,14 @@ def last_shift_info(sigma_len):
     return seed.value, np.array(stop[:])
 
 
+def last_shift_error(sigma_len):
+    """||(A + sigma_j I) x_j - b|| / ||b|| of every shift of the last shifted solve run with the option shift_error=1
+    (BICG_SHIFT_ERROR); an empty array if it ran without it."""
+    out = np.zeros(max(int(sigma_len), 1))
+    n = lib.bicg_last_shift_error(out.ctypes.data_as(C.POINTER(C.c_double)), int(sigma_len))
+    return out[:min(n, int(sigma_len))]
+
+
 # ---- extensions ------------------------------------------------------------------------------------------
 def set_option(key, value):
     if lib.bicg_set_option(str(key).encode(), str(value).encode()) != 0:
@@ -319,6 +327,29 @@ class DeviceMatrix:
         st = bicg_stats()
         k = lib.bicg_shifted_solve_ex(self.h, SHIFTED_SOLVE_EX[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
         return k, _stats_dict(st)
+
+    def shift_residuals(self, x_set, b, sigma):
+        """bicg_shift_residuals: ||(A + sigma_j I) x_j - b|| / ||b|| for every row x_j of x_set (sigma_len, n_loc), computed on
+        the GPU in one fused pass.  x_set and b are both numpy float64 arrays or both CUDA float64 torch tensors (read in
+        place).  Collective over the ranks."""
+        sigma = np.ascontiguousarray(sigma, dtype=np.float64)
+        n, L = self.blk.n_loc, int(sigma.size)
+        out = np.empty(max(L, 1))
+        if isinstance(x_set, np.ndarray):
+            assert isinstance(b, np.ndarray)
+            xp, bp, dev = _vec(x_set, L * n), _vec(b, n), 0
+            assert x_set.size == L * n
+        else:
+            import torch
+            for t in (x_set, b):
+                assert t.is_cuda and t.dtype == torch.float64 and t.is_contiguous(), "need contiguous CUDA float64 tensors"
+            assert x_set.numel() == L * n and b.numel() >= n
+            xp, bp, dev = C.c_void_p(x_set.data_ptr()), C.c_void_p(b.data_ptr()), 1
+            torch.cuda.current_stream().synchronize()       # the library reads them on its own stream
+        rc = lib.bicg_shift_residuals(self.h, xp, bp, _dptr(sigma), L, dev, out.ctypes.data_as(C.POINTER(C.c_double)))
+        if rc != 0:
+            raise ValueError(f"bicg_shift_residuals failed with {rc}")
+        return out[:L]
 
     def spmv(self, x_loc):
         y = np.empty(self.blk.n_loc)

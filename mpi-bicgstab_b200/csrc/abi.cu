@@ -231,6 +231,39 @@ int bicg_last_shift_info(int *seed, int *stop_iter, int cap)
     for (int i = 0; i < n && i < cap; ++i) stop_iter[i] = c.last_shift_stop[(size_t)i];
     return n;
 }
+int bicg_last_shift_error(double *out, int cap)
+{
+    Context &c = ctx();
+    const int n = (int)c.last_shift_err.size();
+    for (int i = 0; i < n && i < cap; ++i) out[i] = c.last_shift_err[(size_t)i];
+    return n;
+}
+int bicg_shift_residuals(bicg_matrix *m, const double *x_set, const double *b, const double *sigma, int sigma_len, int device_vectors,
+                         double *out)
+{
+    Context &c = ctx();
+    // collective: a rank with bad arguments must not leave the others waiting for it in the residual pass, so every rank
+    // learns every rank's verdict (and sigma_len, which must agree) before any of them starts
+    struct Args { int bad, len; } mine{sigma_len <= 0 || !m || !x_set || !b || !sigma || !out, sigma_len};
+    std::vector<Args> all((size_t)c.world);
+    c.host_allgather(&mine, all.data(), sizeof(Args));
+    for (const Args &a : all)
+        if (a.bad || a.len != sigma_len) return -1;
+    c.ensure();
+    const size_t n = (size_t)m->n_loc;
+    const double *dx = x_set, *db = b;
+    double *tmp = nullptr;
+    if (!device_vectors) {
+        tmp = (double *)c.dev_alloc(((size_t)sigma_len + 1) * n * sizeof(double));
+        BICG_CUDA(cudaMemcpyAsync(tmp, x_set, (size_t)sigma_len * n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+        BICG_CUDA(cudaMemcpyAsync(tmp + (size_t)sigma_len * n, b, n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+        dx = tmp; db = tmp + (size_t)sigma_len * n;
+    }
+    const std::vector<double> err = shift_relative_errors(m, dx, (long long)n, db, sigma, sigma_len);
+    if (tmp) c.dev_free(tmp);
+    for (int j = 0; j < sigma_len; ++j) out[j] = err[(size_t)j];
+    return 0;
+}
 int bicg_spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes) { return spmv_time(m, reps, ms, bytes); }
 
 int bicg_last_history(double *out, int cap)

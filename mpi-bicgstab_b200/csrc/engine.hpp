@@ -55,6 +55,7 @@ struct Config {
     int verbose = 0;
     double shift_tol = 1.0e-12;  // EPS of the shifted solvers (shifted_switching_solver.c:5)
     int shift_max_iter = 1000;   // their MAX_ITER (:6)
+    int shift_error = 0;         // 1: after a shifted solve, the relative error of every shift (their DISPLAY_ERROR, :17)
     int peer_timeout_s = 20;     // bound of device-side waits for peers / other CTAs (then: error + exit(1))
     int fence_writers = 0;       // 1: every thread that stored to a peer also fences at system scope itself (debug aid;
                                  // the CTA barrier + one system fence per CTA is sufficient and much cheaper)
@@ -87,6 +88,7 @@ struct Context {
     bicg_stats last_stats{};
     std::vector<int> last_shift_stop;     // shifted solver: iteration at which every shift stopped
     int last_shift_seed = 0;              // ... and the seed it ended with
+    std::vector<double> last_shift_err;   // BICG_SHIFT_ERROR: ||(A + sigma_j I) x_j - b|| / ||b|| of the last shifted solve
     // host-pointer keyed cache of uploaded matrices
     std::map<const void *, bicg_matrix *> cache;
     std::map<TuneKey, TuneVal> tuned;     // SpMV autotune winners by matrix shape
@@ -245,6 +247,11 @@ void run_batches(int max_iter, int U, int depth, const int *d_done, const std::f
 // the iterations performed), -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len)
 int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
                    int max_iter);
+// shift_check.cu, collective: x_j = d_x + j ldx (own rows, device), d_b (device), sigma (host) -> sum_i ((A + sigma_j I) x_j - b)_i^2
+// for j < L and sum_i b_i^2 last (L + 1 values, over every rank, added in rank order); enqueued on the stream, synchronises
+std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
+// ... as ||(A + sigma_j I) x_j - b|| / ||b||
+std::vector<double> shift_relative_errors(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, int prof_class = 0);
@@ -268,9 +275,10 @@ struct PhaseLauncher {
     explicit PhaseLauncher(bicg_matrix *mm) : m(mm), c(ctx()) {}
     VecPtrs ptrs() const;
     KernelCommon common(TailDesc tail) const;
-    PushDesc make_push(int id) const;
+    // the boundary runs of arena vector `id` into its ghost slots on the peers; push_src: take the values from there instead
+    PushDesc make_push(int id, const double *push_src = nullptr) const;
     // one fused vector kernel; push_vec >= 0: that vector is the next SpMV's input (PH_PUSH: the push alone)
-    void vec(int phase, TailDesc tail, int push_vec = -1);
+    void vec(int phase, TailDesc tail, int push_vec = -1, const double *push_src = nullptr);
     // y = A x (+ sigma x) with ndot (0..4) epilogue dots (a_k, b_k); a null b_k is the y just computed
     void spmv(int x_id, int y_id, TailDesc tail, int ndot = 0, const double *a0 = nullptr, const double *b0 = nullptr,
               const double *a1 = nullptr, const double *b1 = nullptr, const double *a2 = nullptr, const double *b2 = nullptr,

@@ -65,6 +65,7 @@ int set_option(Config &c, const char *key, const char *value)
     else if (k == "PEER_TIMEOUT_S") c.peer_timeout_s = std::max(1, as_int());
     else if (k == "SHIFT_TOL") c.shift_tol = atof(value);
     else if (k == "SHIFT_MAX_ITER") c.shift_max_iter = std::max(1, as_int());
+    else if (k == "SHIFT_ERROR") c.shift_error = as_int();
     else if (k == "FENCE_WRITERS") c.fence_writers = as_int();
     else return -1;
     return 0;
@@ -75,7 +76,8 @@ void load_config_from_env(Config &c)
     static const char *keys[] = {"BICG_TOL", "BICG_MAX_ITER", "BICG_OUT_ITER", "BICG_QUIET", "BICG_SPMV",
                                  "BICG_SPMV_LANES", "BICG_SPMV_THREADS", "BICG_SPMV_STAGES", "BICG_SPMV_CTAS",
                                  "BICG_AUTOTUNE", "BICG_GRAPH", "BICG_UNROLL", "BICG_CACHE", "BICG_MEGA", "BICG_MEGA_THREADS", "BICG_MEGA_TRACE", "BICG_MEGA_LANES", "BICG_L2_HINT", "BICG_GATHER_CG", "BICG_RESIDENT", "BICG_STAGE_UPLOAD", "BICG_BOUNDARY_WEIGHT", "BICG_ROW_WEIGHT", "BICG_DEVICE",
-                                 "BICG_HALO_GAP", "BICG_VERBOSE", "BICG_PEER_TIMEOUT_S", "BICG_SHIFT_TOL", "BICG_SHIFT_MAX_ITER", "BICG_FENCE_WRITERS"};
+                                 "BICG_HALO_GAP", "BICG_VERBOSE", "BICG_PEER_TIMEOUT_S", "BICG_SHIFT_TOL", "BICG_SHIFT_MAX_ITER", "BICG_FENCE_WRITERS",
+                                 "BICG_SHIFT_ERROR"};
     for (const char *k : keys)
         if (const char *v = getenv(k)) set_option(c, k, v);
 }

@@ -427,6 +427,7 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
         printf("Total iter   : %d\n", k - 1);
         print_times(s.ms * 1e-3, k);
     }
+    s.report_error(sigma, out.seed);
     return fixed ? k - 1 : k;                                                         // :255 / :600
 }
 

@@ -388,6 +388,7 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
         printf("Final r      : %e\n", res);
         print_times(s.ms * 1e-3, k);
     }
+    s.report_error(sigma, seed);
     return k;                                                                         // :352 / :894
 }
 

@@ -25,6 +25,7 @@ struct ShiftedSolve {
     const int n, L;
     const long long stride;                  // doubles between consecutive shifts in x_set / p_set (16-byte aligned blocks)
     double *d_x = nullptr;                   // [L][stride] the solutions x_j
+    double *d_b = nullptr;                   // BICG_SHIFT_ERROR only: the caller's b
     float ms = 0.f;                          // length of the timed region
     int launches0 = 0;
     std::vector<void *> owned;
@@ -48,6 +49,10 @@ struct ShiftedSolve {
         BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
                                     cudaMemcpyHostToDevice, c.stream));
         BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+        if (c.cfg.shift_error) {
+            d_b = alloc<double>(n);
+            BICG_CUDA(cudaMemcpyAsync(d_b, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
+        }
         reset_scalars(m, 0.0, 0);
     }
     // the reference's timed region: run.prologue(), then batches of U run.iteration() until the device raises *d_done
@@ -84,6 +89,26 @@ struct ShiftedSolve {
         st.kernel_launches = c.launches - launches0;
         st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
         return st;
+    }
+    // The last step of every shifted solver, after its own printout: with BICG_SHIFT_ERROR, the relative error
+    // ||(A + sigma_j I) x_j - b|| / ||b|| of every shift from d_x (collective), kept for bicg_last_shift_error and printed by
+    // rank 0 as the reference's DISPLAY_ERROR block does (shifted_switching_solver.c:570-598), `seed` being the seed the solve
+    // ended with.  The reference measures against (A + sigma_seed I) 1, the b its drivers build; this is the b passed in.
+    // It runs after finish() and after the solver took stats(): d_x lives until the ShiftedSolve is destroyed, the host x_set
+    // is already a copy of it, and the check's launches and time stay out of kernel_launches and loop_ms, like the reference's
+    // check, which runs after its timed region.
+    void report_error(const double *sigma, int seed)
+    {
+        c.last_shift_err.clear();
+        if (!d_b) return;
+        c.last_shift_err = shift_relative_errors(m, d_x, stride, d_b, sigma, L);
+        if (c.rank != 0 || c.cfg.quiet) return;
+        printf("seed(0:seed, 1:shift), sigma, relative error\n");                  // :572
+        for (int i = 0; i < L; ++i) {
+            if (i == seed) printf("0, %e, %e\n", sigma[i], c.last_shift_err[(size_t)i]);               // :593
+            else if (i % 10 == 0) printf("1, %e, %e\n", sigma[i], c.last_shift_err[(size_t)i]);        // :594
+        }
+        fflush(stdout);
     }
 
 private:

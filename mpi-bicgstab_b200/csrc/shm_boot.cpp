@@ -223,5 +223,29 @@ int bicg_shim_MPI_Gather(const void *sbuf, int scount, int st, void *rbuf, int, 
     free(tmp);
     return rc;
 }
+int bicg_shim_MPI_Allreduce(const void *sbuf, void *rbuf, int count, int type, int op, int)
+{
+    if (type != 1 || op != 1) {                                 // MPI_DOUBLE / MPI_SUM of compat/mpi.h
+        fprintf(stderr, "bicgstab_b200: MPI_Allreduce supports MPI_DOUBLE with MPI_SUM only (got type %d, op %d)\n", type, op);
+        exit(1);
+    }
+    if (count <= 0) return 0;
+    const size_t bytes = (size_t)count * sizeof(double);
+    const void *src = (sbuf == (const void *)-1) ? rbuf : sbuf;    // MPI_IN_PLACE
+    const int world = bicg_comm_world();
+    if (world == 1) { if (src != rbuf) memcpy(rbuf, src, bytes); return 0; }
+    double *all = (double *)malloc(bytes * (size_t)world);
+    const int rc = shm_allgather(nullptr, src, all, bytes);
+    if (rc == 0) {
+        double *out = (double *)rbuf;
+        for (int i = 0; i < count; ++i) {
+            double s = all[i];
+            for (int p = 1; p < world; ++p) s += all[(size_t)p * count + i];
+            out[i] = s;
+        }
+    }
+    free(all);
+    return rc;
+}
 
 } // extern "C"

@@ -66,13 +66,13 @@ KernelCommon PhaseLauncher::common(TailDesc tail) const
 }
 
 // where the runs of vector `id` that peers need go: their ghost slots, addressed through the IPC mappings
-PushDesc PhaseLauncher::make_push(int id) const
+PushDesc PhaseLauncher::make_push(int id, const double *push_src) const
 {
     PushDesc pd{};
     if (m->world == 1) return pd;
     pd.npeers = m->npush;
     pd.fence_writers = c.cfg.fence_writers;
-    pd.src = m->vec(id);
+    pd.src = push_src ? push_src : m->vec(id);
     for (int s = 0; s < m->npush; ++s) {
         const int d = m->push_peer[s];
         pd.dst[s] = (double *)((char *)m->peer_base[d] + m->peer_vec_off[d]) + (long long)id * m->peer_vstride[d] +
@@ -83,7 +83,7 @@ PushDesc PhaseLauncher::make_push(int id) const
     return pd;
 }
 
-void PhaseLauncher::vec(int phase, TailDesc tail, int push_vec)
+void PhaseLauncher::vec(int phase, TailDesc tail, int push_vec, const double *push_src)
 {
     VecArgs a{};
     a.kc = common(tail);
@@ -91,7 +91,7 @@ void PhaseLauncher::vec(int phase, TailDesc tail, int push_vec)
     a.push.npeers = 0; a.push.src = nullptr;
     if (push_vec >= 0 && m->world > 1) {
         a.kc.tail.signal_halo = 1;               // every rank advances its halo epoch, senders also signal
-        a.push = make_push(push_vec);
+        a.push = make_push(push_vec, push_src);
     } else if (phase == PH_PUSH) {
         return;                                   // single rank: nothing to exchange
     }
