@@ -195,6 +195,15 @@ int bicg_last_shift_info(int *seed, int *stop_iter, int cap);
 enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP = 2, BICG_SHIFTED_LOPBICG = 3 };
 int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
                           bicg_stats *stats);
+/* bicg_shifted_solve_ex on DEVICE memory: x_set is sigma_len contiguous blocks of n_loc doubles (initial guesses in, solutions
+ * out, updated in place; no padding or alignment required), r is n_loc doubles (b in, seed residual out). sigma stays a host
+ * array. Same methods, return values, stdout, statistics, bicg_last_* results and BICG_SHIFT_ERROR report as
+ * bicg_shifted_solve_ex, except that h2d_bytes and d2h_bytes are 0: x_set is never copied and no second copy of it is
+ * allocated. Returns once the library's stream has synchronised, with the results in the caller's buffers. Collective:
+ * every rank returns -1 if any rank passed a null pointer, an unknown method, sigma_len <= 0 or a seed outside
+ * [0, sigma_len), or if the ranks disagree on method, sigma_len or seed. */
+int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                           bicg_stats *stats);
 
 /* out[j] = ||(A + sigma_j I) x_j - b|| / ||b||, j < sigma_len; x_set: sigma_len blocks of n_loc doubles, b: n_loc doubles, both
  * host pointers, or device pointers when device_vectors != 0.  Collective over the ranks, which pass the same sigma_len: every rank

@@ -72,6 +72,7 @@ SYMBOLS = {
     "bicg_shifted_solve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_last_shift_info": (C.c_int, [_P(C.c_int), _P(C.c_int), C.c_int]),
     "bicg_shifted_solve_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
+    "bicg_shifted_solve_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_shift_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(C.c_double)]),
     "bicg_last_shift_error": (C.c_int, [_P(C.c_double), C.c_int]),
     "bicg_spmv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -265,6 +265,36 @@ def shifted_pipe_lopbicgstab(blk, x_set, r_loc, sigma, seed):
                                         int(seed))
 
 
+def _cuda_vectors(*args):
+    """Device pointers of CUDA float64 torch tensors, given as (name, tensor, expected shape) triples.  Everything the library
+    cannot check itself is checked here, before it is called: all are torch tensors, float64, contiguous, of the expected shape,
+    on the library's GPU.  Then torch's current stream is synchronised, because the library works on its own stream."""
+    import torch
+    checks = [(lambda t, s: isinstance(t, torch.Tensor), TypeError,
+               lambda t, s: f"numpy arrays and torch tensors cannot be mixed in one call (got {type(t).__name__})"),
+              (lambda t, s: t.dtype == torch.float64, TypeError, lambda t, s: f"need a float64 tensor, got {t.dtype}"),
+              (lambda t, s: t.is_contiguous(), ValueError, lambda t, s: "need a contiguous tensor"),
+              (lambda t, s: tuple(t.shape) == tuple(s), ValueError, lambda t, s: f"shape {tuple(t.shape)}, expected {tuple(s)}"),
+              (lambda t, s: t.is_cuda, TypeError, lambda t, s: f"need a CUDA tensor, got one on {t.device}")]
+    for ok, exc, msg in checks:              # each check over every argument before the next one
+        for name, t, shape in args:
+            if not ok(t, shape):
+                raise exc(f"{name}: {msg(t, shape)}")
+    dev = lib.bicg_device()
+    for name, t, _ in args:
+        if t.device.index != dev:
+            raise ValueError(f"{name}: tensor on {t.device}, the library runs on cuda:{dev}")
+    torch.cuda.current_stream(args[0][1].device).synchronize()
+    return [C.c_void_p(t.data_ptr()) for _, t, _ in args]
+
+
+def _host_sigma(sigma):
+    """sigma as a contiguous float64 numpy array; a torch tensor (on any device) is copied to the host."""
+    if not isinstance(sigma, np.ndarray) and hasattr(sigma, "detach"):
+        sigma = sigma.detach().cpu().numpy()
+    return np.ascontiguousarray(sigma, dtype=np.float64)
+
+
 def last_shift_info(sigma_len):
     seed = C.c_int()
     stop = (C.c_int * sigma_len)()
@@ -317,15 +347,32 @@ class DeviceMatrix:
             raise RuntimeError("bicg_matrix_create failed")
 
     def solve(self, method, x, r, krr=0, nrr=0):
+        """bicg_solve: x (initial guess in, solution out) and r (b in, final residual out) are both numpy float64 arrays, or both
+        contiguous CUDA float64 torch tensors of shape (n_loc,), which are updated in place.  Returns (iterations, stats)."""
+        n = self.blk.n_loc
+        if isinstance(x, np.ndarray) and isinstance(r, np.ndarray):
+            xp, rp, dev = _vec(x, n), _vec(r, n), 0
+        else:
+            (xp, rp), dev = _cuda_vectors(("x", x, (n,)), ("r", r, (n,))), 1
         st = bicg_stats()
-        it = lib.bicg_solve(self.h, METHODS[method], _vec(x, self.blk.n_loc), _vec(r, self.blk.n_loc), krr, nrr, 0, C.byref(st))
+        it = lib.bicg_solve(self.h, METHODS[method], xp, rp, krr, nrr, dev, C.byref(st))
         return it, _stats_dict(st)
 
     def shifted_solve(self, method, x_set, r, sigma, seed):
-        """bicg_shifted_solve_ex: method is a key of SHIFTED_SOLVE_EX; returns (that solver's return value, stats)."""
-        xp, rp, sigma = _shifted_args(self.blk, x_set, r, sigma)
+        """bicg_shifted_solve_ex: method is a key of SHIFTED_SOLVE_EX; returns (that solver's return value, stats).  x_set
+        (sigma_len, n_loc) and r (n_loc) are both numpy float64 arrays, or both contiguous CUDA float64 torch tensors, which go
+        through bicg_shifted_solve_dev and are updated in place (a view at any element offset works).  sigma: numpy array or
+        tensor (copied to the host)."""
         st = bicg_stats()
-        k = lib.bicg_shifted_solve_ex(self.h, SHIFTED_SOLVE_EX[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
+        if isinstance(x_set, np.ndarray) and isinstance(r, np.ndarray):
+            xp, rp, sigma = _shifted_args(self.blk, x_set, r, _host_sigma(sigma))
+            fn = lib.bicg_shifted_solve_ex
+        else:
+            sigma = _host_sigma(sigma)
+            n = self.blk.n_loc
+            xp, rp = _cuda_vectors(("x_set", x_set, (sigma.size, n)), ("r", r, (n,)))
+            fn = lib.bicg_shifted_solve_dev
+        k = fn(self.h, SHIFTED_SOLVE_EX[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
         return k, _stats_dict(st)
 
     def shift_residuals(self, x_set, b, sigma):

@@ -223,6 +223,25 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
     if (stats) *stats = c.last_stats;
     return k;
 }
+int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                           bicg_stats *stats)
+{
+    Context &c = ctx();
+    // collective: a rank with bad arguments must not leave the others waiting for it in the solve's halo exchanges and
+    // reductions, so every rank learns every rank's verdict, method, sigma_len and seed before any of them starts
+    const bool known = method == BICG_SHIFTED_SWITCHING || method == BICG_SHIFTED_LOP || method == BICG_SHIFTED_PIPE_LOP ||
+                       method == BICG_SHIFTED_LOPBICG;
+    struct Args { int bad, method, len, seed; } mine{!m || !x_set || !r || !sigma || !known || sigma_len <= 0 || seed < 0 ||
+                                                     seed >= sigma_len, method, sigma_len, seed};
+    std::vector<Args> all((size_t)c.world);
+    c.host_allgather(&mine, all.data(), sizeof(Args));
+    for (const Args &a : all)
+        if (a.bad || a.method != method || a.len != sigma_len || a.seed != seed) return -1;
+    c.ensure();
+    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, true);
+    if (stats) *stats = c.last_stats;
+    return k;
+}
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap)
 {
     Context &c = ctx();

@@ -244,9 +244,10 @@ void reset_scalars(bicg_matrix *m, double tol, int max_iter);   // Scalars of a 
 // stops once the flag was raised by its end.  The loop test runs on the device, which returns from every kernel after it.
 void run_batches(int max_iter, int U, int depth, const int *d_done, const std::function<void(int)> &enqueue_batch);
 // shifted.cu: method = BICG_SHIFTED_*; returns what that solver returns (shifted_lopbicg_switching: iterations + 1, the others:
-// the iterations performed), -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len)
+// the iterations performed), -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len).  dev: x_set (sigma_len
+// blocks of n_loc, any 8-byte alignment) and r are device pointers, updated in place; sigma is always a host array.
 int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
-                   int max_iter);
+                   int max_iter, bool dev = false);
 // shift_check.cu, collective: x_j = d_x + j ldx (own rows, device), d_b (device), sigma (host) -> sum_i ((A + sigma_j I) x_j - b)_i^2
 // for j < L and sum_i b_i^2 last (L + 1 values, over every rank, added in rank order); enqueued on the stream, synchronises
 std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);

@@ -200,7 +200,8 @@ struct ShVec {
     const ShiftDev *sd;
     double *r, *rh, *p, *s, *y, *qc, *rold;      // arena vectors (own parts)
     double *x_set, *p_set;
-    long long stride;                            // doubles between consecutive shifts in x_set / p_set
+    long long xstride;                           // doubles between consecutive shifts in x_set (blocks may be misaligned)
+    long long stride;                            // ... in p_set (even: every block starts 16-byte aligned)
     int n, L;
 };
 
@@ -235,7 +236,7 @@ __global__ void __launch_bounds__(256) sh_vec_xr(const __grid_constant__ ShVec a
     if (a.sd->done) return;
     __shared__ double scratch[32 * MAX_DOTS];
     const double al = a.kc.sc->alpha, om = a.kc.sc->omega;
-    double *x = a.x_set + (size_t)a.sd->seed * a.stride;
+    double *x = a.x_set + (size_t)a.sd->seed * a.xstride;
     double dot[2] = {0.0, 0.0};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
         const double q = a.r[i];
@@ -251,6 +252,11 @@ __global__ void __launch_bounds__(256) sh_vec_xr(const __grid_constant__ ShVec a
 }
 // all active shifts at once                                                                            :435-445
 //   x_j += c1 q + alpha_j p_j ;  p_j += c2 q + c3 r_old ;  p_j = beta_j p_j + c4 r
+// Two rows per thread.  p_j moves as one 16-byte access; so does x_j when its block starts 16-byte aligned.  A caller's
+// device x_set has blocks of n doubles from any 8-byte aligned base, so a block may not be: then x_j moves as two 8-byte
+// accesses.  i is even, so the choice depends on the shift alone and is the same for the whole warp.  XA: the host found
+// every block aligned (always so for a host x_set) and the test is compiled out.
+template <bool XA>
 __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVec a)
 {
     const ShiftDev *sd = a.sd;
@@ -262,25 +268,29 @@ __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVe
     for (int t = threadIdx.x; t < na; t += blockDim.x) s_idx[t] = sd->active[t];
     __syncthreads();
     for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
-        const bool two = i + 1 < a.n;                        // stride is even and every block starts 16-byte aligned
+        const bool two = i + 1 < a.n;
         double q0 = a.qc[i], q1 = two ? a.qc[i + 1] : 0.0;
         double o0 = a.rold[i], o1 = two ? a.rold[i + 1] : 0.0;
         double r0 = a.r[i], r1 = two ? a.r[i + 1] : 0.0;
 #pragma unroll 2
         for (int t = 0; t < na; ++t) {
             const double *c = s_coef + (size_t)t * SH_COEF;
-            double *xj = a.x_set + (size_t)s_idx[t] * a.stride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
+            double *xj = a.x_set + (size_t)s_idx[t] * a.xstride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
+            const bool xa = XA || (reinterpret_cast<size_t>(xj) & 15) == 0;
             double x0, x1, p0, p1;
             if (two) {
-                const double2 xv = *reinterpret_cast<const double2 *>(xj), pv = *reinterpret_cast<const double2 *>(pj);
-                x0 = xv.x; x1 = xv.y; p0 = pv.x; p1 = pv.y;
+                const double2 pv = *reinterpret_cast<const double2 *>(pj);
+                p0 = pv.x; p1 = pv.y;
+                if (xa) { const double2 xv = *reinterpret_cast<const double2 *>(xj); x0 = xv.x; x1 = xv.y; }
+                else { x0 = xj[0]; x1 = xj[1]; }
             } else { x0 = xj[0]; p0 = pj[0]; x1 = p1 = 0.0; }
             x0 = fma(c[0], q0, x0); x0 = fma(c[1], p0, x0);
             x1 = fma(c[0], q1, x1); x1 = fma(c[1], p1, x1);
             p0 = fma(c[2], q0, p0); p0 = fma(c[3], o0, p0); p0 = c[4] * p0; p0 = fma(c[5], r0, p0);
             p1 = fma(c[2], q1, p1); p1 = fma(c[3], o1, p1); p1 = c[4] * p1; p1 = fma(c[5], r1, p1);
             if (two) {
-                *reinterpret_cast<double2 *>(xj) = make_double2(x0, x1);
+                if (xa) *reinterpret_cast<double2 *>(xj) = make_double2(x0, x1);
+                else { xj[0] = x0; xj[1] = x1; }
                 *reinterpret_cast<double2 *>(pj) = make_double2(p0, p1);
             } else { xj[0] = x0; pj[0] = p0; }
         }
@@ -313,6 +323,7 @@ __global__ void __launch_bounds__(256) sh_vec_p(const __grid_constant__ ShVec a)
 struct ShRun : PhaseLauncher {
     ShiftDev *d_sd = nullptr;
     ShVec base{};
+    bool xa = true;                                  // every x_j block 16-byte aligned: sh_vec_shift<true>
     using PhaseLauncher::PhaseLauncher;
 
     ShVec vargs(TailDesc tail) const
@@ -341,7 +352,9 @@ struct ShRun : PhaseLauncher {
         sh_vec_xr<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));                     // x[seed], r, (r,r), (r#,r)   :411-416
         sh_scalar_iter<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                       // beta ... loop test          :420, 429-537
         const size_t smem = (size_t)base.L * (SH_COEF * sizeof(double) + sizeof(int));
-        sh_vec_shift<<<std::max(1, std::min(c.sm_count * 8, (m->n_loc + 511) / 512)), 256, smem, c.stream>>>(vargs(tail_none()));
+        const int sgrid = std::max(1, std::min(c.sm_count * 8, (m->n_loc + 511) / 512));
+        if (xa) sh_vec_shift<true><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
+        else sh_vec_shift<false><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
         sh_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // p[seed] (or the switch)     :421-423 / :499
         vec(PH_PUSH, tail_none(), V_P);
         c.launches += 7;
@@ -351,9 +364,9 @@ struct ShRun : PhaseLauncher {
 } // namespace
 
 int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
-                    int max_iter_opt)
+                    int max_iter_opt, bool dev)
 {
-    ShiftedSolve s(m, L);
+    ShiftedSolve s(m, L, dev);
     Context &c = s.c;
     const int n = s.n;
     const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
@@ -388,9 +401,14 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);
-    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.stride = s.stride; run.base.n = n; run.base.L = L;
+    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
+    run.base.n = n; run.base.L = L;
+    run.xa = s.x_aligned();
     const size_t smem = (size_t)L * (SH_COEF * sizeof(double) + sizeof(int));
-    if (smem > 48 * 1024) BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    if (smem > 48 * 1024) {
+        BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    }
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :364
     const ShiftDev out = s.finish(x_set, r, d_sd);
@@ -432,15 +450,16 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
 }
 
 // the one mapping from a BICG_SHIFTED_* method to its solver
-int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter)
+int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
+                  bool dev)
 {
     ctx().ensure();
     if (L <= 0 || seed < 0 || seed >= L) return -1;
     switch (method) {
-    case BICG_SHIFTED_SWITCHING: return switching_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter);
-    case BICG_SHIFTED_LOPBICG:   return switching_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter);
-    case BICG_SHIFTED_LOP:       return lop_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter);
-    case BICG_SHIFTED_PIPE_LOP:  return lop_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter);
+    case BICG_SHIFTED_SWITCHING: return switching_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter, dev);
+    case BICG_SHIFTED_LOPBICG:   return switching_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);
+    case BICG_SHIFTED_LOP:       return lop_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter, dev);
+    case BICG_SHIFTED_PIPE_LOP:  return lop_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);
     default: return -1;
     }
 }

@@ -133,7 +133,8 @@ struct LopVec {
     const LopDev *sd;
     double *r, *rh, *p, *s, *y, *z, *w, *v, *t, *rold;  // arena vectors (own parts); y, z, w, v, t as the algorithm uses them
     double *x_set, *p_set;
-    long long stride;                                   // doubles between consecutive shifts in x_set / p_set
+    long long xstride;                                  // doubles between consecutive shifts in x_set (blocks may be misaligned)
+    long long stride;                                   // ... in p_set (even: every block starts 16-byte aligned)
     int n, L;
 };
 
@@ -147,6 +148,19 @@ __device__ __forceinline__ void st2(double *p, int i, bool two, const double (&v
     if (two) *reinterpret_cast<double2 *>(p + i) = make_double2(v[0], v[1]);
     else p[i] = v[0];
 }
+// the same for a block of x_set, which starts 16-byte aligned (al) or only 8-byte aligned: a caller's device x_set has blocks of
+// n doubles from any 8-byte aligned base; then the pair moves as two 8-byte accesses
+__device__ __forceinline__ void ld2x(const double *p, int i, bool two, bool al, double (&v)[2])
+{
+    if (two && !al) { v[0] = p[i]; v[1] = p[i + 1]; }
+    else ld2(p, i, two, v);
+}
+__device__ __forceinline__ void st2x(double *p, int i, bool two, bool al, const double (&v)[2])
+{
+    if (two && !al) { p[i] = v[0]; p[i + 1] = v[1]; }
+    else st2(p, i, two, v);
+}
+__device__ __forceinline__ bool aligned16(const double *p) { return (reinterpret_cast<size_t>(p) & 15) == 0; }
 
 // r# = r, p[seed] = r, (r,r); PIPE-LOP also zeroes s, z, v (pinned, see the top)          :240-252 / :763, 772-782
 __global__ void __launch_bounds__(256) lop_vec_init(const __grid_constant__ LopVec a, int pipe)
@@ -203,13 +217,15 @@ __global__ void __launch_bounds__(256) lop_vec_pipe1(const __grid_constant__ Lop
     block_sum<2>(dot, scratch);
     kernel_tail<2>(a.kc, dot, scratch);
 }
-// The seed's x and residual and every shift's x_j, p_j in one pass over the rows (two rows per thread, 16-byte accesses).
+// The seed's x and residual and every shift's x_j, p_j in one pass over the rows (two rows per thread, 16-byte accesses; an
+// x_set block that does not start 16-byte aligned takes two 8-byte accesses instead -- i is even, so that choice depends on
+// the shift alone and is the same for the whole warp; XA: the host found every block aligned and the test is compiled out).
 //   seed   x[seed] += alpha p + omega q; r = q - omega y                                   :294-295, 305 / :830-831, 841
 //          PIPE-LOP: w = y - omega (t - alpha v)                                          :843-844
 //   shifts p_j = beta_j p_j + c4 r_old; x_j += c1 q + alpha_j p_j; p_j += c2 q + c3 r_old   :267-268, 299-302 / :807-808, 835-838
 //   dots   LOP (r,r), (r#,r)                                                               :306, 308
 //          PIPE-LOP (r,r), (r#,r), (r#,w), (r#,s), (r#,z)                                  :842, 846-849
-template <bool PIPE>
+template <bool PIPE, bool XA>
 __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ LopVec a)
 {
     const LopDev *sd = a.sd;
@@ -221,7 +237,8 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
     for (int t = threadIdx.x; t < na * LOP_COEF; t += blockDim.x) s_coef[t] = sd->coef[t];
     __syncthreads();
     const double al = sd->alpha, om = sd->omega;
-    double *xs = a.x_set + (size_t)seed * a.stride;
+    double *xs = a.x_set + (size_t)seed * a.xstride;
+    const bool xs_al = XA || aligned16(xs);
     double dot[ND];
 #pragma unroll
     for (int d = 0; d < ND; ++d) dot[d] = 0.0;
@@ -229,7 +246,7 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
         const bool two = i + 1 < a.n;                   // stride and arena vectors are 16-byte aligned, i is even
         const int ne = two ? 2 : 1;
         double q[2], o[2], x[2], p[2], y[2], r[2], rh[2];
-        ld2(a.r, i, two, q); ld2(a.rold, i, two, o); ld2(xs, i, two, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
+        ld2(a.r, i, two, q); ld2(a.rold, i, two, o); ld2x(xs, i, two, xs_al, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
         ld2(PIPE ? a.w : a.y, i, two, y);
         for (int e = 0; e < ne; ++e) {
             x[e] = fma(al, p[e], x[e]);
@@ -238,7 +255,7 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
             dot[0] = fma(r[e], r[e], dot[0]);
             dot[1] = fma(rh[e], r[e], dot[1]);
         }
-        st2(xs, i, two, x); st2(a.r, i, two, r);
+        st2x(xs, i, two, xs_al, x); st2(a.r, i, two, r);
         if constexpr (PIPE) {
             double t[2], v[2], w[2], s[2], z[2];
             ld2(a.t, i, two, t); ld2(a.v, i, two, v); ld2(a.s, i, two, s); ld2(a.z, i, two, z);
@@ -256,16 +273,17 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
         for (int t = 0; t < na; ++t) {
             const double *c = s_coef + (size_t)t * LOP_COEF;
             const size_t j = (size_t)(t < seed ? t : t + 1);
-            double *xj = a.x_set + j * a.stride + i, *pj = a.p_set + j * a.stride + i;
+            double *xj = a.x_set + j * a.xstride + i, *pj = a.p_set + j * a.stride + i;
+            const bool xa = XA || aligned16(xj);
             double xv[2], pv[2];
-            ld2(xj, 0, two, xv); ld2(pj, 0, two, pv);
+            ld2x(xj, 0, two, xa, xv); ld2(pj, 0, two, pv);
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 pv[e] = c[0] * pv[e]; pv[e] = fma(c[1], o[e], pv[e]);
                 xv[e] = fma(c[2], q[e], xv[e]); xv[e] = fma(c[3], pv[e], xv[e]);
                 pv[e] = fma(c[4], q[e], pv[e]); pv[e] = fma(c[5], o[e], pv[e]);
             }
-            st2(xj, 0, two, xv); st2(pj, 0, two, pv);
+            st2x(xj, 0, two, xa, xv); st2(pj, 0, two, pv);
         }
     }
     block_sum<ND>(dot, scratch);
@@ -276,6 +294,7 @@ struct LopRun : PhaseLauncher {
     LopDev *d_sd = nullptr;
     LopVec base{};
     bool pipe = false;
+    bool xa = true;                                     // every x_j block 16-byte aligned: lop_vec_update<PIPE, true>
     int ugrid = 1;                                      // grid of lop_vec_update
     size_t smem = 0;                                    // its coefficient table
     using PhaseLauncher::PhaseLauncher;
@@ -310,7 +329,8 @@ struct LopRun : PhaseLauncher {
             vec(PH_PUSH, tail_none(), V_R);
             spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);   // y = (A + sigma I) q, (q,q), (q,y)  :278-282
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
-            lop_vec_update<false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            if (xa) lop_vec_update<false, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            else lop_vec_update<false, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
             lop_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // p[seed]                      :319-321
             vec(PH_PUSH, tail_none(), V_P);
@@ -320,7 +340,8 @@ struct LopRun : PhaseLauncher {
             vec(PH_PUSH, tail_none(), V_Z);
             spmv(V_Z, V_V, tail_none());                                               // v = (A + sigma I) z           :815-816
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
-            lop_vec_update<true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            if (xa) lop_vec_update<true, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            else lop_vec_update<true, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
             vec(PH_PUSH, tail_none(), V_W);
             spmv(V_W, V_T, tail_none());                                               // t = (A + sigma I) w           :850-851
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 1);                   // beta, alpha, loop test       :857-865
@@ -331,9 +352,10 @@ struct LopRun : PhaseLauncher {
 
 } // namespace
 
-int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter)
+int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
+              bool dev)
 {
-    ShiftedSolve s(m, L);
+    ShiftedSolve s(m, L, dev);
     Context &c = s.c;
     const int n = s.n;
 
@@ -361,12 +383,16 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.z = m->vec(V_Z); run.base.w = m->vec(V_W); run.base.v = m->vec(V_V); run.base.t = m->vec(V_T);
     run.base.rold = m->vec(pipe ? V_AX : V_V);
-    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.stride = s.stride; run.base.n = n; run.base.L = L;
+    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
+    run.base.n = n; run.base.L = L;
+    run.xa = s.x_aligned();
     run.ugrid = std::max(1, std::min(c.sm_count * 8, (n + 511) / 512));
     run.smem = (size_t)(L - 1) * LOP_COEF * sizeof(double);
     if (run.smem > 48 * 1024) {
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
+        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
     }
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :237 / :759

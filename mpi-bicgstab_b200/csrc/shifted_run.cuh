@@ -2,8 +2,8 @@
 // arena vectors through PhaseLauncher (engine.hpp) with shift_sigma set, so its SpMVs compute y = (A + sigma_seed I) x, and
 // tail_store puts the reduced epilogue dots into Scalars::pend[] for the solver's own scalar kernels.  ShiftedSolve holds
 // everything around a solver's own device state and kernel sequence: the device memory the solve owns, the sigma_len
-// solutions x_j in one strided device buffer, b in / the seed residual out through the arena's r, the timed loop and the
-// statistics every shifted solver reports alike.
+// solutions x_j (host x_set: copied into one strided device buffer; device x_set: the caller's buffer, updated in place),
+// b in / the seed residual out through the arena's r, the timed loop and the statistics every shifted solver reports alike.
 #pragma once
 #include "engine.hpp"
 
@@ -13,42 +13,53 @@
 namespace bicg {
 
 // the two families behind shifted_solve, which has checked sigma_len and seed: shifted.cu (fixed: shifted_lopbicg, else
-// shifted_lopbicg_switching) and shifted_lop.cu (pipe: PIPE-LOP, else LOP)
+// shifted_lopbicg_switching) and shifted_lop.cu (pipe: PIPE-LOP, else LOP); dev: x_set and r are device pointers
 int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
-                    int max_iter);
-int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter);
+                    int max_iter, bool dev);
+int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
+              bool dev);
 
 struct ShiftedSolve {
     static constexpr int U = 8, DEPTH = 2;   // iterations per batch; batches enqueued ahead of the done flag the host reads
     bicg_matrix *m;
     Context &c;
     const int n, L;
-    const long long stride;                  // doubles between consecutive shifts in x_set / p_set (16-byte aligned blocks)
-    double *d_x = nullptr;                   // [L][stride] the solutions x_j
+    const bool dev;                          // x_set and r are device pointers: no copy of x_set, r moves device to device
+    const long long stride;                  // doubles between consecutive shifts in the solver's p_set (16-byte aligned blocks)
+    const long long xstride;                 // ... in d_x: stride (host x_set), n (the caller's device x_set; any alignment)
+    double *d_x = nullptr;                   // [L][xstride] the solutions x_j
     double *d_b = nullptr;                   // BICG_SHIFT_ERROR only: the caller's b
     float ms = 0.f;                          // length of the timed region
     int launches0 = 0;
     std::vector<void *> owned;
 
-    ShiftedSolve(bicg_matrix *mm, int sigma_len)
-        : m(mm), c(ctx()), n(mm->n_loc), L(sigma_len), stride(((long long)mm->n_loc + 15) / 16 * 16) {}
+    ShiftedSolve(bicg_matrix *mm, int sigma_len, bool device_vectors)
+        : m(mm), c(ctx()), n(mm->n_loc), L(sigma_len), dev(device_vectors), stride(((long long)mm->n_loc + 15) / 16 * 16),
+          xstride(device_vectors ? (long long)mm->n_loc : stride) {}
     ~ShiftedSolve() { for (void *p : owned) c.dev_free(p); }
     ShiftedSolve(const ShiftedSolve &) = delete;
     ShiftedSolve &operator=(const ShiftedSolve &) = delete;
 
+    // every x_j block starts 16-byte aligned (always for a host x_set): the update kernels' XA = true variant applies
+    bool x_aligned() const { return xstride % 2 == 0 && (reinterpret_cast<size_t>(d_x) & 15) == 0; }
     template <class T> T *alloc(size_t count)       // device memory freed when the solve ends
     {
         void *p = c.dev_alloc(std::max<size_t>(count * sizeof(T), 16));
         owned.push_back(p);
         return (T *)p;
     }
-    // x_set (L blocks of n) -> d_x, b -> the arena's r, fresh solver scalars
-    void upload(const double *x_set, const double *r)
+    // x_set (L blocks of n) -> d_x (device x_set: d_x is x_set), b -> the arena's r, fresh solver scalars
+    void upload(double *x_set, const double *r)
     {
-        d_x = alloc<double>((size_t)L * stride);
-        BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double), L,
-                                    cudaMemcpyHostToDevice, c.stream));
-        BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+        if (dev) {
+            d_x = x_set;
+        } else {
+            d_x = alloc<double>((size_t)L * stride);
+            BICG_CUDA(cudaMemcpy2DAsync(d_x, stride * sizeof(double), x_set, (size_t)n * sizeof(double), (size_t)n * sizeof(double),
+                                        L, cudaMemcpyHostToDevice, c.stream));
+        }
+        BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, (size_t)n * sizeof(double), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice,
+                                  c.stream));
         if (c.cfg.shift_error) {
             d_b = alloc<double>(n);
             BICG_CUDA(cudaMemcpyAsync(d_b, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, c.stream));
@@ -65,12 +76,14 @@ struct ShiftedSolve {
         run_batches(max_iter, U, DEPTH, d_done, [&](int) { for (int u = 0; u < U; ++u) run.iteration(); });
         BICG_CUDA(cudaEventRecord(e1, c.stream));
     }
-    // after run(): x_set, the seed residual r and the solver's device state *d_state back to the host
+    // after run(): x_set (host x_set only), the seed residual r and the solver's device state *d_state back to the host
     template <class State> State finish(double *x_set, double *r, const State *d_state)
     {
-        BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
-                                    cudaMemcpyDeviceToHost, c.stream));
-        BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+        if (!dev)
+            BICG_CUDA(cudaMemcpy2DAsync(x_set, (size_t)n * sizeof(double), d_x, stride * sizeof(double), (size_t)n * sizeof(double), L,
+                                        cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), (size_t)n * sizeof(double), dev ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost,
+                                  c.stream));
         State out{};
         BICG_CUDA(cudaMemcpyAsync(&out, d_state, sizeof(State), cudaMemcpyDeviceToHost, c.stream));
         Scalars hs;
@@ -87,21 +100,21 @@ struct ShiftedSolve {
         bicg_stats st{};
         st.loop_ms = ms;
         st.kernel_launches = c.launches - launches0;
-        st.h2d_bytes = (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
+        st.h2d_bytes = dev ? 0 : (uint64_t)L * n * 8 + (uint64_t)n * 8; st.d2h_bytes = st.h2d_bytes;
         return st;
     }
     // The last step of every shifted solver, after its own printout: with BICG_SHIFT_ERROR, the relative error
     // ||(A + sigma_j I) x_j - b|| / ||b|| of every shift from d_x (collective), kept for bicg_last_shift_error and printed by
     // rank 0 as the reference's DISPLAY_ERROR block does (shifted_switching_solver.c:570-598), `seed` being the seed the solve
     // ended with.  The reference measures against (A + sigma_seed I) 1, the b its drivers build; this is the b passed in.
-    // It runs after finish() and after the solver took stats(): d_x lives until the ShiftedSolve is destroyed, the host x_set
-    // is already a copy of it, and the check's launches and time stay out of kernel_launches and loop_ms, like the reference's
+    // It runs after finish() and after the solver took stats(): d_x lives until the ShiftedSolve is destroyed (or is the
+    // caller's x_set), a host x_set is already a copy of it, and the check's launches and time stay out of kernel_launches and loop_ms, like the reference's
     // check, which runs after its timed region.
     void report_error(const double *sigma, int seed)
     {
         c.last_shift_err.clear();
         if (!d_b) return;
-        c.last_shift_err = shift_relative_errors(m, d_x, stride, d_b, sigma, L);
+        c.last_shift_err = shift_relative_errors(m, d_x, xstride, d_b, sigma, L);
         if (c.rank != 0 || c.cfg.quiet) return;
         printf("seed(0:seed, 1:shift), sigma, relative error\n");                  // :572
         for (int i = 0; i < L; ++i) {
