@@ -137,8 +137,9 @@ int bicg_abi_version(void);
  *   BICG_RESIDENT  1 persistent kernel keeps a CTA's matrix slice in shared memory for the whole solve when it fits (default) | 0
  *   BICG_PARTITION rows (matrix.c:295-308, default) | nnz (archive/matrix.c:407-420) in the loader and the generators
  *   BICG_PEER_TIMEOUT_S  bound of every device-side wait for another CTA / GPU (default 20)
- *   tuning / experiments: BICG_MEGA_THREADS, BICG_MEGA_LANES, BICG_ROW_WEIGHT, BICG_BOUNDARY_WEIGHT, BICG_L2_HINT,
- *   BICG_GATHER_CG, BICG_STAGE_UPLOAD, BICG_AUTOTUNE, BICG_SPMV_THREADS / _STAGES / _CTAS, BICG_HALO_GAP, BICG_VERBOSE,
+ *   BICG_SHIFT_TOL (1e-12) / BICG_SHIFT_MAX_ITER (1000) / BICG_SHIFT_ERROR (0): the shifted solvers, see below
+ *   tuning / experiments: BICG_MEGA_THREADS, BICG_MEGA_LANES, BICG_ROW_WEIGHT, BICG_BOUNDARY_WEIGHT, BICG_AUTOTUNE,
+ *   BICG_SPMV_THREADS / _STAGES / _CTAS, BICG_HALO_GAP, BICG_VERBOSE,
  *   BICG_MEGA_TRACE (per-phase device timestamps of the persistent kernel on stderr)
  * Returns 0 on success, -1 for an unknown key. */
 int bicg_set_option(const char *key, const char *value);

@@ -210,13 +210,6 @@ __device__ __forceinline__ void fence_gpu() { asm volatile("fence.acq_rel.gpu;" 
 __device__ __forceinline__ void fence_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
 // plain ld.global: L1-cached but never the non-coherent (.nc) path -- for vectors that other SMs / peer GPUs rewrite
 // while the kernel is running (visibility comes from the acquire fence that follows the flag wait)
-// L2-only gather (ld.global.cg): never allocates in L1, so it cannot return a line that went stale in this SM's L1
-__device__ __forceinline__ double ld_l2(const double *p)
-{
-    double v;
-    asm volatile("ld.global.cg.f64 %0, [%1];" : "=d"(v) : "l"(p));
-    return v;
-}
 __device__ __forceinline__ double ld_coherent(const double *p)
 {
     double v;

@@ -44,10 +44,7 @@ struct Config {
     int mega_threads = 0;        // 0 choose (512, else 256)
     int mega_trace = 0;
     int mega_lanes = 0;          // lanes per row of the persistent kernel's SpMV (0 choose from the mean row length)
-    int stage_upload = 1;        // large pageable host arrays are uploaded through multi-threaded pinned staging (Context::h2d)
     int resident = 1;            // persistent kernel: keep a CTA's matrix slice in shared memory for the whole solve when it fits
-    int gather_cg = -1;          // SpMV gathers of the persistent kernel through L2 only + fence-free neighbour waits (-1: default = off)
-    int l2_hint = 1;             // matrix stream loaded with an L2 evict-first policy (persistent kernel)
     int row_weight = 1200;       // per-row cost (byte equivalents) next to 24 B per entry when CTA row ranges are balanced
     int boundary_weight = 300;   // extra work (bytes) charged per pushed row when CTA row ranges are balanced
     int device = -1;
@@ -57,8 +54,6 @@ struct Config {
     int shift_max_iter = 1000;   // their MAX_ITER (:6)
     int shift_error = 0;         // 1: after a shifted solve, the relative error of every shift (their DISPLAY_ERROR, :17)
     int peer_timeout_s = 20;     // bound of device-side waits for peers / other CTAs (then: error + exit(1))
-    int fence_writers = 0;       // 1: every thread that stored to a peer also fences at system scope itself (debug aid;
-                                 // the CTA barrier + one system fence per CTA is sufficient and much cheaper)
 };
 
 struct TuneKey {
@@ -132,8 +127,8 @@ struct Context {
     int stage_threads = 4;
 };
 Context &ctx();
-void load_config_from_env(Config &c);
-int  set_option(Config &c, const char *key, const char *value);
+void load_config_from_env(Config &c);                              // every option of matrix.cu's table set as BICG_<key>
+int  set_option(Config &c, const char *key, const char *value);    // -1: unknown key
 
 
 struct SpmvPlan {

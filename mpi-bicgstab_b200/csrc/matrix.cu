@@ -7,6 +7,7 @@
 #include "engine.hpp"
 
 #include <algorithm>
+#include <climits>
 #include <cmath>
 #include <cstdarg>
 #include <cstring>
@@ -28,58 +29,73 @@ void fatal(const char *fmt, ...)
 // ------------------------------------------------------------------------------------------------
 // configuration
 // ------------------------------------------------------------------------------------------------
+namespace {
+
+enum class Parse { Int, Double, Spmv };   // Spmv: auto | tma | rowsplit -> -1 | 0 | 1
+
+// Every runtime option: its key (BICG_<key> in the environment; the prefix is optional in bicg_set_option), the Config
+// member it sets, how its value is parsed and, for an integer, the least value it takes (smaller ones are raised to it).
+struct Option {
+    const char *key;
+    Parse parse;
+    int Config::*i = nullptr;
+    double Config::*d = nullptr;
+    int min = INT_MIN;
+};
+
+const Option OPTIONS[] = {
+    {"TOL", Parse::Double, nullptr, &Config::tol},
+    {"MAX_ITER", Parse::Int, &Config::max_iter},
+    {"OUT_ITER", Parse::Int, &Config::out_iter},
+    {"QUIET", Parse::Int, &Config::quiet},
+    {"SPMV", Parse::Spmv, &Config::spmv_kind},
+    {"SPMV_LANES", Parse::Int, &Config::spmv_lanes},
+    {"SPMV_THREADS", Parse::Int, &Config::spmv_threads},
+    {"SPMV_STAGES", Parse::Int, &Config::spmv_stages},
+    {"SPMV_CTAS", Parse::Int, &Config::spmv_ctas},
+    {"AUTOTUNE", Parse::Int, &Config::autotune},
+    {"GRAPH", Parse::Int, &Config::graph},
+    {"UNROLL", Parse::Int, &Config::unroll, nullptr, 1},
+    {"CACHE", Parse::Int, &Config::cache},
+    {"MEGA", Parse::Int, &Config::mega},
+    {"MEGA_THREADS", Parse::Int, &Config::mega_threads},
+    {"MEGA_TRACE", Parse::Int, &Config::mega_trace},
+    {"MEGA_LANES", Parse::Int, &Config::mega_lanes},
+    {"RESIDENT", Parse::Int, &Config::resident},
+    {"BOUNDARY_WEIGHT", Parse::Int, &Config::boundary_weight, nullptr, 0},
+    {"ROW_WEIGHT", Parse::Int, &Config::row_weight, nullptr, 1},
+    {"DEVICE", Parse::Int, &Config::device},
+    {"HALO_GAP", Parse::Int, &Config::halo_gap, nullptr, 0},
+    {"VERBOSE", Parse::Int, &Config::verbose},
+    {"PEER_TIMEOUT_S", Parse::Int, &Config::peer_timeout_s, nullptr, 1},
+    {"SHIFT_TOL", Parse::Double, nullptr, &Config::shift_tol},
+    {"SHIFT_MAX_ITER", Parse::Int, &Config::shift_max_iter, nullptr, 1},
+    {"SHIFT_ERROR", Parse::Int, &Config::shift_error},
+};
+
+void apply(Config &c, const Option &o, const char *value)
+{
+    switch (o.parse) {
+    case Parse::Int:    c.*o.i = std::max(o.min, atoi(value)); break;
+    case Parse::Double: c.*o.d = atof(value); break;
+    case Parse::Spmv:   c.*o.i = !strcmp(value, "tma") ? 0 : !strcmp(value, "rowsplit") ? 1 : -1; break;
+    }
+}
+
+} // namespace
+
 int set_option(Config &c, const char *key, const char *value)
 {
-    std::string k(key);
-    if (k.rfind("BICG_", 0) == 0) k = k.substr(5);
-    auto as_int = [&] { return atoi(value); };
-    if (k == "TOL") c.tol = atof(value);
-    else if (k == "MAX_ITER") c.max_iter = as_int();
-    else if (k == "OUT_ITER") c.out_iter = as_int();
-    else if (k == "QUIET") c.quiet = as_int();
-    else if (k == "SPMV") {
-        std::string v(value);
-        c.spmv_kind = (v == "tma") ? 0 : (v == "rowsplit") ? 1 : -1;
-    }
-    else if (k == "SPMV_LANES") c.spmv_lanes = as_int();
-    else if (k == "SPMV_THREADS") c.spmv_threads = as_int();
-    else if (k == "SPMV_STAGES") c.spmv_stages = as_int();
-    else if (k == "SPMV_CTAS") c.spmv_ctas = as_int();
-    else if (k == "AUTOTUNE") c.autotune = as_int();
-    else if (k == "GRAPH") c.graph = as_int();
-    else if (k == "UNROLL") c.unroll = std::max(1, as_int());
-    else if (k == "CACHE") c.cache = as_int();
-    else if (k == "MEGA") c.mega = as_int();
-    else if (k == "MEGA_THREADS") c.mega_threads = as_int();
-    else if (k == "MEGA_TRACE") c.mega_trace = as_int();
-    else if (k == "MEGA_LANES") c.mega_lanes = as_int();
-    else if (k == "L2_HINT") c.l2_hint = as_int();
-    else if (k == "GATHER_CG") c.gather_cg = as_int();
-    else if (k == "RESIDENT") c.resident = as_int();
-    else if (k == "STAGE_UPLOAD") c.stage_upload = as_int();
-    else if (k == "BOUNDARY_WEIGHT") c.boundary_weight = std::max(0, as_int());
-    else if (k == "ROW_WEIGHT") c.row_weight = std::max(1, as_int());
-    else if (k == "DEVICE") c.device = as_int();
-    else if (k == "HALO_GAP") c.halo_gap = std::max(0, as_int());
-    else if (k == "VERBOSE") c.verbose = as_int();
-    else if (k == "PEER_TIMEOUT_S") c.peer_timeout_s = std::max(1, as_int());
-    else if (k == "SHIFT_TOL") c.shift_tol = atof(value);
-    else if (k == "SHIFT_MAX_ITER") c.shift_max_iter = std::max(1, as_int());
-    else if (k == "SHIFT_ERROR") c.shift_error = as_int();
-    else if (k == "FENCE_WRITERS") c.fence_writers = as_int();
-    else return -1;
-    return 0;
+    if (!strncmp(key, "BICG_", 5)) key += 5;
+    for (const Option &o : OPTIONS)
+        if (!strcmp(key, o.key)) { apply(c, o, value); return 0; }
+    return -1;
 }
 
 void load_config_from_env(Config &c)
 {
-    static const char *keys[] = {"BICG_TOL", "BICG_MAX_ITER", "BICG_OUT_ITER", "BICG_QUIET", "BICG_SPMV",
-                                 "BICG_SPMV_LANES", "BICG_SPMV_THREADS", "BICG_SPMV_STAGES", "BICG_SPMV_CTAS",
-                                 "BICG_AUTOTUNE", "BICG_GRAPH", "BICG_UNROLL", "BICG_CACHE", "BICG_MEGA", "BICG_MEGA_THREADS", "BICG_MEGA_TRACE", "BICG_MEGA_LANES", "BICG_L2_HINT", "BICG_GATHER_CG", "BICG_RESIDENT", "BICG_STAGE_UPLOAD", "BICG_BOUNDARY_WEIGHT", "BICG_ROW_WEIGHT", "BICG_DEVICE",
-                                 "BICG_HALO_GAP", "BICG_VERBOSE", "BICG_PEER_TIMEOUT_S", "BICG_SHIFT_TOL", "BICG_SHIFT_MAX_ITER", "BICG_FENCE_WRITERS",
-                                 "BICG_SHIFT_ERROR"};
-    for (const char *k : keys)
-        if (const char *v = getenv(k)) set_option(c, k, v);
+    for (const Option &o : OPTIONS)
+        if (const char *v = getenv(("BICG_" + std::string(o.key)).c_str())) apply(c, o, v);
 }
 
 Context &ctx()
@@ -195,7 +211,7 @@ void Context::h2d(void *dst, const void *src, size_t bytes)
 {
     constexpr size_t CHUNK = (size_t)8 << 20, MIN_STAGED = (size_t)16 << 20;
     bool pageable = false;
-    if (bytes >= MIN_STAGED && cfg.stage_upload) {
+    if (bytes >= MIN_STAGED) {
         cudaPointerAttributes at{};
         const cudaError_t e = cudaPointerGetAttributes(&at, src);
         if (e != cudaSuccess) (void)cudaGetLastError();

@@ -256,7 +256,7 @@ struct Mega {
                     if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { ok = false; break; }
                 }
             }
-            if (!a.gather_cg) fence_gpu();                   // acquire (+ L1 invalidate): the gathers that follow see the data
+            fence_gpu();                                     // acquire (+ L1 invalidate): the gathers that follow see the data
             if (!__all_sync(0xffffffffu, ok) && lane == 0) fail();
         }
         nbar(1, CT);
@@ -433,22 +433,14 @@ struct Mega {
     }
 
     // ---------------------------------------------------------------- SpMV over this CTA's tiles ----------
-    // gather_cg (BICG_GATHER_CG=1, multi-GPU experiments): x is gathered with L2-only loads; the neighbour waits then need no
-    // acquire fence (no L1 line can be stale), which takes a MEMBAR + CCTL.IVALL off every neighbour wait
     template <int EPI>
     __device__ void spmv(const double *x, double *y, double (&dot)[4])
     {
         if constexpr (LANES == 1) {
-            if (resident) {
-                if (a.gather_cg) spmv_res<EPI, true>(x, y, dot); else spmv_res<EPI, false>(x, y, dot);
-                return;
-            }
+            if (resident) { spmv_res<EPI>(x, y, dot); return; }
         }
-        if (coded) {
-            if (a.gather_cg) spmv_impl<EPI, true, true>(x, y, dot); else spmv_impl<EPI, false, true>(x, y, dot);
-        } else {
-            if (a.gather_cg) spmv_impl<EPI, true, false>(x, y, dot); else spmv_impl<EPI, false, false>(x, y, dot);
-        }
+        if (coded) spmv_impl<EPI, true>(x, y, dot);
+        else spmv_impl<EPI, false>(x, y, dot);
     }
     // one row's epilogue: y and the dots fused into the SpMV (same operations, same order as the streaming path)
     template <int EPI>
@@ -466,7 +458,7 @@ struct Mega {
     // columns); a row's entries are accumulated in storage order, like spmv_impl.  Loads are unconditional on clamped indices
     // (always a valid entry of this slice; no predicate per load, so the U gathers of a pass are in flight together), only the
     // multiply-adds are guarded.
-    template <int EPI, bool CG>
+    template <int EPI>
     __device__ void spmv_res(const double *x, double *y, double (&dot)[4])
     {
         constexpr int U = 16;
@@ -489,8 +481,7 @@ struct Mega {
 #pragma unroll
                 for (int u = 0; u < U; ++u) {
                     const unsigned c = rs_col[min(min(j + (unsigned)u, e - 1u), last)];
-                    const double *src = (c < ospan ? xo : xg) + c;
-                    xv[u] = CG ? ld_l2(src) : ld_coherent(src);
+                    xv[u] = ld_coherent((c < ospan ? xo : xg) + c);
                 }
 #pragma unroll
                 for (int u = 0; u < U; ++u) {                  // the values come from shared memory when they are needed
@@ -505,7 +496,7 @@ struct Mega {
 
     // CODED: the stage's column area holds the CTA's 16-bit column codes (its first half; the stage layout is the same for
     // both formats), each turned back into the column with one select and one add before its gather
-    template <int EPI, bool CG, bool CODED>
+    template <int EPI, bool CODED>
     __device__ void spmv_impl(const double *x, double *y, double (&dot)[4])
     {
         const int stages = a.stages, cap = a.cap;
@@ -531,8 +522,7 @@ struct Mega {
 #pragma unroll
                     for (int u = 0; u < 4; ++u) {
                         const unsigned idx = min(jj + (unsigned)(u * CT), h.hi - 1u);
-                        const double *src = x + column(idx);
-                        pv[u] = sval[idx]; px[u] = CG ? ld_l2(src) : ld_coherent(src);
+                        pv[u] = sval[idx]; px[u] = ld_coherent(x + column(idx));
                     }
 #pragma unroll
                     for (int u = 0; u < 4; ++u)
@@ -585,7 +575,7 @@ struct Mega {
                     v[u] = sval[idx];
                 }
 #pragma unroll
-                for (int u = 0; u < UNR; ++u) xv[u] = CG ? ld_l2(x + c[u]) : ld_coherent(x + c[u]);
+                for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
 #pragma unroll
                 for (int u = 0; u < UNR; ++u)
                     if (j + u * LANES < e) acc = fma(v[u], xv[u], acc);
@@ -639,7 +629,7 @@ struct Mega {
                 }
             }
             nbar(2, RED_THREADS);
-            if (tid < 32 && !a.gather_cg) fence_gpu(); // acquire (+ L1 invalidate) after ALL pollers are through
+            if (tid < 32) fence_gpu();                 // acquire (+ L1 invalidate) after ALL pollers are through
         }
         nbar(1, CT);
         if (sh.flags[3]) { if (tid == 0) { sh.sc.error = 1; sh.sc.done = 1; } nbar(1, CT); }
@@ -743,7 +733,8 @@ struct Mega {
     // measured at ~4.5 us), the consumer polls exactly the elements it needs.  The LL copy of s alternates between
     // two regions: a peer may already push s of iteration k + 1 while this rank still applies s of iteration k to its
     // ghost p; r needs one region (its next push follows a reduction that this rank enters after consuming it).
-    __device__ void run_bicgstab_multi()
+    // __noinline__: inlined next to run_ca, it makes bicg_mega_kernel<512, 1> spill the CTA's column window
+    __device__ __noinline__ void run_bicgstab_multi()
     {
         double d4[4], d2[2], d1[1], d0[1];
         d0[0] = 0.0;
@@ -786,7 +777,8 @@ struct Mega {
         }
     }
     // ---------------------------------------------------------------- solver.c:86-127 -----------------------
-    __device__ void run_bicgstab()
+    // __noinline__: inlined into the kernel body, it makes the four 512-thread kernels spill under their 96-register cap
+    __device__ __noinline__ void run_bicgstab()
     {
         double d4[4], d2[2], d1[1], d0[1];
         d0[0] = 0.0;
@@ -848,7 +840,8 @@ struct Mega {
         }
     }
     // ---------------------------------------------------------------- solver.c:351-398 / 494-547 ------------
-    __device__ void run_pipe(bool rr)
+    // __noinline__ for the same reason as run_bicgstab
+    __device__ __noinline__ void run_pipe(bool rr)
     {
         double d5[5], d4[4], d2[2], d0[1];
         d0[0] = 0.0; d4[0] = d4[1] = d4[2] = d4[3] = 0.0;
@@ -922,7 +915,6 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
         if (tid == CT && my_tiles > 0 && !rp.on) {
             volatile int *flags = sh.flags;
             const unsigned long long pol = l2_evict_first_policy();
-            const bool hint = a.l2_hint != 0;
             // 16-bit codes: 2 bytes per entry; a bulk copy moves whole 16-byte units, so the entry window of a tile is
             // aligned to 8 entries (4 suffice for 4-byte columns); the plan's stage capacity covers the wider window
             const bool coded = streams_codes(a, rp, my_tiles);
@@ -953,13 +945,8 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
                 mbar_arrive_expect_tx(bar, cnt * (8u + cbytes) + (unsigned)cntp * 4u);
                 if (cnt) {
                     const void *csrc = (const char *)cols + (size_t)a0 * cbytes;
-                    if (hint) {
-                        tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
-                        tma_load_1d_hint(smem_u32(scol), csrc, cnt * cbytes, bar, pol);
-                    } else {
-                        tma_load_1d(smem_u32(sval), a.val + a0, cnt * 8u, bar);
-                        tma_load_1d(smem_u32(scol), csrc, cnt * cbytes, bar);
-                    }
+                    tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
+                    tma_load_1d_hint(smem_u32(scol), csrc, cnt * cbytes, bar, pol);
                 }
                 tma_load_1d(smem_u32(sptr), a.ptr + rowa, (unsigned)cntp * 4u, bar);
             }

@@ -65,8 +65,6 @@ struct MegaArgs {
     const int      *tile_flag;  // null, or per tile: 0 whole rows, 1 / 2 chunk of ONE long row (more follow / last)
     int cap, stages;
     int ghost_off;
-    int l2_hint;                // 1: matrix stream is loaded with an L2 evict-first policy
-    int gather_cg;              // 1: SpMV gathers bypass L1 (ld.global.cg) and the neighbour waits skip the acquire fence
     int resident;               // 1: a CTA whose whole matrix slice fits into its shared memory (strong scaling: 8 GPUs x one CTA per SM)
                                 //    loads it ONCE per solve (values + 16-bit CTA-relative columns + row pointers) instead of streaming it
                                 //    through the TMA ring in every SpMV

@@ -71,7 +71,6 @@ PushDesc PhaseLauncher::make_push(int id, const double *push_src) const
     PushDesc pd{};
     if (m->world == 1) return pd;
     pd.npeers = m->npush;
-    pd.fence_writers = c.cfg.fence_writers;
     pd.src = push_src ? push_src : m->vec(id);
     for (int s = 0; s < m->npush; ++s) {
         const int d = m->push_peer[s];
@@ -163,8 +162,7 @@ struct Seq : PhaseLauncher {
         a.tile_row = m->mega.d_tile_row; a.tile_nz = m->mega.d_tile_nz; a.cta_tile = m->mega.d_cta_tile;
         a.tile_flag = m->mega.d_tile_flag;
         a.cap = m->mega.cap; a.stages = m->mega.stages;
-        a.ghost_off = m->ghost_off; a.l2_hint = c.cfg.l2_hint;
-        a.gather_cg = c.cfg.gather_cg >= 0 ? c.cfg.gather_cg : 0;
+        a.ghost_off = m->ghost_off;
         size_t smem = m->mega.smem;
         a.resident = (c.cfg.resident && m->mega.res_smem) ? 1 : 0;
         if (a.resident) smem = std::max(smem, m->mega.res_smem);

@@ -53,7 +53,7 @@ __global__ void __launch_bounds__(256) vec_kernel(const __grid_constant__ VecArg
     const bool pushing = a.push.npeers > 0;
     if (pushing) {
         __syncthreads();                 // this CTA's elements are final
-        (void)push_chunk(a.push, lo, hi, (int)threadIdx.x, (int)blockDim.x);
+        push_chunk(a.push, lo, hi, (int)threadIdx.x, (int)blockDim.x);
         // the peer stores are ordered before the halo flag by ONE system-scope fence per CTA: kernel_tail's
         // thread 0 fences after the __syncthreads that follows (cumulativity covers the whole CTA's stores);
         // a fence.sys in every thread costs microseconds per kernel

@@ -9,7 +9,6 @@ struct PushRun { int src; int len; int dst_off; };
 
 struct PushDesc {
     int npeers;                              // 0: nothing to push
-    int fence_writers;                       // 1: every thread that stored to a peer issues its own fence.sys
     const double  *src;                      // the vector being pushed (own part)
     double        *dst[MAX_RANKS - 1];       // peer-mapped base of that vector's ghost region on peer i
     const PushRun *runs[MAX_RANKS - 1];      // runs for peer i, sorted by src, disjoint

@@ -221,9 +221,8 @@ __device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, dou
 
 
 // copy the parts of this CTA's chunk [lo, hi) that peers need into their ghost regions (peer stores)
-__device__ __forceinline__ bool push_chunk(const PushDesc &pd, int lo, int hi, int tid, int nthreads)
+__device__ __forceinline__ void push_chunk(const PushDesc &pd, int lo, int hi, int tid, int nthreads)
 {
-    bool stored = false;
     for (int pi = 0; pi < pd.npeers; ++pi) {
         const PushRun *runs = pd.runs[pi];
         const int nr = pd.nruns[pi];
@@ -246,15 +245,10 @@ __device__ __forceinline__ bool push_chunk(const PushDesc &pd, int lo, int hi, i
                 for (int u = 0; u < 8; ++u) t[u] = __ldcg(pd.src + i + u * nthreads);
 #pragma unroll
                 for (int u = 0; u < 8; ++u) d[i + u * nthreads] = t[u];
-                stored = true;
             }
-            for (; i < e; i += nthreads) { d[i] = __ldcg(pd.src + i); stored = true; }
+            for (; i < e; i += nthreads) d[i] = __ldcg(pd.src + i);
         }
     }
-    // a thread that wrote to a peer orders its own NVLink stores before anything that follows (the halo flag
-    // is released by the tail after a CTA barrier, a grid-wide ticket and another system fence)
-    if (stored && pd.fence_writers) __threadfence_system();
-    return stored;
 }
 
 
