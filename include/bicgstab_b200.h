@@ -186,13 +186,16 @@ int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nr
 
 /* shifted_lopbicg_switching on a resident matrix; bicg_last_shift_info: the seed the last shifted solve ended with and the
  * iteration at which every shift stopped (returns sigma_len).  The stop iteration is 1-based (the iteration after whose
- * convergence test the shift stopped), 0 for a shift that never stopped; for shifted_lopbicg the seed is the one passed in. */
+ * convergence test the shift stopped), 0 for a shift that never stopped; for shifted_lopbicg the seed is the one passed in.
+ * After a solve of the LOP family it is the seed passed in and 0 for every shift: there no shift stops on its own. */
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats);
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap);
 /* Any shifted solver on a resident matrix: BICG_SHIFTED_SWITCHING = shifted_lopbicg_switching (returns iterations + 1, like
  * bicg_shifted_solve), BICG_SHIFTED_LOP = shifted_lopbicgstab, BICG_SHIFTED_PIPE_LOP = shifted_pipe_lopbicgstab,
  * BICG_SHIFTED_LOPBICG = shifted_lopbicg (these three return the iterations performed).  -1 for an unknown method,
- * sigma_len <= 0 or seed outside [0, sigma_len). */
+ * sigma_len <= 0 or seed outside [0, sigma_len).  Any sigma_len > 0 works, in every shifted entry point of this header, as
+ * far as device memory holds x_set, p_j of every shift and, for the switching and fixed-seed solvers, their
+ * sigma_len x (BICG_SHIFT_MAX_ITER + 1) history of pi. */
 enum { BICG_SHIFTED_SWITCHING = 0, BICG_SHIFTED_LOP = 1, BICG_SHIFTED_PIPE_LOP = 2, BICG_SHIFTED_LOPBICG = 3 };
 int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
                           bicg_stats *stats);

@@ -29,6 +29,7 @@ namespace bicg {
 namespace {
 
 constexpr int SH_COEF = 6;          // per active shift: c1, alpha_j, c2, c3, beta_j, c4
+constexpr size_t SH_ENTRY = SH_COEF * sizeof(double) + sizeof(int);     // shared memory of sh_vec_shift per shift: coefficients, index
 constexpr int SH_EVENTS = 16;       // seed switches remembered for the reference's printf lines
 
 struct ShiftDev {
@@ -203,6 +204,7 @@ struct ShVec {
     long long xstride;                           // doubles between consecutive shifts in x_set (blocks may be misaligned)
     long long stride;                            // ... in p_set (even: every block starts 16-byte aligned)
     int n, L;
+    int chunk;                                   // shifts per pass of sh_vec_shift, the size of its coefficient table (<= L)
 };
 
 // r# = r, p[seed] (arena) = r, p[j] = r for every shift, (r,r)                                        :342-354
@@ -256,43 +258,49 @@ __global__ void __launch_bounds__(256) sh_vec_xr(const __grid_constant__ ShVec a
 // device x_set has blocks of n doubles from any 8-byte aligned base, so a block may not be: then x_j moves as two 8-byte
 // accesses.  i is even, so the choice depends on the shift alone and is the same for the whole warp.  XA: the host found
 // every block aligned (always so for a host x_set) and the test is compiled out.
+// The active shifts go in passes of a.chunk: each pass loads their coefficients into shared memory and walks the rows.  A shift
+// is updated in exactly one pass, with the same operations, so the number of passes does not change any result.
 template <bool XA>
 __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVec a)
 {
     const ShiftDev *sd = a.sd;
     if (!sd->live) return;
-    extern __shared__ double s_coef[];                       // [n_active][SH_COEF] then the shift indices
-    const int na = sd->n_active;
-    int *s_idx = reinterpret_cast<int *>(s_coef + (size_t)na * SH_COEF);
-    for (int t = threadIdx.x; t < na * SH_COEF; t += blockDim.x) s_coef[t] = sd->coef[t];
-    for (int t = threadIdx.x; t < na; t += blockDim.x) s_idx[t] = sd->active[t];
-    __syncthreads();
-    for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
-        const bool two = i + 1 < a.n;
-        double q0 = a.qc[i], q1 = two ? a.qc[i + 1] : 0.0;
-        double o0 = a.rold[i], o1 = two ? a.rold[i + 1] : 0.0;
-        double r0 = a.r[i], r1 = two ? a.r[i + 1] : 0.0;
+    extern __shared__ double s_coef[];                       // [chunk][SH_COEF] then the shift indices
+    int *s_idx = reinterpret_cast<int *>(s_coef + (size_t)a.chunk * SH_COEF);
+    const int n_active = sd->n_active;
+    for (int t0 = 0; t0 < n_active; t0 += a.chunk) {
+        const int na = min(a.chunk, n_active - t0);
+        __syncthreads();                                     // the previous pass is done with the table
+        for (int t = threadIdx.x; t < na * SH_COEF; t += blockDim.x) s_coef[t] = sd->coef[(size_t)t0 * SH_COEF + t];
+        for (int t = threadIdx.x; t < na; t += blockDim.x) s_idx[t] = sd->active[t0 + t];
+        __syncthreads();
+        for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
+            const bool two = i + 1 < a.n;
+            double q0 = a.qc[i], q1 = two ? a.qc[i + 1] : 0.0;
+            double o0 = a.rold[i], o1 = two ? a.rold[i + 1] : 0.0;
+            double r0 = a.r[i], r1 = two ? a.r[i + 1] : 0.0;
 #pragma unroll 2
-        for (int t = 0; t < na; ++t) {
-            const double *c = s_coef + (size_t)t * SH_COEF;
-            double *xj = a.x_set + (size_t)s_idx[t] * a.xstride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
-            const bool xa = XA || (reinterpret_cast<size_t>(xj) & 15) == 0;
-            double x0, x1, p0, p1;
-            if (two) {
-                const double2 pv = *reinterpret_cast<const double2 *>(pj);
-                p0 = pv.x; p1 = pv.y;
-                if (xa) { const double2 xv = *reinterpret_cast<const double2 *>(xj); x0 = xv.x; x1 = xv.y; }
-                else { x0 = xj[0]; x1 = xj[1]; }
-            } else { x0 = xj[0]; p0 = pj[0]; x1 = p1 = 0.0; }
-            x0 = fma(c[0], q0, x0); x0 = fma(c[1], p0, x0);
-            x1 = fma(c[0], q1, x1); x1 = fma(c[1], p1, x1);
-            p0 = fma(c[2], q0, p0); p0 = fma(c[3], o0, p0); p0 = c[4] * p0; p0 = fma(c[5], r0, p0);
-            p1 = fma(c[2], q1, p1); p1 = fma(c[3], o1, p1); p1 = c[4] * p1; p1 = fma(c[5], r1, p1);
-            if (two) {
-                if (xa) *reinterpret_cast<double2 *>(xj) = make_double2(x0, x1);
-                else { xj[0] = x0; xj[1] = x1; }
-                *reinterpret_cast<double2 *>(pj) = make_double2(p0, p1);
-            } else { xj[0] = x0; pj[0] = p0; }
+            for (int t = 0; t < na; ++t) {
+                const double *c = s_coef + (size_t)t * SH_COEF;
+                double *xj = a.x_set + (size_t)s_idx[t] * a.xstride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
+                const bool xa = XA || (reinterpret_cast<size_t>(xj) & 15) == 0;
+                double x0, x1, p0, p1;
+                if (two) {
+                    const double2 pv = *reinterpret_cast<const double2 *>(pj);
+                    p0 = pv.x; p1 = pv.y;
+                    if (xa) { const double2 xv = *reinterpret_cast<const double2 *>(xj); x0 = xv.x; x1 = xv.y; }
+                    else { x0 = xj[0]; x1 = xj[1]; }
+                } else { x0 = xj[0]; p0 = pj[0]; x1 = p1 = 0.0; }
+                x0 = fma(c[0], q0, x0); x0 = fma(c[1], p0, x0);
+                x1 = fma(c[0], q1, x1); x1 = fma(c[1], p1, x1);
+                p0 = fma(c[2], q0, p0); p0 = fma(c[3], o0, p0); p0 = c[4] * p0; p0 = fma(c[5], r0, p0);
+                p1 = fma(c[2], q1, p1); p1 = fma(c[3], o1, p1); p1 = c[4] * p1; p1 = fma(c[5], r1, p1);
+                if (two) {
+                    if (xa) *reinterpret_cast<double2 *>(xj) = make_double2(x0, x1);
+                    else { xj[0] = x0; xj[1] = x1; }
+                    *reinterpret_cast<double2 *>(pj) = make_double2(p0, p1);
+                } else { xj[0] = x0; pj[0] = p0; }
+            }
         }
     }
 }
@@ -335,7 +343,9 @@ struct ShRun : PhaseLauncher {
     void prologue()
     {
         sh_vec_init<<<m->vgrid, 256, 0, c.stream>>>(vargs(tail_store(1)));          // :342-354
+        check_launch("sh_vec_init");
         sh_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc);
+        check_launch("sh_scalar_init");
         vec(PH_PUSH, tail_none(), V_P);
         c.launches += 2;
     }
@@ -345,17 +355,24 @@ struct ShRun : PhaseLauncher {
         const double *Y = nullptr;
         spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), Y);                            // s = (A + sigma I) p, (r#,s)   :377-387
         sh_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
+        check_launch("sh_scalar_alpha");
         sh_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // q, r_old, q_copy            :374, 391-392
+        check_launch("sh_vec_q");
         vec(PH_PUSH, tail_none(), V_R);
         spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), Y);   // y = (A + sigma I) q, (q,q), (q,y)  :395-406
         sh_scalar_omega<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
+        check_launch("sh_scalar_omega");
         sh_vec_xr<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));                     // x[seed], r, (r,r), (r#,r)   :411-416
+        check_launch("sh_vec_xr");
         sh_scalar_iter<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                       // beta ... loop test          :420, 429-537
-        const size_t smem = (size_t)base.L * (SH_COEF * sizeof(double) + sizeof(int));
+        check_launch("sh_scalar_iter");
+        const size_t smem = (size_t)base.chunk * SH_ENTRY;
         const int sgrid = std::max(1, std::min(c.sm_count * 8, (m->n_loc + 511) / 512));
         if (xa) sh_vec_shift<true><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
         else sh_vec_shift<false><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
+        check_launch("sh_vec_shift");
         sh_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // p[seed] (or the switch)     :421-423 / :499
+        check_launch("sh_vec_p");
         vec(PH_PUSH, tail_none(), V_P);
         c.launches += 7;
     }
@@ -404,11 +421,7 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
     run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
     run.base.n = n; run.base.L = L;
     run.xa = s.x_aligned();
-    const size_t smem = (size_t)L * (SH_COEF * sizeof(double) + sizeof(int));
-    if (smem > 48 * 1024) {
-        BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        BICG_CUDA(cudaFuncSetAttribute(sh_vec_shift<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    }
+    run.base.chunk = std::min(L, run.xa ? table_chunk(sh_vec_shift<true>, SH_ENTRY) : table_chunk(sh_vec_shift<false>, SH_ENTRY));
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :364
     const ShiftDev out = s.finish(x_set, r, d_sd);

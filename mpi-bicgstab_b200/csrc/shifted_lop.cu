@@ -136,6 +136,7 @@ struct LopVec {
     long long xstride;                                  // doubles between consecutive shifts in x_set (blocks may be misaligned)
     long long stride;                                   // ... in p_set (even: every block starts 16-byte aligned)
     int n, L;
+    int chunk;                                          // non-seed shifts per pass of lop_vec_update, the size of its table
 };
 
 __device__ __forceinline__ void ld2(const double *p, int i, bool two, double (&v)[2])
@@ -225,54 +226,52 @@ __global__ void __launch_bounds__(256) lop_vec_pipe1(const __grid_constant__ Lop
 //   shifts p_j = beta_j p_j + c4 r_old; x_j += c1 q + alpha_j p_j; p_j += c2 q + c3 r_old   :267-268, 299-302 / :807-808, 835-838
 //   dots   LOP (r,r), (r#,r)                                                               :306, 308
 //          PIPE-LOP (r,r), (r#,r), (r#,w), (r#,s), (r#,z)                                  :842, 846-849
-template <bool PIPE, bool XA>
-__global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ LopVec a)
+// The non-seed shifts go in passes of a.chunk, each of which loads their coefficients into shared memory and walks the rows;
+// the seed is updated in the last pass, because that overwrites q (in r), which every earlier pass reads.  A shift is updated
+// in exactly one pass, with the same operations, so the number of passes does not change any result.
+template <bool PIPE, bool XA, bool SEED>
+__device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, int t0, int na, double (&dot)[PIPE ? 5 : 2])
 {
     const LopDev *sd = a.sd;
-    if (sd->done) return;
-    constexpr int ND = PIPE ? 5 : 2;
-    __shared__ double scratch[32 * MAX_DOTS];
-    extern __shared__ double s_coef[];                  // [L - 1][LOP_COEF]
-    const int na = a.L - 1, seed = sd->seed;
-    for (int t = threadIdx.x; t < na * LOP_COEF; t += blockDim.x) s_coef[t] = sd->coef[t];
-    __syncthreads();
+    const int seed = sd->seed;
     const double al = sd->alpha, om = sd->omega;
     double *xs = a.x_set + (size_t)seed * a.xstride;
     const bool xs_al = XA || aligned16(xs);
-    double dot[ND];
-#pragma unroll
-    for (int d = 0; d < ND; ++d) dot[d] = 0.0;
     for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
         const bool two = i + 1 < a.n;                   // stride and arena vectors are 16-byte aligned, i is even
-        const int ne = two ? 2 : 1;
-        double q[2], o[2], x[2], p[2], y[2], r[2], rh[2];
-        ld2(a.r, i, two, q); ld2(a.rold, i, two, o); ld2x(xs, i, two, xs_al, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
-        ld2(PIPE ? a.w : a.y, i, two, y);
-        for (int e = 0; e < ne; ++e) {
-            x[e] = fma(al, p[e], x[e]);
-            x[e] = fma(om, q[e], x[e]);
-            r[e] = fma(-om, y[e], q[e]);
-            dot[0] = fma(r[e], r[e], dot[0]);
-            dot[1] = fma(rh[e], r[e], dot[1]);
-        }
-        st2x(xs, i, two, xs_al, x); st2(a.r, i, two, r);
-        if constexpr (PIPE) {
-            double t[2], v[2], w[2], s[2], z[2];
-            ld2(a.t, i, two, t); ld2(a.v, i, two, v); ld2(a.s, i, two, s); ld2(a.z, i, two, z);
+        double q[2], o[2];
+        ld2(a.r, i, two, q); ld2(a.rold, i, two, o);
+        if constexpr (SEED) {
+            const int ne = two ? 2 : 1;
+            double x[2], p[2], y[2], r[2], rh[2];
+            ld2x(xs, i, two, xs_al, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
+            ld2(PIPE ? a.w : a.y, i, two, y);
             for (int e = 0; e < ne; ++e) {
-                t[e] = fma(-al, v[e], t[e]);            // t itself is overwritten by t = (A + sigma I) w next
-                w[e] = fma(-om, t[e], y[e]);
-                dot[2] = fma(rh[e], w[e], dot[2]);
-                dot[3] = fma(rh[e], s[e], dot[3]);
-                dot[4] = fma(rh[e], z[e], dot[4]);
+                x[e] = fma(al, p[e], x[e]);
+                x[e] = fma(om, q[e], x[e]);
+                r[e] = fma(-om, y[e], q[e]);
+                dot[0] = fma(r[e], r[e], dot[0]);
+                dot[1] = fma(rh[e], r[e], dot[1]);
             }
-            st2(a.w, i, two, w);
+            st2x(xs, i, two, xs_al, x); st2(a.r, i, two, r);
+            if constexpr (PIPE) {
+                double t[2], v[2], w[2], s[2], z[2];
+                ld2(a.t, i, two, t); ld2(a.v, i, two, v); ld2(a.s, i, two, s); ld2(a.z, i, two, z);
+                for (int e = 0; e < ne; ++e) {
+                    t[e] = fma(-al, v[e], t[e]);        // t itself is overwritten by t = (A + sigma I) w next
+                    w[e] = fma(-om, t[e], y[e]);
+                    dot[2] = fma(rh[e], w[e], dot[2]);
+                    dot[3] = fma(rh[e], s[e], dot[3]);
+                    dot[4] = fma(rh[e], z[e], dot[4]);
+                }
+                st2(a.w, i, two, w);
+            }
         }
         if (!two) { q[1] = 0.0; o[1] = 0.0; }
 #pragma unroll 2
         for (int t = 0; t < na; ++t) {
             const double *c = s_coef + (size_t)t * LOP_COEF;
-            const size_t j = (size_t)(t < seed ? t : t + 1);
+            const size_t j = (size_t)(t0 + t < seed ? t0 + t : t0 + t + 1);
             double *xj = a.x_set + j * a.xstride + i, *pj = a.p_set + j * a.stride + i;
             const bool xa = XA || aligned16(xj);
             double xv[2], pv[2];
@@ -286,6 +285,30 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
             st2x(xj, 0, two, xa, xv); st2(pj, 0, two, pv);
         }
     }
+}
+template <bool PIPE, bool XA>
+__global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ LopVec a)
+{
+    const LopDev *sd = a.sd;
+    if (sd->done) return;
+    constexpr int ND = PIPE ? 5 : 2;
+    __shared__ double scratch[32 * MAX_DOTS];
+    extern __shared__ double s_coef[];                  // [chunk][LOP_COEF]
+    const int n_shift = a.L - 1;
+    double dot[ND];
+#pragma unroll
+    for (int d = 0; d < ND; ++d) dot[d] = 0.0;
+    for (int t0 = 0;; t0 += a.chunk) {
+        const int na = min(a.chunk, n_shift - t0);
+        __syncthreads();                                // the previous pass is done with the table
+        for (int t = threadIdx.x; t < na * LOP_COEF; t += blockDim.x) s_coef[t] = sd->coef[(size_t)t0 * LOP_COEF + t];
+        __syncthreads();
+        if (t0 + na >= n_shift) {
+            lop_rows<PIPE, XA, true>(a, s_coef, t0, na, dot);
+            break;
+        }
+        lop_rows<PIPE, XA, false>(a, s_coef, t0, na, dot);
+    }
     block_sum<ND>(dot, scratch);
     kernel_tail<ND>(a.kc, dot, scratch);
 }
@@ -296,7 +319,6 @@ struct LopRun : PhaseLauncher {
     bool pipe = false;
     bool xa = true;                                     // every x_j block 16-byte aligned: lop_vec_update<PIPE, true>
     int ugrid = 1;                                      // grid of lop_vec_update
-    size_t smem = 0;                                    // its coefficient table
     using PhaseLauncher::PhaseLauncher;
 
     LopVec vargs(TailDesc tail) const
@@ -309,12 +331,15 @@ struct LopRun : PhaseLauncher {
     {
         const int G = m->vgrid;
         lop_vec_init<<<G, 256, 0, c.stream>>>(vargs(tail_store(1)), pipe ? 1 : 0);
+        check_launch("lop_vec_init");
         lop_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc, pipe ? 1 : 0);
+        check_launch("lop_scalar_init");
         c.launches += 2;
         if (!pipe) { vec(PH_PUSH, tail_none(), V_P); return; }
         vec(PH_PUSH, tail_none(), V_R);
         spmv(V_R, V_W, tail_store(1), 1, m->vec(V_R), nullptr);                         // w = (A + sigma I) r, (r,w)  :765-767
         lop_scalar_pipe_init<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                       :787
+        check_launch("lop_scalar_pipe_init");
         vec(PH_PUSH, tail_none(), V_W);
         spmv(V_W, V_T, tail_none());                                                   // t = (A + sigma I) w          :769-770
         c.launches += 1;
@@ -322,29 +347,40 @@ struct LopRun : PhaseLauncher {
     void iteration()
     {
         const int G = m->vgrid;
+        const size_t smem = (size_t)base.chunk * LOP_COEF * sizeof(double);
         if (!pipe) {
             spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), nullptr);                    // s = (A + sigma I) p, (r#,s)   :261-263
             lop_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                        :276
+            check_launch("lop_scalar_alpha");
             lop_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // r_old, q                     :271, 277
+            check_launch("lop_vec_q");
             vec(PH_PUSH, tail_none(), V_R);
             spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);   // y = (A + sigma I) q, (q,q), (q,y)  :278-282
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            check_launch("lop_scalar_shift");
             if (xa) lop_vec_update<false, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
             else lop_vec_update<false, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            check_launch("lop_vec_update");
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
+            check_launch("lop_scalar_end");
             lop_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // p[seed]                      :319-321
+            check_launch("lop_vec_p");
             vec(PH_PUSH, tail_none(), V_P);
             c.launches += 6;
         } else {
             lop_vec_pipe1<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));              // p, s, z, q, y, (q,y), (y,y)   :795-814
+            check_launch("lop_vec_pipe1");
             vec(PH_PUSH, tail_none(), V_Z);
             spmv(V_Z, V_V, tail_none());                                               // v = (A + sigma I) z           :815-816
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            check_launch("lop_scalar_shift");
             if (xa) lop_vec_update<true, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
             else lop_vec_update<true, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            check_launch("lop_vec_update");
             vec(PH_PUSH, tail_none(), V_W);
             spmv(V_W, V_T, tail_none());                                               // t = (A + sigma I) w           :850-851
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 1);                   // beta, alpha, loop test       :857-865
+            check_launch("lop_scalar_end");
             c.launches += 4;
         }
     }
@@ -387,13 +423,10 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     run.base.n = n; run.base.L = L;
     run.xa = s.x_aligned();
     run.ugrid = std::max(1, std::min(c.sm_count * 8, (n + 511) / 512));
-    run.smem = (size_t)(L - 1) * LOP_COEF * sizeof(double);
-    if (run.smem > 48 * 1024) {
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
-        BICG_CUDA(cudaFuncSetAttribute(lop_vec_update<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)run.smem));
-    }
+    constexpr size_t entry = LOP_COEF * sizeof(double);
+    const int chunk = pipe ? (run.xa ? table_chunk(lop_vec_update<true, true>, entry) : table_chunk(lop_vec_update<true, false>, entry))
+                           : (run.xa ? table_chunk(lop_vec_update<false, true>, entry) : table_chunk(lop_vec_update<false, false>, entry));
+    run.base.chunk = std::min(L - 1, chunk);
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :237 / :759
     const LopDev out = s.finish(x_set, r, d_sd);
@@ -408,6 +441,8 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     st.converged = out.max_zeta_pi * out.max_zeta_pi * out.dot_r <= out.tol * out.tol * out.dot_zero;      // false after a NaN
     st.final_res = res;
     c.last_stats = st;
+    c.last_shift_stop.assign((size_t)L, 0);                                           // no shift stops on its own
+    c.last_shift_seed = seed;
 
     if (c.rank == 0 && !c.cfg.quiet) {                                                // :339-346 / :882-889
         printf("Total iter   : %d\n", k);

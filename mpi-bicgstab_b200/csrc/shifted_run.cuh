@@ -19,6 +19,23 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
 int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
               bool dev);
 
+// After each launch of a shifted solver's own kernels: a launch that fails (its configuration, its shared memory) is reported
+// at that kernel instead of at the next checked launch.
+inline void check_launch(const char *kernel)
+{
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) fatal("bicgstab_b200: %s launch failed: %s", kernel, cudaGetErrorString(e));
+}
+// Shifts per pass of an update kernel whose coefficient table in dynamic shared memory takes `entry` bytes per shift: as many
+// as fit, next to the kernel's static shared memory, into the 48 KB a block gets without opting in to more.  The kernel walks
+// its rows once per pass, so any number of shifts works with one launch configuration.
+template <class Kernel> int table_chunk(Kernel kernel, size_t entry)
+{
+    cudaFuncAttributes fa{};
+    BICG_CUDA(cudaFuncGetAttributes(&fa, kernel));
+    return std::max(1, (int)((48 * 1024 - fa.sharedSizeBytes) / entry));
+}
+
 struct ShiftedSolve {
     static constexpr int U = 8, DEPTH = 2;   // iterations per batch; batches enqueued ahead of the done flag the host reads
     bicg_matrix *m;
