@@ -3,9 +3,10 @@
 //
 // One seed system is iterated with BiCGStab on the arena vectors with the same fused SpMV (+ sigma_seed x in the
 // epilogue) and reduction tails as the un-shifted solvers; every other shift is advanced from the seed's Krylov data:
-//   * the per-shift scalar recurrences (eta, pi, zeta, alpha_j, omega_j, beta_j; :431-445), the convergence tests
-//     (:451-476) and the seed switch (:490-527, history of alpha / beta / omega / pi re-derived for the new seed) run in
-//     ONE small kernel per iteration (sh_scalar_iter), entirely on the device;
+//   * the per-shift scalar recurrences (eta, pi, zeta, alpha_j, omega_j, beta_j; :431-445; all but beta_j through
+//     shift_step of shifted_run.cuh), the convergence tests (:451-476) and the seed switch (:490-527, history of alpha /
+//     beta / omega / pi re-derived for the new seed) run in ONE small kernel per iteration (sh_scalar_iter), entirely on
+//     the device;
 //   * the six daxpy / dscal passes per shift and iteration of the reference (:435-445: up to 512 shifts x 6 passes over
 //     length-n vectors) are ONE multi-vector kernel (sh_vec_shift): q, r_old and r are loaded once per row, then x_j and
 //     p_j of every active shift are read and written exactly once -- 32 B per row and shift, the HBM floor of the method.
@@ -111,23 +112,17 @@ __global__ void __launch_bounds__(512) sh_scalar_iter(ShiftDev *sd, Scalars *sc)
     const double al_o = sd->alpha_arch[k - 1], be_o = sd->beta_arch[k - 1], sg_s = sd->sigma[seed];
     for (int j = t; j < L; j += T) {                                                // :429-446 (scalars; vectors: sh_vec_shift)
         if (j == seed || sd->stop_flag[j]) continue;
-        const double pi_o = PI(j, k - 1), zeta_o = sd->zeta_set[j];
-        const double eta = (be_o / al_o) * al_k * sd->eta_set[j] - (sg_s - sd->sigma[j]) * al_k * pi_o;
-        const double pi_n = eta + pi_o;
-        const double al_j = (pi_o / pi_n) * al_k;
-        const double om_j = om_k / (1.0 - om_k * (sg_s - sd->sigma[j]));
-        const double c1 = om_j / (pi_n * zeta_o);
-        const double c2 = om_j / (al_j * zeta_o * pi_n);
-        const double c3 = -om_j / (al_j * zeta_o * pi_o);
-        const double zeta_n = (1.0 - om_k * (sg_s - sd->sigma[j])) * zeta_o;
-        const double be_j = (pi_o / pi_n) * (pi_o / pi_n) * be_k;
-        const double c4 = 1.0 / (pi_n * zeta_n);
-        sd->eta_set[j] = eta; PI(j, k) = pi_n; sd->alpha_set[j] = al_j; sd->omega_set[j] = om_j;
-        sd->zeta_set[j] = zeta_n; sd->beta_set[j] = be_j;
+        const double pi_o = PI(j, k - 1);
+        const ShiftStep u = shift_step(al_k, al_o, be_o, om_k, sg_s - sd->sigma[j], sd->eta_set[j], pi_o, sd->zeta_set[j]);
+        // p_j is scaled at the end of this iteration, so with this iteration's beta, pi and zeta (:442-445)
+        const double be_j = (pi_o / u.pi) * (pi_o / u.pi) * be_k;
+        const double c4 = 1.0 / (u.pi * u.zeta);
+        sd->eta_set[j] = u.eta; PI(j, k) = u.pi; sd->alpha_set[j] = u.alpha; sd->omega_set[j] = u.omega;
+        sd->zeta_set[j] = u.zeta; sd->beta_set[j] = be_j;
         const int slot = atomicAdd(&s_n, 1);
         sd->active[slot] = j;
         double *c = sd->coef + (size_t)slot * SH_COEF;
-        c[0] = c1; c[1] = al_j; c[2] = c2; c[3] = c3; c[4] = be_j; c[5] = c4;
+        c[0] = u.c1; c[1] = u.alpha; c[2] = u.c2; c[3] = u.c3; c[4] = be_j; c[5] = c4;
     }
     __syncthreads();
     if (t == 0) {
@@ -254,13 +249,9 @@ __global__ void __launch_bounds__(256) sh_vec_xr(const __grid_constant__ ShVec a
 }
 // all active shifts at once                                                                            :435-445
 //   x_j += c1 q + alpha_j p_j ;  p_j += c2 q + c3 r_old ;  p_j = beta_j p_j + c4 r
-// Two rows per thread.  p_j moves as one 16-byte access; so does x_j when its block starts 16-byte aligned.  A caller's
-// device x_set has blocks of n doubles from any 8-byte aligned base, so a block may not be: then x_j moves as two 8-byte
-// accesses.  i is even, so the choice depends on the shift alone and is the same for the whole warp.  XA: the host found
-// every block aligned (always so for a host x_set) and the test is compiled out.
+// Two rows per thread, moved by the row-pair accesses of shifted_run.cuh.
 // The active shifts go in passes of a.chunk: each pass loads their coefficients into shared memory and walks the rows.  A shift
 // is updated in exactly one pass, with the same operations, so the number of passes does not change any result.
-template <bool XA>
 __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVec a)
 {
     const ShiftDev *sd = a.sd;
@@ -276,30 +267,21 @@ __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVe
         __syncthreads();
         for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
             const bool two = i + 1 < a.n;
-            double q0 = a.qc[i], q1 = two ? a.qc[i + 1] : 0.0;
-            double o0 = a.rold[i], o1 = two ? a.rold[i + 1] : 0.0;
-            double r0 = a.r[i], r1 = two ? a.r[i + 1] : 0.0;
+            double q[2], o[2], r[2];
+            ld2(a.qc, i, two, q); ld2(a.rold, i, two, o); ld2(a.r, i, two, r);
 #pragma unroll 2
             for (int t = 0; t < na; ++t) {
                 const double *c = s_coef + (size_t)t * SH_COEF;
                 double *xj = a.x_set + (size_t)s_idx[t] * a.xstride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
-                const bool xa = XA || (reinterpret_cast<size_t>(xj) & 15) == 0;
-                double x0, x1, p0, p1;
-                if (two) {
-                    const double2 pv = *reinterpret_cast<const double2 *>(pj);
-                    p0 = pv.x; p1 = pv.y;
-                    if (xa) { const double2 xv = *reinterpret_cast<const double2 *>(xj); x0 = xv.x; x1 = xv.y; }
-                    else { x0 = xj[0]; x1 = xj[1]; }
-                } else { x0 = xj[0]; p0 = pj[0]; x1 = p1 = 0.0; }
-                x0 = fma(c[0], q0, x0); x0 = fma(c[1], p0, x0);
-                x1 = fma(c[0], q1, x1); x1 = fma(c[1], p1, x1);
-                p0 = fma(c[2], q0, p0); p0 = fma(c[3], o0, p0); p0 = c[4] * p0; p0 = fma(c[5], r0, p0);
-                p1 = fma(c[2], q1, p1); p1 = fma(c[3], o1, p1); p1 = c[4] * p1; p1 = fma(c[5], r1, p1);
-                if (two) {
-                    if (xa) *reinterpret_cast<double2 *>(xj) = make_double2(x0, x1);
-                    else { xj[0] = x0; xj[1] = x1; }
-                    *reinterpret_cast<double2 *>(pj) = make_double2(p0, p1);
-                } else { xj[0] = x0; pj[0] = p0; }
+                const bool xa = aligned16(xj);
+                double x[2], p[2];
+                ld2x(xj, 0, two, xa, x); ld2(pj, 0, two, p);
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                    x[e] = fma(c[0], q[e], x[e]); x[e] = fma(c[1], p[e], x[e]);
+                    p[e] = fma(c[2], q[e], p[e]); p[e] = fma(c[3], o[e], p[e]); p[e] = c[4] * p[e]; p[e] = fma(c[5], r[e], p[e]);
+                }
+                st2x(xj, 0, two, xa, x); st2(pj, 0, two, p);
             }
         }
     }
@@ -331,7 +313,7 @@ __global__ void __launch_bounds__(256) sh_vec_p(const __grid_constant__ ShVec a)
 struct ShRun : PhaseLauncher {
     ShiftDev *d_sd = nullptr;
     ShVec base{};
-    bool xa = true;                                  // every x_j block 16-byte aligned: sh_vec_shift<true>
+    int ugrid = 1;                                   // grid of sh_vec_shift
     using PhaseLauncher::PhaseLauncher;
 
     ShVec vargs(TailDesc tail) const
@@ -366,10 +348,7 @@ struct ShRun : PhaseLauncher {
         check_launch("sh_vec_xr");
         sh_scalar_iter<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                       // beta ... loop test          :420, 429-537
         check_launch("sh_scalar_iter");
-        const size_t smem = (size_t)base.chunk * SH_ENTRY;
-        const int sgrid = std::max(1, std::min(c.sm_count * 8, (m->n_loc + 511) / 512));
-        if (xa) sh_vec_shift<true><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
-        else sh_vec_shift<false><<<sgrid, 256, smem, c.stream>>>(vargs(tail_none()));
+        sh_vec_shift<<<ugrid, 256, (size_t)base.chunk * SH_ENTRY, c.stream>>>(vargs(tail_none()));   // x_j, p_j   :435-445
         check_launch("sh_vec_shift");
         sh_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // p[seed] (or the switch)     :421-423 / :499
         check_launch("sh_vec_p");
@@ -420,8 +399,8 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);
     run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
     run.base.n = n; run.base.L = L;
-    run.xa = s.x_aligned();
-    run.base.chunk = std::min(L, run.xa ? table_chunk(sh_vec_shift<true>, SH_ENTRY) : table_chunk(sh_vec_shift<false>, SH_ENTRY));
+    run.ugrid = s.update_grid();
+    run.base.chunk = std::min(L, table_chunk(sh_vec_shift, SH_ENTRY));
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :364
     const ShiftDev out = s.finish(x_set, r, d_sd);

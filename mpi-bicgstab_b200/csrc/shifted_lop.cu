@@ -6,10 +6,10 @@
 // max_zeta_pi^2 dot_r <= tol^2 dot_zero (max_zeta_pi = max(1, max_j |1 / (zeta_j pi_j)|)) or MAX_ITER.
 //
 // Per iteration the seed runs on the arena vectors with the shifted SpMV epilogue (y = A x + sigma_seed x, PhaseLauncher),
-// one scalar kernel derives every shift's coefficients (lop_scalar_shift), and ONE fused pass (lop_vec_update) updates the
-// seed's x and residual together with x_j and p_j of every shift, each read and written exactly once (32 B per row and
-// shift).  The reference scales p_j at the START of an iteration (p_j = beta_j p_j + r / (pi zeta), :264-269); that step is
-// moved into the same pass, where r of the iteration start is r_old, so the pass does
+// one scalar kernel derives every shift's coefficients (lop_scalar_shift, with shift_step of shifted_run.cuh), and ONE fused
+// pass (lop_vec_update) updates the seed's x and residual together with x_j and p_j of every shift, each read and written
+// exactly once (32 B per row and shift).  The reference scales p_j at the START of an iteration (p_j = beta_j p_j + r /
+// (pi zeta), :264-269); that step is moved into the same pass, where r of the iteration start is r_old, so the pass does
 //   p_j = beta_j p_j + c4 r_old ;  x_j += c1 q + alpha_j p_j ;  p_j += c2 q + c3 r_old
 // with the reference's operands and operation order.  Iteration 1 starts from p_j = 0, beta_j = 0, c4 = 1: p_j = r exactly.
 // Element-wise order = the reference's call order with gcc's FMA contraction (y += a x -> fma(a, x, y)).
@@ -81,21 +81,15 @@ __global__ void __launch_bounds__(512) lop_scalar_shift(LopDev *sd, Scalars *sc)
     double mx = 1.0;
     for (int s = t; s < sd->L - 1; s += T) {
         const int j = s < seed ? s : s + 1;
-        const double pi_oo = sd->pi_old[j], pi_o = sd->pi_new[j], zeta_o = sd->zeta[j], dsg = sg_s - sd->sigma[j];
+        const double pi_oo = sd->pi_old[j], pi_o = sd->pi_new[j], zeta_o = sd->zeta[j];
+        // p_j is scaled at the start of this iteration, so with the previous iteration's beta, pi and zeta (:264-269 / :804-809)
         const double be_j = (pi_oo / pi_o) * (pi_oo / pi_o) * be_o;              // :266 / :806
         const double c4 = 1.0 / (pi_o * zeta_o);                                // :268 / :808
-        const double eta = (be_o / al_o) * al * sd->eta[j] - dsg * al * pi_o;    // :285 / :821 (pi_old <- pi_new, :270 / :817)
-        const double pi_n = eta + pi_o;                                         // :287 / :823
-        const double al_j = (pi_o / pi_n) * al;                                 // :288 / :824
-        const double om_j = om / (1.0 - om * dsg);                              // :298 / :834
-        const double c1 = om_j / (pi_n * zeta_o);                               // :299 / :835
-        const double c2 = om_j / (al_j * zeta_o * pi_n);                        // :301 / :837
-        const double c3 = -om_j / (al_j * zeta_o * pi_o);                       // :302 / :838
-        const double zeta_n = (1.0 - om * dsg) * zeta_o;                        // :303 / :839
-        sd->eta[j] = eta; sd->pi_old[j] = pi_o; sd->pi_new[j] = pi_n; sd->zeta[j] = zeta_n;
+        const ShiftStep u = shift_step(al, al_o, be_o, om, sg_s - sd->sigma[j], sd->eta[j], pi_o, zeta_o);
+        sd->eta[j] = u.eta; sd->pi_old[j] = pi_o; sd->pi_new[j] = u.pi; sd->zeta[j] = u.zeta;    // pi_old <- pi_new, :270 / :817
         double *c = sd->coef + (size_t)s * LOP_COEF;
-        c[0] = be_j; c[1] = c4; c[2] = c1; c[3] = al_j; c[4] = c2; c[5] = c3;
-        const double azp = fabs(1.0 / (zeta_n * pi_n));                         // :316 / :863
+        c[0] = be_j; c[1] = c4; c[2] = u.c1; c[3] = u.alpha; c[4] = u.c2; c[5] = u.c3;
+        const double azp = fabs(1.0 / (u.zeta * u.pi));                         // :316 / :863
         if (azp > mx) mx = azp;
     }
     for (int o = 16; o > 0; o >>= 1) { const double v = __shfl_xor_sync(0xffffffffu, mx, o); if (v > mx) mx = v; }
@@ -138,30 +132,6 @@ struct LopVec {
     int n, L;
     int chunk;                                          // non-seed shifts per pass of lop_vec_update, the size of its table
 };
-
-__device__ __forceinline__ void ld2(const double *p, int i, bool two, double (&v)[2])
-{
-    if (two) { const double2 t = *reinterpret_cast<const double2 *>(p + i); v[0] = t.x; v[1] = t.y; }
-    else { v[0] = p[i]; v[1] = 0.0; }
-}
-__device__ __forceinline__ void st2(double *p, int i, bool two, const double (&v)[2])
-{
-    if (two) *reinterpret_cast<double2 *>(p + i) = make_double2(v[0], v[1]);
-    else p[i] = v[0];
-}
-// the same for a block of x_set, which starts 16-byte aligned (al) or only 8-byte aligned: a caller's device x_set has blocks of
-// n doubles from any 8-byte aligned base; then the pair moves as two 8-byte accesses
-__device__ __forceinline__ void ld2x(const double *p, int i, bool two, bool al, double (&v)[2])
-{
-    if (two && !al) { v[0] = p[i]; v[1] = p[i + 1]; }
-    else ld2(p, i, two, v);
-}
-__device__ __forceinline__ void st2x(double *p, int i, bool two, bool al, const double (&v)[2])
-{
-    if (two && !al) { p[i] = v[0]; p[i + 1] = v[1]; }
-    else st2(p, i, two, v);
-}
-__device__ __forceinline__ bool aligned16(const double *p) { return (reinterpret_cast<size_t>(p) & 15) == 0; }
 
 // r# = r, p[seed] = r, (r,r); PIPE-LOP also zeroes s, z, v (pinned, see the top)          :240-252 / :763, 772-782
 __global__ void __launch_bounds__(256) lop_vec_init(const __grid_constant__ LopVec a, int pipe)
@@ -218,9 +188,8 @@ __global__ void __launch_bounds__(256) lop_vec_pipe1(const __grid_constant__ Lop
     block_sum<2>(dot, scratch);
     kernel_tail<2>(a.kc, dot, scratch);
 }
-// The seed's x and residual and every shift's x_j, p_j in one pass over the rows (two rows per thread, 16-byte accesses; an
-// x_set block that does not start 16-byte aligned takes two 8-byte accesses instead -- i is even, so that choice depends on
-// the shift alone and is the same for the whole warp; XA: the host found every block aligned and the test is compiled out).
+// The seed's x and residual and every shift's x_j, p_j in one pass over the rows (two rows per thread, moved by the row-pair
+// accesses of shifted_run.cuh).
 //   seed   x[seed] += alpha p + omega q; r = q - omega y                                   :294-295, 305 / :830-831, 841
 //          PIPE-LOP: w = y - omega (t - alpha v)                                          :843-844
 //   shifts p_j = beta_j p_j + c4 r_old; x_j += c1 q + alpha_j p_j; p_j += c2 q + c3 r_old   :267-268, 299-302 / :807-808, 835-838
@@ -229,14 +198,14 @@ __global__ void __launch_bounds__(256) lop_vec_pipe1(const __grid_constant__ Lop
 // The non-seed shifts go in passes of a.chunk, each of which loads their coefficients into shared memory and walks the rows;
 // the seed is updated in the last pass, because that overwrites q (in r), which every earlier pass reads.  A shift is updated
 // in exactly one pass, with the same operations, so the number of passes does not change any result.
-template <bool PIPE, bool XA, bool SEED>
+template <bool PIPE, bool SEED>
 __device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, int t0, int na, double (&dot)[PIPE ? 5 : 2])
 {
     const LopDev *sd = a.sd;
     const int seed = sd->seed;
     const double al = sd->alpha, om = sd->omega;
     double *xs = a.x_set + (size_t)seed * a.xstride;
-    const bool xs_al = XA || aligned16(xs);
+    const bool xs_al = aligned16(xs);
     for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
         const bool two = i + 1 < a.n;                   // stride and arena vectors are 16-byte aligned, i is even
         double q[2], o[2];
@@ -273,7 +242,7 @@ __device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, 
             const double *c = s_coef + (size_t)t * LOP_COEF;
             const size_t j = (size_t)(t0 + t < seed ? t0 + t : t0 + t + 1);
             double *xj = a.x_set + j * a.xstride + i, *pj = a.p_set + j * a.stride + i;
-            const bool xa = XA || aligned16(xj);
+            const bool xa = aligned16(xj);
             double xv[2], pv[2];
             ld2x(xj, 0, two, xa, xv); ld2(pj, 0, two, pv);
 #pragma unroll
@@ -286,7 +255,7 @@ __device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, 
         }
     }
 }
-template <bool PIPE, bool XA>
+template <bool PIPE>
 __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ LopVec a)
 {
     const LopDev *sd = a.sd;
@@ -304,10 +273,10 @@ __global__ void __launch_bounds__(256) lop_vec_update(const __grid_constant__ Lo
         for (int t = threadIdx.x; t < na * LOP_COEF; t += blockDim.x) s_coef[t] = sd->coef[(size_t)t0 * LOP_COEF + t];
         __syncthreads();
         if (t0 + na >= n_shift) {
-            lop_rows<PIPE, XA, true>(a, s_coef, t0, na, dot);
+            lop_rows<PIPE, true>(a, s_coef, t0, na, dot);
             break;
         }
-        lop_rows<PIPE, XA, false>(a, s_coef, t0, na, dot);
+        lop_rows<PIPE, false>(a, s_coef, t0, na, dot);
     }
     block_sum<ND>(dot, scratch);
     kernel_tail<ND>(a.kc, dot, scratch);
@@ -317,7 +286,6 @@ struct LopRun : PhaseLauncher {
     LopDev *d_sd = nullptr;
     LopVec base{};
     bool pipe = false;
-    bool xa = true;                                     // every x_j block 16-byte aligned: lop_vec_update<PIPE, true>
     int ugrid = 1;                                      // grid of lop_vec_update
     using PhaseLauncher::PhaseLauncher;
 
@@ -358,8 +326,7 @@ struct LopRun : PhaseLauncher {
             spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);   // y = (A + sigma I) q, (q,q), (q,y)  :278-282
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
             check_launch("lop_scalar_shift");
-            if (xa) lop_vec_update<false, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
-            else lop_vec_update<false, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            lop_vec_update<false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
             check_launch("lop_vec_update");
             lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
             check_launch("lop_scalar_end");
@@ -374,8 +341,7 @@ struct LopRun : PhaseLauncher {
             spmv(V_Z, V_V, tail_none());                                               // v = (A + sigma I) z           :815-816
             lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
             check_launch("lop_scalar_shift");
-            if (xa) lop_vec_update<true, true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
-            else lop_vec_update<true, false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            lop_vec_update<true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
             check_launch("lop_vec_update");
             vec(PH_PUSH, tail_none(), V_W);
             spmv(V_W, V_T, tail_none());                                               // t = (A + sigma I) w           :850-851
@@ -421,12 +387,9 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     run.base.rold = m->vec(pipe ? V_AX : V_V);
     run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
     run.base.n = n; run.base.L = L;
-    run.xa = s.x_aligned();
-    run.ugrid = std::max(1, std::min(c.sm_count * 8, (n + 511) / 512));
+    run.ugrid = s.update_grid();
     constexpr size_t entry = LOP_COEF * sizeof(double);
-    const int chunk = pipe ? (run.xa ? table_chunk(lop_vec_update<true, true>, entry) : table_chunk(lop_vec_update<true, false>, entry))
-                           : (run.xa ? table_chunk(lop_vec_update<false, true>, entry) : table_chunk(lop_vec_update<false, false>, entry));
-    run.base.chunk = std::min(L - 1, chunk);
+    run.base.chunk = std::min(L - 1, pipe ? table_chunk(lop_vec_update<true>, entry) : table_chunk(lop_vec_update<false>, entry));
 
     s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :237 / :759
     const LopDev out = s.finish(x_set, r, d_sd);

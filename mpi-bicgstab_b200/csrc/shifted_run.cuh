@@ -1,9 +1,13 @@
-// shifted_run.cuh -- the host side every shifted solver shares (shifted.cu, shifted_lop.cu).  The seed system runs on the
-// arena vectors through PhaseLauncher (engine.hpp) with shift_sigma set, so its SpMVs compute y = (A + sigma_seed I) x, and
-// tail_store puts the reduced epilogue dots into Scalars::pend[] for the solver's own scalar kernels.  ShiftedSolve holds
-// everything around a solver's own device state and kernel sequence: the device memory the solve owns, the sigma_len
-// solutions x_j (host x_set: copied into one strided device buffer; device x_set: the caller's buffer, updated in place),
-// b in / the seed residual out through the arena's r, the timed loop and the statistics every shifted solver reports alike.
+// shifted_run.cuh -- what every shifted solver shares (shifted.cu, shifted_lop.cu).
+// Host: the seed system runs on the arena vectors through PhaseLauncher (engine.hpp) with shift_sigma set, so its SpMVs
+// compute y = (A + sigma_seed I) x, and tail_store puts the reduced epilogue dots into Scalars::pend[] for the solver's own
+// scalar kernels.  ShiftedSolve holds everything around a solver's own device state and kernel sequence: the device memory
+// the solve owns, the sigma_len solutions x_j (host x_set: copied into one strided device buffer; device x_set: the caller's
+// buffer, updated in place), b in / the seed residual out through the arena's r, the update kernels' grid, the timed loop
+// and the statistics every shifted solver reports alike.
+// Device: the per-shift scalar recurrence both families evaluate (shift_step) and the row-pair accesses their update
+// kernels move x_j and p_j with (ld2, st2, ld2x, st2x).  Each family keeps its own update loop: they apply the six
+// coefficients in different orders, and LOP folds the seed's update into its last pass.
 #pragma once
 #include "engine.hpp"
 
@@ -36,6 +40,54 @@ template <class Kernel> int table_chunk(Kernel kernel, size_t entry)
     return std::max(1, (int)((48 * 1024 - fa.sharedSizeBytes) / entry));
 }
 
+// One step of shift j's scalars from the seed's alpha_k, alpha_{k-1}, beta_{k-1}, omega_k, dsg = sigma_seed - sigma_j and
+// the shift's eta, pi, zeta (shifted_switching_solver.c:431-441; shifted_solver.c:285-303 / :821-839).  beta_j and c4 stay
+// with the callers, who take them one iteration apart.
+struct ShiftStep {
+    double eta, pi, alpha, omega, c1, c2, c3, zeta;     // eta, pi_new, alpha_j, omega_j, the update coefficients, zeta_new
+};
+__device__ __forceinline__ ShiftStep shift_step(double al, double al_o, double be_o, double om, double dsg, double eta, double pi_o,
+                                                double zeta_o)
+{
+    ShiftStep s;
+    s.eta = (be_o / al_o) * al * eta - dsg * al * pi_o;
+    s.pi = s.eta + pi_o;
+    s.alpha = (pi_o / s.pi) * al;
+    s.omega = om / (1.0 - om * dsg);
+    s.c1 = s.omega / (s.pi * zeta_o);
+    s.c2 = s.omega / (s.alpha * zeta_o * s.pi);
+    s.c3 = -s.omega / (s.alpha * zeta_o * pi_o);
+    s.zeta = (1.0 - om * dsg) * zeta_o;
+    return s;
+}
+
+// Rows i, i + 1 (two) or i alone of a vector, as one 16-byte access: the arena vectors and every p_set block start 16-byte
+// aligned, and the update kernels give each thread an even i.
+__device__ __forceinline__ void ld2(const double *p, int i, bool two, double (&v)[2])
+{
+    if (two) { const double2 t = *reinterpret_cast<const double2 *>(p + i); v[0] = t.x; v[1] = t.y; }
+    else { v[0] = p[i]; v[1] = 0.0; }
+}
+__device__ __forceinline__ void st2(double *p, int i, bool two, const double (&v)[2])
+{
+    if (two) *reinterpret_cast<double2 *>(p + i) = make_double2(v[0], v[1]);
+    else p[i] = v[0];
+}
+// The same for a block of x_set, which starts 16-byte aligned (al) or only 8-byte aligned: a caller's device x_set has blocks
+// of n doubles from any 8-byte aligned base; then the pair moves as two 8-byte accesses.  i is even, so al depends on the
+// block alone and is the same for the whole warp.
+__device__ __forceinline__ void ld2x(const double *p, int i, bool two, bool al, double (&v)[2])
+{
+    if (two && !al) { v[0] = p[i]; v[1] = p[i + 1]; }
+    else ld2(p, i, two, v);
+}
+__device__ __forceinline__ void st2x(double *p, int i, bool two, bool al, const double (&v)[2])
+{
+    if (two && !al) { p[i] = v[0]; p[i + 1] = v[1]; }
+    else st2(p, i, two, v);
+}
+__device__ __forceinline__ bool aligned16(const double *p) { return (reinterpret_cast<size_t>(p) & 15) == 0; }
+
 struct ShiftedSolve {
     static constexpr int U = 8, DEPTH = 2;   // iterations per batch; batches enqueued ahead of the done flag the host reads
     bicg_matrix *m;
@@ -57,8 +109,8 @@ struct ShiftedSolve {
     ShiftedSolve(const ShiftedSolve &) = delete;
     ShiftedSolve &operator=(const ShiftedSolve &) = delete;
 
-    // every x_j block starts 16-byte aligned (always for a host x_set): the update kernels' XA = true variant applies
-    bool x_aligned() const { return xstride % 2 == 0 && (reinterpret_cast<size_t>(d_x) & 15) == 0; }
+    // grid of the per-shift update kernels (sh_vec_shift, lop_vec_update): 256 threads of two rows each
+    int update_grid() const { return std::max(1, std::min(c.sm_count * 8, (n + 511) / 512)); }
     template <class T> T *alloc(size_t count)       // device memory freed when the solve ends
     {
         void *p = c.dev_alloc(std::max<size_t>(count * sizeof(T), 16));
