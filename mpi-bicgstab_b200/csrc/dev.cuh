@@ -134,28 +134,24 @@ __device__ __forceinline__ void tma_load_1d(unsigned dst_smem, const void *src, 
                  ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
 
+__device__ __forceinline__ void mbar_arrive(unsigned bar)
+{
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+// named CTA barrier over the first `nthreads` threads: the producer warp of a warp-specialised kernel free-runs
+__device__ __forceinline__ void nbar(int id, int nthreads)
+{
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
 __device__ __forceinline__ void st_release_sys(unsigned long long *p, unsigned long long v)
 {
     asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void st_flag_sys(unsigned long long *p, unsigned long long v)
-{
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 __device__ __forceinline__ unsigned long long ld_acquire_sys(const unsigned long long *p)
 {
     unsigned long long v;
     asm volatile("ld.acquire.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void st_release_gpu(unsigned *p, unsigned v)
-{
-    asm volatile("st.release.gpu.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ unsigned ld_acquire_gpu(const unsigned *p)
-{
-    unsigned v;
-    asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
 // ---- LL words: {flag32 | data32}; a double travels as two of them ------------------------------------------
@@ -200,12 +196,6 @@ __device__ __forceinline__ void ld_ll_gpu2(const unsigned long long *p, unsigned
 {
     asm volatile("ld.relaxed.gpu.global.v2.b64 {%0, %1}, [%2];" : "=l"(w0), "=l"(w1) : "l"(p) : "memory");
 }
-__device__ __forceinline__ unsigned long long ld_relaxed_sys(const unsigned long long *p)
-{
-    unsigned long long v;
-    asm volatile("ld.relaxed.sys.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ void fence_gpu() { asm volatile("fence.acq_rel.gpu;" ::: "memory"); }
 __device__ __forceinline__ void fence_sys() { asm volatile("fence.acq_rel.sys;" ::: "memory"); }
 // plain ld.global: L1-cached but never the non-coherent (.nc) path -- for vectors that other SMs / peer GPUs rewrite
@@ -216,21 +206,12 @@ __device__ __forceinline__ double ld_coherent(const double *p)
     asm volatile("ld.global.f64 %0, [%1];" : "=d"(v) : "l"(p));
     return v;
 }
-__device__ __forceinline__ double ld_volatile_f64(const double *p)
-{
-    double v;
-    asm volatile("ld.volatile.global.f64 %0, [%1];" : "=d"(v) : "l"(p) : "memory");
-    return v;
-}
 __device__ __forceinline__ unsigned long long globaltimer_ns()
 {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
     return t;
 }
-
-constexpr unsigned long long PEER_TIMEOUT_NS = 20000000000ull;  // default bound (20 s): a lost peer must not hang the GPU, but
-                                                                // ordinary host-side skew between ranks must not kill the job
 
 // ------------------------------------------------------------------------------------------------
 // reductions
@@ -240,6 +221,61 @@ __device__ __forceinline__ double warp_sum(double v)
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+// sum over the LANES consecutive threads that share one row (butterfly: every one of them gets the sum)
+template <int LANES>
+__device__ __forceinline__ double lanes_sum(double v)
+{
+#pragma unroll
+    for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// ------------------------------------------------------------------------------------------------
+// TMA-fed CSR SpMV: what the stand-alone spmv_ws_kernel (spmv.cu) and the persistent kernel (mega.cu) share
+// ------------------------------------------------------------------------------------------------
+constexpr int PROW_PAD = 8;       // extra ptr / epilogue slots per stage for the 16-byte alignment window
+
+// The part of the arrays that one tile of rows [row0, row1) with entries [p0, p1) puts into a stage: entries
+// [a0, a0 + cnt) and row pointers [rowa, rowa + cntp), widened to whole 16-byte units for the bulk copies.  `al` is the
+// alignment mask of the entry window: 3 for 4-byte columns, 7 for 2-byte column codes.
+struct TileWindow { unsigned a0, cnt; int rowa, cntp; };
+__device__ __forceinline__ TileWindow tile_window(int row0, int row1, unsigned p0, unsigned p1, unsigned al)
+{
+    TileWindow w;
+    w.a0 = p0 & ~al;
+    w.cnt = ((p1 + al) & ~al) - w.a0;
+    w.rowa = row0 & ~3;
+    w.cntp = ((row1 + 1 + 3) & ~3) - w.rowa;
+    return w;
+}
+
+// One row's product with x over the staged entries [j, e) (j already includes the thread's offset in its group of
+// LANES), summed over the group.  This loop decides the bits of y: entries in storage order, one fma each, then
+// lanes_sum.  UNR gathers are in flight per thread; `column(idx)` returns the column of staged entry idx.
+template <int LANES, int UNR, class Column>
+__device__ __forceinline__ double row_product(const double *sval, Column column, const double *x, int j, int e)
+{
+    double acc = 0.0;
+    while (j < e) {
+        unsigned c[UNR];
+        double v[UNR], xv[UNR];
+#pragma unroll
+        for (int u = 0; u < UNR; ++u) {
+            // clamp instead of predicating: unconditional loads batch freely (a predicated load per slot runs out
+            // of predicate registers after 7); the FMA below is what is predicated
+            const int idx = min(j + u * LANES, e - 1);
+            c[u] = column(idx);
+            v[u] = sval[idx];
+        }
+#pragma unroll
+        for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
+#pragma unroll
+        for (int u = 0; u < UNR; ++u)
+            if (j + u * LANES < e) acc = fma(v[u], xv[u], acc);
+        j += UNR * LANES;
+    }
+    return lanes_sum<LANES>(acc);
 }
 
 // Sum N per-thread values over the CTA.  Result is valid in every lane of warp 0.  `scratch` holds
@@ -406,13 +442,10 @@ __device__ __forceinline__ bool halo_wait_epoch(const CommDev &c, unsigned expec
     return __all_sync(0xffffffffu, ok);
 }
 
-__device__ __forceinline__ bool halo_wait(const CommDev &c, unsigned expect) { return halo_wait_epoch(c, expect); }
-
 // What the elected warp does once the grid's dots are combined: `tot` holds the totals in every lane.
-// Runs the TailDesc (cross-GPU reduction over the peer mailboxes, scalar recurrence, halo-ready signal) and, when
-// wait_halo is set (persistent kernel), also waits for the peers' halo signal of the same epoch.
+// Runs the TailDesc: cross-GPU reduction over the peer mailboxes, scalar recurrence, halo-ready signal to the peers.
 template <int NDOT>
-__device__ __forceinline__ void tail_warp(const KernelCommon &kc, double (&tot)[NDOT > 0 ? NDOT : 1], bool wait_halo)
+__device__ __forceinline__ void tail_warp(const KernelCommon &kc, double (&tot)[NDOT > 0 ? NDOT : 1])
 {
     Scalars *sc = kc.sc;
     const int tid = threadIdx.x & 31;
@@ -471,7 +504,6 @@ __device__ __forceinline__ void tail_warp(const KernelCommon &kc, double (&tot)[
         if (lane < kc.comm.world && ((kc.comm.send_mask >> lane) & 1u))
             st_release_sys(&kc.comm.hflag[lane][kc.comm.rank].epoch, (unsigned long long)he);
         __syncwarp();
-        if (wait_halo && !halo_wait_epoch(kc.comm, he) && lane == 0) { sc->error = 1; sc->done = 1; }
         if (lane == 0) sc->halo_epoch = he;
     }
 }
@@ -515,7 +547,7 @@ __device__ __forceinline__ void kernel_tail(const KernelCommon &kc, double (&loc
         block_sum<(NDOT > 0 ? NDOT : 1)>(tot, scratch);
     }
     if (tid >= 32) return;                       // warp 0 finishes the job
-    tail_warp<NDOT>(kc, tot, false);
+    tail_warp<NDOT>(kc, tot);
     if (tid == 0) { __threadfence(); sc->ticket = 0u; }
 }
 

@@ -31,7 +31,7 @@
 // Coherence: gathered vectors are read with plain (L1-cached) loads; every neighbour wait ends in an acquire fence at gpu
 // scope (SASS: MEMBAR + CCTL.IVALL), so rows rewritten by other SMs are re-fetched from L2; values from peers are taken
 // from the LL words with system-scope loads and re-stored locally by the consuming CTA.
-// Every wait is bounded by CommDev::timeout_ns (BICG_PEER_TIMEOUT_S): a lost CTA or rank raises Scalars::error instead of hanging the GPU.
+// Every wait is bounded (BICG_PEER_TIMEOUT_S, Mega::timed_out): a lost CTA or rank raises Scalars::error instead of hanging the GPU.
 #include "mega.cuh"
 #include "vec_body.cuh"
 
@@ -39,19 +39,10 @@ namespace bicg {
 
 namespace {
 
-constexpr int PROW_PAD = 8;
 constexpr int RED_THREADS = MEGA_MAX_CTAS;          // one polled slot per thread
 constexpr int RED_WARPS = RED_THREADS / 32;
 struct StageHdr { int row0, row1; unsigned a0; int rowa; unsigned lo, hi; int flag; int pad_; };   // lo, hi: the tile's entries relative to a0
 
-__device__ __forceinline__ void mbar_arrive(unsigned bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void nbar(int id, int nthreads)  // named CTA barrier (the producer warp free-runs)
-{
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
 __device__ __forceinline__ unsigned long long l2_evict_first_policy()
 {
     unsigned long long pol;
@@ -70,13 +61,6 @@ __device__ __forceinline__ void tma_load_1d_hint(unsigned dst_smem, const void *
 __device__ __forceinline__ void poll_pause(unsigned spins)
 {
     if (spins > 2u) __nanosleep(spins > 16u ? 256u : (spins > 6u ? 128u : 64u));
-}
-template <int LANES>
-__device__ __forceinline__ double lanes_sum(double v)
-{
-#pragma unroll
-    for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
 }
 
 // CTA-wide sum over the consumer threads only; result valid in every lane of warp 0
@@ -198,6 +182,12 @@ struct Mega {
 
     __device__ bool stop_now() const { return sh.sc.done != 0 || sh.sc.error != 0; }
     __device__ void fail() { sh.flags[3] = 1; }
+    // the bound of every wait of this kernel: t0 = globaltimer_ns() when the wait began; the clock is read on every 256th
+    // probe only, and a wait that sees true calls fail() and stops polling
+    __device__ __forceinline__ bool timed_out(unsigned long long t0, unsigned spins) const
+    {
+        return (spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns;
+    }
     // one iteration's alpha sync seen by EVERY CTA: [G][2] = arrival, release (globaltimer, per GPU)
     __device__ void snap(int which)
     {
@@ -253,7 +243,7 @@ struct Mega {
                 unsigned spins = 0;
                 while ((unsigned)(ld_ll_gpu(&ring[c].w[0]) >> 32) != gen) {
                     poll_pause(++spins);
-                    if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { ok = false; break; }
+                    if (timed_out(t0, spins)) { ok = false; break; }
                 }
             }
             fence_gpu();                                     // acquire (+ L1 invalidate): the gathers that follow see the data
@@ -291,7 +281,7 @@ struct Mega {
                     if (all) break;
                     ++spins;
                     if (a.comm.world == 1) poll_pause(spins);        // N > 1: only the reducer CTA polls the slots -- no crowd, no pause
-                    if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { fail(); break; }
+                    if (timed_out(t0, spins)) { fail(); break; }
                 }
 #pragma unroll
                 for (int k = 0; k < NV; ++k) v[k] = ll_decode(w0[k], w1[k]);
@@ -348,7 +338,7 @@ struct Mega {
                 for (int k = 0; k < NV; ++k) { ld_ll_sys(w + 2 * k, w0[k], w1[k]); all = all && ll_valid(w0[k], w1[k], red_epoch); }
                 if (all) break;
                 if (++spins > 4u) __nanosleep(48);                   // 8 lines polled by 132 x 8 threads: a short pause is enough
-                if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { fail(); break; }
+                if (timed_out(t0, spins)) { fail(); break; }
             }
 #pragma unroll
             for (int k = 0; k < NV; ++k) sh.contrib[lane][k] = ll_decode(w0[k], w1[k]);
@@ -419,17 +409,22 @@ struct Mega {
         if (after_spmv) {
             double d0[1] = {0.0};
             arrive<0>(d0, false);
-            if (tid < RED_THREADS && tid < (int)gridDim.x && tid != (int)blockIdx.x) {
-                const unsigned long long *w = a.sync->slot[gen & (MEGA_RING - 1)][tid].w;
-                const unsigned long long t0 = globaltimer_ns();
-                unsigned spins = 0;
-                while ((unsigned)(ld_ll_gpu(w) >> 32) != gen) {
-                    poll_pause(++spins);
-                    if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { fail(); break; }
-                }
-            }
+            wait_all();
         }
         finish<NV>(posted_gen, fin, true);
+    }
+    // wait for every other CTA of this GPU to arrive at generation gen: thread c polls CTA c's slot
+    __device__ __forceinline__ void wait_all()
+    {
+        if (tid < RED_THREADS && tid < (int)gridDim.x && tid != (int)blockIdx.x) {
+            const unsigned long long *w = a.sync->slot[gen & (MEGA_RING - 1)][tid].w;
+            const unsigned long long t0 = globaltimer_ns();
+            unsigned spins = 0;
+            while ((unsigned)(ld_ll_gpu(w) >> 32) != gen) {
+                poll_pause(++spins);
+                if (timed_out(t0, spins)) { fail(); break; }
+            }
+        }
     }
 
     // ---------------------------------------------------------------- SpMV over this CTA's tiles ----------
@@ -442,7 +437,15 @@ struct Mega {
         if (coded) spmv_impl<EPI, true>(x, y, dot);
         else spmv_impl<EPI, false>(x, y, dot);
     }
-    // one row's epilogue: y and the dots fused into the SpMV (same operations, same order as the streaming path)
+    // one row's epilogue operands (EPI_RH_Y: r#; EPI_QY_YY: q, kept in v.r; EPI_CA4: r#, r, s, z), loaded before its gathers
+    template <int EPI>
+    __device__ __forceinline__ void epi_load(int row, double &e0, double &e1, double &e2, double &e3) const
+    {
+        if (EPI == EPI_RH_Y) e0 = a.v.rh[row];
+        if (EPI == EPI_QY_YY) e0 = a.v.r[row];
+        if (EPI == EPI_CA4) { e0 = a.v.rh[row]; e1 = a.v.r[row]; e2 = a.v.s[row]; e3 = a.v.z[row]; }
+    }
+    // one row's epilogue: y and the dots fused into the SpMV; every SpMV path of this kernel ends its rows here
     template <int EPI>
     __device__ __forceinline__ void row_done(int row, double acc, double e0, double e1, double e2, double e3, double *y, double (&dot)[4])
     {
@@ -472,9 +475,7 @@ struct Mega {
             unsigned j = rs_ptr[r];
             const unsigned e = rs_ptr[r + 1];
             double e0 = 0.0, e1 = 0.0, e2 = 0.0, e3 = 0.0;     // epilogue operands: in flight during the gathers
-            if (EPI == EPI_RH_Y) e0 = a.v.rh[row];
-            if (EPI == EPI_QY_YY) e0 = a.v.r[row];
-            if (EPI == EPI_CA4) { e0 = a.v.rh[row]; e1 = a.v.r[row]; e2 = a.v.s[row]; e3 = a.v.z[row]; }
+            epi_load<EPI>(row, e0, e1, e2, e3);
             double acc = 0.0;
             while (j < e) {                                    // never entered when the slice is empty
                 double xv[U];
@@ -534,16 +535,9 @@ struct Mega {
                 carry += sh.red[0][0];
                 if (h.flag == 2) {
                     if (tid == 0) {
-                        const int row = h.row0;
-                        const double acc = carry;
-                        y[row] = acc;
-                        if (EPI == EPI_RH_Y) dot[0] = fma(a.v.rh[row], acc, dot[0]);
-                        if (EPI == EPI_QY_YY) { dot[0] = fma(a.v.r[row], acc, dot[0]); dot[1] = fma(acc, acc, dot[1]); }
-                        if (EPI == EPI_CA4) {
-                            const double rh = a.v.rh[row];
-                            dot[0] = fma(rh, a.v.r[row], dot[0]); dot[1] = fma(rh, acc, dot[1]);
-                            dot[2] = fma(rh, a.v.s[row], dot[2]); dot[3] = fma(rh, a.v.z[row], dot[3]);
-                        }
+                        double e0 = 0.0, e1 = 0.0, e2 = 0.0, e3 = 0.0;
+                        epi_load<EPI>(h.row0, e0, e1, e2, e3);
+                        row_done<EPI>(h.row0, carry, e0, e1, e2, e3, y, dot);
                     }
                     carry = 0.0;
                 }
@@ -558,39 +552,10 @@ struct Mega {
             if (valid) {
                 j = (int)(sptr[row - h.rowa] - h.a0) + sub;
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
-                if (sub == 0) {
-                    if (EPI == EPI_RH_Y) e0 = a.v.rh[row];
-                    if (EPI == EPI_QY_YY) e0 = a.v.r[row];
-                    if (EPI == EPI_CA4) { e0 = a.v.rh[row]; e1 = a.v.r[row]; e2 = a.v.s[row]; e3 = a.v.z[row]; }
-                }
+                if (sub == 0) epi_load<EPI>(row, e0, e1, e2, e3);
             }
-            double acc = 0.0;
-            while (j < e) {
-                unsigned c[UNR];
-                double v[UNR], xv[UNR];
-#pragma unroll
-                for (int u = 0; u < UNR; ++u) {
-                    const int idx = min(j + u * LANES, e - 1);
-                    c[u] = column((unsigned)idx);
-                    v[u] = sval[idx];
-                }
-#pragma unroll
-                for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
-#pragma unroll
-                for (int u = 0; u < UNR; ++u)
-                    if (j + u * LANES < e) acc = fma(v[u], xv[u], acc);
-                j += UNR * LANES;
-            }
-            acc = lanes_sum<LANES>(acc);
-            if (valid && sub == 0) {
-                y[row] = acc;
-                if (EPI == EPI_RH_Y) dot[0] = fma(e0, acc, dot[0]);
-                if (EPI == EPI_QY_YY) { dot[0] = fma(e0, acc, dot[0]); dot[1] = fma(acc, acc, dot[1]); }
-                if (EPI == EPI_CA4) {
-                    dot[0] = fma(e0, e1, dot[0]); dot[1] = fma(e0, acc, dot[1]);
-                    dot[2] = fma(e0, e2, dot[2]); dot[3] = fma(e0, e3, dot[3]);
-                }
-            }
+            const double acc = row_product<LANES, UNR>(sval, column, x, j, e);
+            if (valid && sub == 0) row_done<EPI>(row, acc, e0, e1, e2, e3, y, dot);
             __syncwarp();
             if (lane == 0) mbar_arrive(smem_u32(&sh.empty_bar[s]));
         }
@@ -618,16 +583,8 @@ struct Mega {
         double d0[1] = {0.0};
         arrive<0>(d0, true);
         if (!all) { wait_nbr(); return; }
+        wait_all();
         if (tid < RED_THREADS) {
-            if (tid < (int)gridDim.x && tid != (int)blockIdx.x) {
-                const unsigned long long *w = a.sync->slot[gen & (MEGA_RING - 1)][tid].w;
-                const unsigned long long t0 = globaltimer_ns();
-                unsigned spins = 0;
-                while ((unsigned)(ld_ll_gpu(w) >> 32) != gen) {
-                    poll_pause(++spins);
-                    if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { fail(); break; }
-                }
-            }
             nbar(2, RED_THREADS);
             if (tid < 32) fence_gpu();                 // acquire (+ L1 invalidate) after ALL pollers are through
         }
@@ -670,7 +627,7 @@ struct Mega {
             ld_ll_sys(w, w0, w1);
             if (ll_valid(w0, w1, epoch)) break;
             poll_pause(++spins);
-            if ((spins & 255u) == 0u && globaltimer_ns() - t0 > a.comm.timeout_ns) { fail(); break; }
+            if (timed_out(t0, spins)) { fail(); break; }
         }
         return ll_decode(w0, w1);
     }
@@ -934,8 +891,7 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
                 const int t = t0 + (int)(v % (unsigned)my_tiles);
                 const int row0 = a.tile_row[t], row1 = a.tile_row[t + 1];
                 const unsigned p0 = a.tile_nz[t], p1 = a.tile_nz[t + 1];
-                const unsigned a0 = p0 & ~al, cnt = ((p1 + al) & ~al) - a0;
-                const int rowa = row0 & ~3, cntp = ((row1 + 1 + 3) & ~3) - rowa;
+                const auto [a0, cnt, rowa, cntp] = tile_window(row0, row1, p0, p1, al);
                 unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
                 double   *sval = reinterpret_cast<double *>(st);
                 unsigned *scol = reinterpret_cast<unsigned *>(sval + cap);
@@ -1020,7 +976,7 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
         nbar(1, CT);
         if (a.comm.world > 1 && (m.reads_ghost || m.gs_hi > m.gs_lo)) {
             // the vectors the first phases read were pushed by the init kernels (kernel-per-phase protocol)
-            if (tid < 32 && !halo_wait(a.comm, sh.sc.halo_epoch) && tid == 0) { sh.sc.error = 1; sh.sc.done = 1; }
+            if (tid < 32 && !halo_wait_epoch(a.comm, sh.sc.halo_epoch) && tid == 0) { sh.sc.error = 1; sh.sc.done = 1; }
             if (tid < 32) fence_sys();
             nbar(1, CT);
         }

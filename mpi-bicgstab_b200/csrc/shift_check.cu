@@ -57,7 +57,7 @@ __global__ void __launch_bounds__(SC_THREADS) shift_res_kernel(const __grid_cons
     const int W = a.nj + 1;
     for (int t = tid; t < SC_WARPS * W; t += SC_THREADS) s_part[t] = 0.0;
     if (a.wait_halo && tid < 32) {
-        const bool ok = halo_wait(a.kc.comm, a.kc.sc->halo_epoch);
+        const bool ok = halo_wait_epoch(a.kc.comm, a.kc.sc->halo_epoch);
         if (!ok && tid == 0) a.kc.sc->error = 1;
     }
     __syncthreads();

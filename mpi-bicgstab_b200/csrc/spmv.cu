@@ -29,29 +29,10 @@ namespace bicg {
 
 namespace {
 
-template <int LANES>
-__device__ __forceinline__ double lanes_sum(double v)
-{
-#pragma unroll
-    for (int o = LANES / 2; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 __device__ __forceinline__ bool needs_tail(const KernelCommon &kc)
 {
     return kc.tail.op != TAIL_NONE || kc.tail.signal_halo;
 }
-
-__device__ __forceinline__ void mbar_arrive(unsigned bar)
-{
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads)
-{
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
-constexpr int PROW_PAD = 8;       // extra ptr / epilogue slots per stage for the 16-byte alignment window
 
 struct StageHdr { int row0, row1; unsigned a0; int rowa; };
 
@@ -94,9 +75,7 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
             for (int i = 0; i < my_tiles; ++i) {
                 const int t = (int)blockIdx.x + i * (int)gridDim.x, s = i % stages;
                 const int row0 = a.tile_row[t], row1 = a.tile_row[t + 1];
-                const unsigned p0 = a.tile_nz[t], p1 = a.tile_nz[t + 1];
-                const unsigned a0 = p0 & ~3u, cnt = ((p1 + 3u) & ~3u) - a0;          // 16-byte aligned windows
-                const int rowa = row0 & ~3, cntp = ((row1 + 1 + 3) & ~3) - rowa;
+                const auto [a0, cnt, rowa, cntp] = tile_window(row0, row1, a.tile_nz[t], a.tile_nz[t + 1], 3u);
                 if (i >= stages) mbar_wait(smem_u32(&empty_bar[s]), (unsigned)(i / stages - 1) & 1u);
                 unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
                 double   *sval = reinterpret_cast<double *>(st);
@@ -121,10 +100,10 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
         // the first gather (the reference's MPI_Wait on the allgather, matrix.c:439).
         if (a.wait_halo) {
             if (tid < 32) {
-                const bool ok = halo_wait(a.kc.comm, a.kc.sc->halo_epoch);
+                const bool ok = halo_wait_epoch(a.kc.comm, a.kc.sc->halo_epoch);
                 if (!ok && tid == 0) a.kc.sc->error = 1;
             }
-            named_bar_sync(1, CTHREADS);
+            nbar(1, CTHREADS);
         }
         const int lane = tid % LANES;
         const int row_in_tile = tid / LANES;
@@ -148,26 +127,7 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
                 j = (int)(sptr[row - h.rowa] - h.a0) + lane;
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
             }
-            double acc = 0.0;
-            while (j < e) {                                   // UNR gathers in flight, summed in order
-                unsigned c[UNR];
-                double v[UNR], xv[UNR];
-#pragma unroll
-                for (int u = 0; u < UNR; ++u) {
-                    // clamp instead of predicating: unconditional loads batch freely (a predicated load per
-                    // slot runs out of predicate registers after 7); the FMA below is what is predicated
-                    const int idx = min(j + u * LANES, e - 1);
-                    c[u] = scol[idx];
-                    v[u] = sval[idx];
-                }
-#pragma unroll
-                for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
-#pragma unroll
-                for (int u = 0; u < UNR; ++u)
-                    if (j + u * LANES < e) acc = fma(v[u], xv[u], acc);
-                j += UNR * LANES;
-            }
-            acc = lanes_sum<LANES>(acc);
+            double acc = row_product<LANES, UNR>(sval, [&](int idx) { return scol[idx]; }, x, j, e);
             if (valid && lane == 0) {
                 if (a.shift_sigma) acc = fma(*a.shift_sigma, ld_coherent(x + row), acc);     // s += sigma p (daxpy after the SpMV)
                 a.y[row] = acc;
@@ -199,7 +159,7 @@ __global__ void __launch_bounds__(256) spmv_rowsplit_kernel(const __grid_constan
     const int tid = threadIdx.x;
     if (a.wait_halo) {
         if (tid < 32) {
-            const bool ok = halo_wait(a.kc.comm, a.kc.sc->halo_epoch);
+            const bool ok = halo_wait_epoch(a.kc.comm, a.kc.sc->halo_epoch);
             if (!ok && tid == 0) a.kc.sc->error = 1;
         }
         __syncthreads();
