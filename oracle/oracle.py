@@ -192,12 +192,12 @@ def ref_solve(method, n, ptr, col, val, b, x0=None, tol=1e-15, max_iter=1000, kr
             "avg_time": L.orc_ref_avg_time(), "total_time": L.orc_ref_total_time()}
 
 
-def shifted_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_iter=1000):
-    """Restated shifted_lopbicg_switching (shifted_switching_solver.c:260-602).  Returns dict(ret, iters, x (sigma_len x n), r, hist,
-    seed, stop_iter)."""
+def shifted_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_iter=1000, x0=None):
+    """Restated shifted_lopbicg_switching (shifted_switching_solver.c:260-602) from the initial x_set x0 (None: zero).  Returns
+    dict(ret, iters, x (sigma_len x n), r, hist, seed, stop_iter)."""
     ptr, col, val = _csr(ptr, col, val)
     sigma = np.ascontiguousarray(sigma, dtype=np.float64)
-    x = np.zeros((sigma.size, n))
+    x = np.zeros((sigma.size, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(sigma.size, n)
     r = np.array(b, dtype=np.float64)
     hist = np.full(max_iter + 2, np.nan)
     seed_out = C.c_int(seed)
@@ -207,9 +207,10 @@ def shifted_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_iter=100
     return {"ret": ret, "iters": ret - 1, "x": x, "r": r, "hist": hist[:ret], "seed": seed_out.value, "stop_iter": np.array(stop_iter[:])}
 
 
-def ref_shifted_solve(n, ptr, col, val, b, sigma, seed, tol=1e-12, max_iter=1000, flavour="strict", variant="shifted_lopbicg_switching"):
+def ref_shifted_solve(n, ptr, col, val, b, sigma, seed, tol=1e-12, max_iter=1000, flavour="strict", variant="shifted_lopbicg_switching",
+                      x0=None):
     """The reference's own shifted_lopbicg_switching() (or its _noovlp twin, shifted_switching_solver.c:611) at P = 1, called
-    in-process on an in-memory CSR."""
+    in-process on an in-memory CSR, from the initial x_set x0 (None: zero)."""
     L = ref_lib(flavour)
     ptr, col, val = _csr(ptr, col, val)
     sigma = np.ascontiguousarray(sigma, dtype=np.float64)
@@ -224,7 +225,7 @@ def ref_shifted_solve(n, ptr, col, val, b, sigma, seed, tol=1e-12, max_iter=1000
     ds = (C.c_int * 1)(0)
     info.nz, info.rows, info.cols, info.code = int(ptr[-1]), n, n, b"MCRG"
     info.recvcounts, info.displs = C.cast(rc, C.POINTER(C.c_int)), C.cast(ds, C.POINTER(C.c_int))
-    x = np.zeros((sigma.size, n))
+    x = np.zeros((sigma.size, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(sigma.size, n)
     r = np.array(b, dtype=np.float64)
     L.orc_ref_config(tol, max_iter, 1, 1)
     L.orc_ref_hist_reset()

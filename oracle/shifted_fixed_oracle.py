@@ -30,13 +30,13 @@ def lib():
     return _lib
 
 
-def shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_iter=1000):
-    """Restated shifted_lopbicg (shifted_switching_solver.c:20-257).  Returns dict(ret, x (sigma_len x n), r, hist, stop_iter) with
-    ret = iterations performed, hist[k] = dot_r/dot_zero after iteration k and stop_iter[j] = the iteration after which shift j
-    stopped (0: never)."""
+def shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_iter=1000, x0=None):
+    """Restated shifted_lopbicg (shifted_switching_solver.c:20-257) from the initial x_set x0 (None: zero).  Returns dict(ret,
+    x (sigma_len x n), r, hist, stop_iter) with ret = iterations performed, hist[k] = dot_r/dot_zero after iteration k and
+    stop_iter[j] = the iteration after which shift j stopped (0: never)."""
     ptr, col, val = _csr(ptr, col, val)
     sigma = np.ascontiguousarray(sigma, dtype=np.float64)
-    x = np.zeros((sigma.size, n))
+    x = np.zeros((sigma.size, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(sigma.size, n)
     r = np.array(b, dtype=np.float64)
     hist = np.full(max_iter + 2, np.nan)
     stop_iter = (C.c_int * sigma.size)()
@@ -45,8 +45,8 @@ def shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, P=1, tol=1e-12, max_it
     return {"ret": ret, "x": x, "r": r, "hist": hist[:ret + 1], "stop_iter": np.array(stop_iter[:])}
 
 
-def ref_shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, tol=1e-12, max_iter=1000):
+def ref_shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, tol=1e-12, max_iter=1000, x0=None):
     """The reference's own shifted_lopbicg (P = 1) called in-process.  Returns dict(ret, x, r, res) with res = the
     sqrt(dot_r/dot_zero) it printed after every iteration."""
-    out = ref_shifted_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter, variant="shifted_lopbicg")
+    out = ref_shifted_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter, variant="shifted_lopbicg", x0=x0)
     return {k: out[k] for k in ("ret", "x", "r", "res")}

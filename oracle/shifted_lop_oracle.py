@@ -34,12 +34,13 @@ def lib():
     return _lib
 
 
-def shifted_lop_solve(n, ptr, col, val, b, sigma, seed, pipe=False, P=1, tol=1e-12, max_iter=1000):
-    """Restated shifted_lopbicgstab (shifted_solver.c:182-354) or, with pipe, shifted_pipe_lopbicgstab (:703-895).  Returns
+def shifted_lop_solve(n, ptr, col, val, b, sigma, seed, pipe=False, P=1, tol=1e-12, max_iter=1000, x0=None):
+    """Restated shifted_lopbicgstab (shifted_solver.c:182-354) or, with pipe, shifted_pipe_lopbicgstab (:703-895), from the
+    initial x_set x0 (None: zero).  Returns
     dict(ret, x (sigma_len x n), r, hist) with ret = iterations performed and hist[k] = dot_r/dot_zero."""
     ptr, col, val = _csr(ptr, col, val)
     sigma = np.ascontiguousarray(sigma, dtype=np.float64)
-    x = np.zeros((sigma.size, n))
+    x = np.zeros((sigma.size, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(sigma.size, n)
     r = np.array(b, dtype=np.float64)
     hist = np.full(max_iter + 2, np.nan)
     fn = lib().orc_shifted_pipe_lopbicgstab if pipe else lib().orc_shifted_lopbicgstab
@@ -67,8 +68,9 @@ def ref_lib():
     return _ref
 
 
-def ref_shifted_lop_solve(n, ptr, col, val, b, sigma, seed, variant, tol=1e-12, max_iter=1000):
-    """The reference's own shifted_solver.h function `variant` (P = 1) called in-process on an in-memory CSR.  Returns
+def ref_shifted_lop_solve(n, ptr, col, val, b, sigma, seed, variant, tol=1e-12, max_iter=1000, x0=None):
+    """The reference's own shifted_solver.h function `variant` (P = 1) called in-process on an in-memory CSR, from the initial
+    x_set x0 (None: zero).  Returns
     dict(ret, x (sigma_len x n), r, res) with res = the sqrt(dot_r/dot_zero) it printed after every iteration."""
     L = ref_lib()
     ptr, col, val = _csr(ptr, col, val)
@@ -84,7 +86,7 @@ def ref_shifted_lop_solve(n, ptr, col, val, b, sigma, seed, variant, tol=1e-12, 
     ds = (C.c_int * 1)(0)
     info.nz, info.rows, info.cols, info.code = int(ptr[-1]), n, n, b"MCRG"
     info.recvcounts, info.displs = C.cast(rc, C.POINTER(C.c_int)), C.cast(ds, C.POINTER(C.c_int))
-    x = np.zeros((sigma.size, n))
+    x = np.zeros((sigma.size, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(sigma.size, n)
     r = np.array(b, dtype=np.float64)
     L.orc_ref_config(tol, max_iter, 1, 1)
     L.orc_ref_hist_reset()

@@ -1,4 +1,6 @@
 """Shared test inputs: small members of the BASELINE.json matrix families (csrc/gen.cpp)."""
+import os
+
 import numpy as np
 
 # (name, kind, g, p0): sizes the oracle finishes in well under a second
@@ -29,6 +31,29 @@ def shifted_problem(O, n, ptr, col, val, L, scale, seed):
     b = O.spmv(n, ptr, col, val, np.ones(n))
     O.daxpy(sigma[seed], np.ones(n), b)
     return sigma, b
+
+
+# nonzero initial guesses: standard normal, or a warm start 1 + 1e-3 noise near the solution x* = 1 of b = A 1.  Either way
+# r0 = b - A x0 differs from b, so the init SpMV, r# = r0, dot_zero = (r0, r0) and the b of the replacements all show.
+X0_KINDS = ("normal", "warm")
+
+
+def initial_guess(kind, n, seed=0):
+    noise = np.random.default_rng(seed + 7919 * n).standard_normal(n)
+    return noise if kind == "normal" else 1.0 + 1e-3 * noise
+
+
+def initial_x_set(L, n, seed=0):
+    """A nonzero initial x_set of the shifted solvers, 0.1 standard normal: no larger than the corrections they add to it."""
+    return 0.1 * np.random.default_rng(seed + 7919 * n + L).standard_normal((L, n))
+
+
+# the problems of tests/golden/ref_x0.npz (generator tests/golden/make_golden_x0.py): the compiled reference from nonzero
+# initial guesses.  Plain solvers: (kind, g, p0, generator seed), tol, max_iter, krr / nrr of pipe_bicgstab_rr.  Shifted
+# solvers: (kind, g, p0, number of shifts, shift scale, seed index), tol, max_iter; the seed switches.
+X0_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_x0.npz")
+X0_PLAIN, X0_PLAIN_TOL, X0_PLAIN_MAX_ITER, X0_RR = ("convdiff", 25, 2.0, 99), 1e-11, 400, dict(krr=7, nrr=2)
+X0_SHIFTED, X0_SHIFTED_TOL, X0_SHIFTED_MAX_ITER = ("stencil15", 9, 14.0, 4, 2.0, 3), 1e-12, 1000
 
 
 def global_csr(B, kind, g, p0, seed=12345):
@@ -69,3 +94,13 @@ def big_csr(kind, g, p0, tmpdir="/dev/shm"):
             val = np.fromfile(fh, dtype=np.float64, count=nnz)
         _BIG[key] = (f, n, ptr, col, val)
     return _BIG[key]
+
+
+def x0_shifted_problem(B, O, gold_x0):
+    """The shifted problem of tests/golden/ref_x0.npz: (n, ptr, col, val, b, sigma, seed, x0), x0 as stored."""
+    kind, g, p0, L, scale, seed = X0_SHIFTED
+    _, n, ptr, col, val = global_csr(B, kind, g, p0)
+    sigma, b = shifted_problem(O, n, ptr, col, val, L, scale, seed)
+    x0 = gold_x0["shifted|x0"]
+    assert np.array_equal(x0, initial_x_set(L, n))
+    return n, ptr, col, val, b, sigma, seed, x0

@@ -28,8 +28,8 @@ def _ops(O, n, ptr, col, val, exact):
     return A, dot
 
 
-def _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol):
-    """Run from x0 = 0 until the loop test of solver.c:86 fails for tolerance `tol` and max_iter = max(ks).  Returns
+def _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol, x0=None):
+    """Run from x0 (None: zero) until the loop test of solver.c:86 fails for tolerance `tol` and max_iter = max(ks).  Returns
     ({k: state after iteration k, for the k in ks the loop reaches}, the state the loop ends in)."""
     b = np.ascontiguousarray(b, dtype=np.float64)
     n = b.size
@@ -41,7 +41,7 @@ def _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol):
     want = set(ks)
     max_iter = max(ks)
     out = {}
-    x = np.zeros(n)
+    x = np.zeros(n) if x0 is None else np.array(x0, dtype=np.float64)
     r = b.copy()
     if method == "pipe_bicgstab_rr" and krr <= 0:
         method = "pipe_bicgstab"                                  # the library's reading of krr <= 0 (solve.cu)
@@ -56,7 +56,7 @@ def _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol):
 
     # solver.c:74-79 / 200-203 / 333-336 / 475-479: r = b - A x0, r# = r, (r,r)
     if method == "pipe_bicgstab_rr":
-        bb = r.copy()                                             # :475
+        bb = b.copy()                                             # :475, the caller's b: not r0 unless x0 = 0
     Ax = A(x)
     ax(-1.0, Ax, r)
     rh = r.copy()
@@ -151,13 +151,14 @@ def _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol):
     return out, last.get("state")
 
 
-def reference_state(O, method, ptr, col, val, b, k, krr=0, nrr=0, exact=False, tol=0.0):
+def reference_state(O, method, ptr, col, val, b, k, krr=0, nrr=0, exact=False, tol=0.0, x0=None):
     """Every arena vector the reference leaves defined after iteration k (or after its last iteration, if the loop stops
-    earlier on `tol`), with the scalars the library keeps, "hist" (dot_r / dot_zero after iterations 0..k) and "iters"."""
-    return _run(O, method, ptr, col, val, b, [k], krr, nrr, exact, tol)[1]
+    earlier on `tol`), with the scalars the library keeps, "hist" (dot_r / dot_zero after iterations 0..k) and "iters".
+    x0 is the initial guess (None: zero); exact=True also evaluates its A x0 in long double."""
+    return _run(O, method, ptr, col, val, b, [k], krr, nrr, exact, tol, x0)[1]
 
 
-def reference_states(O, method, ptr, col, val, b, ks, krr=0, nrr=0, exact=False, tol=0.0):
+def reference_states(O, method, ptr, col, val, b, ks, krr=0, nrr=0, exact=False, tol=0.0, x0=None):
     """reference_state() for every k in `ks`, in one pass: {k: state}; a k the loop does not reach is absent.  A state
     holds the vectors under their arena names (ARENA) and the scalars under the names of SCALARS."""
-    return _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol)[0]
+    return _run(O, method, ptr, col, val, b, ks, krr, nrr, exact, tol, x0)[0]

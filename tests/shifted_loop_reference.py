@@ -54,12 +54,12 @@ class _Keeper:
         return self.out
 
 
-def _switching(O, n, ptr, col, val, b, sigma, seed, tol, max_iter_opt, exact, keep, fixed_ret=False):
+def _switching(O, n, ptr, col, val, b, sigma, seed, tol, max_iter_opt, exact, keep, x0):
     """orc_shifted_lopbicg_switching (shifted_switching_solver.c:260-602)."""
     A, dot = _ops(O, n, ptr, col, val, exact)
     ax, sc = O.daxpy, O.dscal
     L = sigma.size
-    x = np.zeros((L, n))
+    x = np.zeros((L, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(L, n)
     r = b.copy()
     k, max_iter, stop_count, max_sigma = 1, max_iter_opt + 1, 0, seed
     rTr = dot(r, r)
@@ -145,12 +145,12 @@ def _switching(O, n, ptr, col, val, b, sigma, seed, tol, max_iter_opt, exact, ke
     return k
 
 
-def _fixed(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep):
+def _fixed(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep, x0):
     """orc_shifted_lopbicg (shifted_switching_solver.c:20-257)."""
     A, dot = _ops(O, n, ptr, col, val, exact)
     ax, sc = O.daxpy, O.dscal
     L = sigma.size
-    x = np.zeros((L, n))
+    x = np.zeros((L, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(L, n)
     r = b.copy()
     k, stop_count = 0, 0
     sg = sigma[seed]
@@ -214,12 +214,12 @@ def _fixed(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep):
     return k
 
 
-def _lop(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep, pipe):
+def _lop(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep, x0, pipe):
     """orc_shifted_lop (shifted_solver.c:182-354 / :703-895)."""
     A, dot = _ops(O, n, ptr, col, val, exact)
     ax, sc = O.daxpy, O.dscal
     L = sigma.size
-    x = np.zeros((L, n))
+    x = np.zeros((L, n)) if x0 is None else np.array(x0, dtype=np.float64).reshape(L, n)
     r = b.copy()
     p = np.zeros((L, n))                                                 # p_loc_set = calloc (:226 / :748)
     s, y, z, w, v, t = (np.zeros(n) for _ in range(6))
@@ -326,7 +326,7 @@ def _lop(O, n, ptr, col, val, b, sigma, seed, tol, max_iter, exact, keep, pipe):
     return k
 
 
-def _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p):
+def _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p, x0=None):
     b = np.ascontiguousarray(b, dtype=np.float64)
     n = b.size
     ptr = np.ascontiguousarray(ptr, dtype=np.uint32)
@@ -334,7 +334,7 @@ def _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p):
     val = np.ascontiguousarray(val, dtype=np.float64)
     sigma = np.ascontiguousarray(sigma, dtype=np.float64)
     keep = _Keeper(ks, keep_p)
-    args = (O, n, ptr, col, val, b, sigma, int(seed), float(tol), max(ks), exact, keep)
+    args = (O, n, ptr, col, val, b, sigma, int(seed), float(tol), max(ks), exact, keep, x0)
     if method == "shifted_lopbicg_switching":
         ret = _switching(*args)
     elif method == "shifted_lopbicg":
@@ -346,7 +346,7 @@ def _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p):
     return keep.done(), keep.last, ret
 
 
-def shifted_reference_states(O, method, ptr, col, val, b, sigma, seed, ks, tol=0.0, exact=False, keep_p=True):
+def shifted_reference_states(O, method, ptr, col, val, b, sigma, seed, ks, tol=0.0, exact=False, keep_p=True, x0=None):
     """The state after iteration k of `method` for every k in ks, in one pass: {k: state}, the state of a solve with
     max_iter = k (the state the loop ends in, if its tolerance test ends it first).  A state holds
       iters, ret          iterations performed and the solver's return value (switching: iterations + 1)
@@ -354,11 +354,13 @@ def shifted_reference_states(O, method, ptr, col, val, b, sigma, seed, ks, tol=0
       r, hist             the seed residual and dot_r / dot_zero after iterations 0 .. iters
       seed, stop_iter     the seed after the last iteration, the iteration at which every shift stopped (0: never)
       shift               per-shift scalars of the last iteration (SCALARS)
-      decisions           every stop / switch decision so far: ("stop", k, j), ("switch", k, new seed), ("converged", k)"""
-    return _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p)[0]
+      decisions           every stop / switch decision so far: ("stop", k, j), ("switch", k, new seed), ("converged", k)
+    x0 (sigma_len, n) is the initial x_set (None: zero).  None of the four solvers forms b - A x0: r starts at b whatever x0 is,
+    and each x_j only ever has corrections added to it."""
+    return _run(O, method, ptr, col, val, b, sigma, seed, ks, tol, exact, keep_p, x0)[0]
 
 
-def shifted_reference_solve(O, method, ptr, col, val, b, sigma, seed, tol, max_iter, keep_p=False):
+def shifted_reference_solve(O, method, ptr, col, val, b, sigma, seed, tol, max_iter, keep_p=False, x0=None):
     """The whole solve: (the state it ends in, the solver's return value)."""
-    _, last, k = _run(O, method, ptr, col, val, b, sigma, seed, [max_iter], tol, False, keep_p)
+    _, last, k = _run(O, method, ptr, col, val, b, sigma, seed, [max_iter], tol, False, keep_p, x0)
     return last, (k if method == "shifted_lopbicg_switching" else last["ret"] if last else 0)

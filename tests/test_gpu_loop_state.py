@@ -24,7 +24,7 @@ import math
 import numpy as np
 import pytest
 
-from helpers import METHODS
+from helpers import METHODS, X0_KINDS, initial_guess
 from loop_reference import ARENA, SCALARS, reference_states
 from state_check import BIG, FACTOR, STANDALONE, _hold, _rel, cap_limit, matrix
 
@@ -54,21 +54,25 @@ def _sm_count():
 _REF = {}
 
 
-def reference(B, O, name, method, ks, krr=0, nrr=0):
-    """(reference states, exact-evaluation states) for ks, computed once per matrix, method and replacement schedule."""
-    key = (name, method, tuple(ks), krr, nrr)
+def reference(B, O, name, method, ks, krr=0, nrr=0, x0_kind=None):
+    """(reference states, exact-evaluation states) for ks, computed once per matrix, method, replacement schedule and initial
+    guess (x0_kind: a helpers.X0_KINDS entry, None for x0 = 0)."""
+    key = (name, method, tuple(ks), krr, nrr, x0_kind)
     if key in _REF:
         return _REF[key]
     n, ptr, col, val = matrix(B, name)
     b = O.spmv(n, ptr, col, val, np.ones(n))
-    ref = tuple(reference_states(O, method, ptr, col, val, b, ks, krr=krr, nrr=nrr, exact=e) for e in (False, True))
+    x0 = None if x0_kind is None else initial_guess(x0_kind, n)
+    ref = tuple(reference_states(O, method, ptr, col, val, b, ks, krr=krr, nrr=nrr, exact=e, x0=x0) for e in (False, True))
     if n < BIG:
         _REF[key] = ref
     return ref
 
 
 def check_state(B, dm, n, k, want, exact, x, r, label):
-    """Every vector, scalar and history entry the solve left against the reference state after iteration k."""
+    """Every vector, scalar and history entry the solve left against the reference state after iteration k.  b (the caller's
+    b, which pipe_bicgstab_rr keeps for its replacements) must be bit for bit what was passed in; every other vector, r# = r0
+    and ax = A x (A x0 until the first replacement) among them, is a computed one and held to its spread."""
     what = f"{label} k={k}"
     ratio = (0.0, "")
     got = np.empty(n)
@@ -76,8 +80,8 @@ def check_state(B, dm, n, k, want, exact, x, r, label):
         if not isinstance(ref, np.ndarray) or name == "hist":
             continue
         assert B.lib.bicg_debug_get_vec(dm.h, ARENA[name], got.ctypes.data_as(C.c_void_p)) == 0
-        if name in ("rh", "b"):
-            assert np.array_equal(got, ref), f"{what}: {name} must be r0 bit for bit"
+        if name == "b":
+            assert np.array_equal(got, ref), f"{what}: b must be the caller's b bit for bit"
             continue
         ratio = max(ratio, _hold(f"{what} {name}", got, ref, exact[name]))
         if name in ("x", "r"):
@@ -96,9 +100,9 @@ def check_state(B, dm, n, k, want, exact, x, r, label):
     return ratio
 
 
-def solve_k(B, dm, n, method, k, b, krr=0, nrr=0):
+def solve_k(B, dm, n, method, k, b, krr=0, nrr=0, x0=None):
     B.set_options(tol=0.0, max_iter=k)
-    x, r = np.zeros(n), b.copy()
+    x, r = np.zeros(n) if x0 is None else x0.copy(), b.copy()
     it, st = dm.solve(method, x, r, krr, nrr)
     assert it == st["iters"] == k, (it, k)
     return st, x, r
@@ -111,13 +115,15 @@ def assert_path(st, method, k, mega):
         assert st["kernel_launches"] >= MEGA_LAUNCHES[method] - 1 + k * KERNELS_PER_ITER[method], st["kernel_launches"]
 
 
-def run_states(B, O, name, method, ks=KS, mega=1, krr=0, nrr=0, codes=None, expect=None):
+def run_states(B, O, name, method, ks=KS, mega=1, krr=0, nrr=0, codes=None, expect=None, x0_kind=None):
     """Solve for every k in ks on a fresh handle of matrix `name`, hold each state to the reference; expect(dm, st) checks
-    the plan shape.  codes=False forces 32-bit columns.  Returns ((largest ratio, where), [(x, r, history) per k])."""
+    the plan shape.  codes=False forces 32-bit columns; x0_kind (helpers.X0_KINDS) starts from a nonzero initial guess.
+    Returns ((largest ratio, where), [(x, r, history) per k])."""
     n, ptr, col, val = matrix(B, name)
     if method == "pipe_bicgstab_rr" and not krr:
         krr, nrr = RR_KW["krr"], RR_KW["nrr"]
-    ref, ex = reference(B, O, name, method, ks, krr, nrr)
+    ref, ex = reference(B, O, name, method, ks, krr, nrr, x0_kind)
+    x0 = None if x0_kind is None else initial_guess(x0_kind, n)
     b = O.spmv(n, ptr, col, val, np.ones(n))
     B.set_options(mega=int(mega))
     dm = B.DeviceMatrix(B.blocks_from_csr(n, ptr, col, val))
@@ -126,7 +132,7 @@ def run_states(B, O, name, method, ks=KS, mega=1, krr=0, nrr=0, codes=None, expe
         if codes is not None:
             dm.stream_codes(codes)
         for k in ks:
-            st, x, r = solve_k(B, dm, n, method, k, b, krr, nrr)
+            st, x, r = solve_k(B, dm, n, method, k, b, krr, nrr, x0)
             assert_path(st, method, k, bool(mega))
             if expect:
                 expect(dm, st)
@@ -134,7 +140,8 @@ def run_states(B, O, name, method, ks=KS, mega=1, krr=0, nrr=0, codes=None, expe
             outs.append((x, r, B.last_history()))
     finally:
         dm.destroy()
-    print(f"[loop-state] {name} {method} mega={mega} codes={codes} krr={krr} nrr={nrr}: largest err/spread ratio {worst[0]:.3g} ({worst[1]})")
+    print(f"[loop-state] {name} {method} mega={mega} codes={codes} krr={krr} nrr={nrr} x0={x0_kind}: "
+          f"largest err/spread ratio {worst[0]:.3g} ({worst[1]})")
     return worst, outs
 
 
@@ -322,3 +329,60 @@ def test_spmv_epilogue_dots_every_variant(B, O, case):
                 assert abs(dots[i] - want) <= 1e-13 * scale, (epi, i, u, v, dots[i], want)
     finally:
         dm.destroy()
+
+
+# ---- nonzero initial guesses ------------------------------------------------------------------------------------------
+# From x0 != 0 the init SpMV computes a real A x0, r0 = b - A x0 differs from b, r# = r0 and dot_zero = (r0, r0) are computed
+# vectors and scalars, and the replacements of pipe_bicgstab_rr (k = 2 and 4) read the caller's b, which is no longer r0.
+# (matrix, options at plan time, plan-shape check of the persistent kernel)
+X0_MATRICES = [("small_n17", {}, None), ("small_n2113", {}, None), ("ragged_4001", {}, None), ("stencil15_g20", {}, None),
+               ("stencil15_g58", dict(resident=1), _all_resident), ("stencil15_g60", dict(resident=0), _all_coded),
+               (f"chunk_cap{cap_limit(512, 1)}", dict(mega_lanes=1), None)]
+
+
+# the warm start on n = 17 under pipe_bicgstab_rr: after the replacement at k = 4 the case's own spread is 9e-10 (t), at k = 5
+# 1.3e-8, so the states kept are k = 1, 2, 3 (the replacement at k = 2 among them)
+X0_KS = {("small_n17", "pipe_bicgstab_rr", "warm"): (1, 2, 3)}
+
+
+@pytest.mark.parametrize("x0_kind", X0_KINDS)
+@pytest.mark.parametrize("mega", [1, 0], ids=["mega", "multikernel"])
+@pytest.mark.parametrize("method", METHODS)
+@pytest.mark.parametrize("case", X0_MATRICES, ids=[c[0] for c in X0_MATRICES])
+def test_nonzero_x0_state(B, O, case, method, mega, x0_kind):
+    name, opts, expect = case
+    B.set_options(**opts)
+    ks = X0_KS.get((name, method, x0_kind), KS)
+    run_states(B, O, name, method, ks=ks, mega=mega, expect=expect if mega else None, x0_kind=x0_kind)
+
+
+@pytest.mark.parametrize("case", STANDALONE, ids=[c[0] for c in STANDALONE])
+def test_nonzero_x0_kernel_per_phase_state(B, O, case):
+    """Every forced stand-alone SpMV variant computes the init's A x0; one method per variant, in turn."""
+    _, name, opts, kind, lanes = case
+    B.set_options(**opts)
+    method = METHODS[STANDALONE.index(case) % len(METHODS)]
+    run_states(B, O, name, method, ks=(1, 2), mega=0, expect=_plan(kind, lanes), x0_kind="normal")
+
+
+@pytest.mark.parametrize("mega", [1, 0], ids=["mega", "multikernel"])
+@pytest.mark.parametrize("method", METHODS)
+def test_exact_initial_guess_does_no_iterations(B, O, method, mega):
+    """x0 = x* with b = A x* from the library's own SpMV (dm.spmv: the plan and kernel of the init SpMV), so r0 = b - A x0 is
+    exactly zero: 0 iterations, x returned bit for bit as given, r all zero, and a history of one entry, dot_r / dot_zero = 0 / 0,
+    NaN as in the reference.  The nonzero-x0 counterpart of test_gpu_parity.py::test_zero_rhs_does_no_iterations."""
+    n, ptr, col, val = matrix(B, "stencil15_g20")
+    B.set_options(mega=mega, tol=1e-10, max_iter=100)
+    dm = B.DeviceMatrix(B.blocks_from_csr(n, ptr, col, val))
+    try:
+        xs = initial_guess("normal", n)
+        b = dm.spmv(xs)
+        x, r = xs.copy(), b.copy()
+        it, st = dm.solve(method, x, r, **(RR_KW if method.endswith("rr") else {}))
+        hist = B.last_history()
+    finally:
+        dm.destroy()
+    assert it == st["iters"] == 0, it
+    assert x.tobytes() == xs.tobytes()
+    assert not np.any(r), np.abs(r).max()
+    assert hist.size == 1 and np.isnan(hist[0]), hist

@@ -12,7 +12,7 @@ import os
 import numpy as np
 import pytest
 
-from helpers import METHODS, RR, SMALL_CASES, big_csr, global_csr, rel_err
+from helpers import METHODS, RR, SMALL_CASES, big_csr, global_csr, initial_guess, rel_err
 
 pytestmark = pytest.mark.gpu
 
@@ -285,3 +285,148 @@ def test_random_block_parity(B, O, request):
     if "mega" in request.node.name:
         assert st["kernel_launches"] <= 8          # the loop ran as one persistent kernel
     dm.destroy()
+
+
+# ---- a handle used again ------------------------------------------------------------------------------------------------
+@pytest.fixture
+def _fixed_plan(B):
+    """autotune off, so that a fresh handle gets the plan of the one it is compared with."""
+    B.set_options(autotune=0)
+    yield
+    B.set_options(autotune=1, tol=1e-15, max_iter=1000)
+
+
+def _kw(method):
+    return RR if method.endswith("rr") else {}
+
+
+def _hold_to_oracle(O, n, ptr, col, val, b, method, x0, tol, max_iter, it, hist, x, what):
+    """C- and H-level rules of this file for a solve from x0: iterations, the first 10 history entries, the true residual."""
+    ref = O.solve(method, n, ptr, col, val, b, x0=x0, tol=tol, max_iter=max_iter, **_kw(method))
+    assert abs(it - ref["iters"]) <= max(2, int(0.02 * ref["iters"])), (what, it, ref["iters"])
+    m = min(10, it, ref["iters"])
+    got, want = np.sqrt(hist[1:m + 1]), np.sqrt(ref["hist"][1:m + 1])
+    assert np.all(np.abs(got - want) <= 1e-10 * want + H_FLOOR), (what, got, want, np.abs(got - want) / want)
+    true_res = np.linalg.norm(b - O.spmv(n, ptr, col, val, x, long_double=True)) / np.linalg.norm(b)
+    assert true_res <= (10 * TOL if "pipe" not in method else 1e3 * TOL), (what, true_res)
+    return ref
+
+
+@pytest.mark.parametrize("entry", ["handle", "entry_point"])
+@pytest.mark.parametrize("method", METHODS)
+def test_restart_from_the_returned_x(B, O, _fixed_plan, method, entry):
+    """Solve to 1e-2, then again from the x it returned with the original b and tol 1e-10, on the same handle (DeviceMatrix,
+    or the reference-facing entry points, which keep one handle per matrix): the second solve is the oracle's from that x.
+    A first solve to 1e-4 would leave r0 = b - A x1 four digits of cancellation: the oracle's first ten history entries
+    from such an x1 then lie up to 7e-9 from their long-double evaluation, the case's own spread, which the H-level rule
+    cannot hold; from 1e-2 that spread stays below 5e-11."""
+    blk, n, ptr, col, val = global_csr(B, "convdiff", 40, 1.5)
+    b = O.spmv(n, ptr, col, val, np.ones(n))
+    dm = B.DeviceMatrix(blk) if entry == "handle" else None
+    run = (lambda x, r: dm.solve(method, x, r, **_kw(method))[0]) if dm else (lambda x, r: B.solve(method, blk, x, r, **_kw(method)))
+    try:
+        x = np.zeros(n)
+        B.set_options(tol=1e-2, max_iter=1000)
+        run(x, b.copy())
+        x1 = x.copy()
+        B.set_options(tol=TOL)
+        it = run(x, b.copy())
+        hist = B.last_history()
+    finally:
+        if dm:
+            dm.destroy()
+    assert it > 0 and not np.array_equal(x1, 0)
+    _hold_to_oracle(O, n, ptr, col, val, b, method, x1, TOL, 1000, it, hist, x, (method, entry))
+
+
+def _solve_bits(B, dm, method, x0, b):
+    x, r = x0.copy(), b.copy()
+    it, _ = dm.solve(method, x, r, **_kw(method))
+    return it, x.tobytes(), r.tobytes(), B.last_history().tobytes()
+
+
+def test_methods_in_sequence_on_one_handle(B, O, _fixed_plan):
+    """pipe_bicgstab_rr, bicgstab, ca_bicgstab, pipe_bicgstab one after another on one handle, each from a nonzero x0: each
+    leaves the bits of the same solve on a fresh handle (nothing one loop leaves in the arena reaches the next)."""
+    blk, n, ptr, col, val = global_csr(B, "convdiff", 40, 1.5)
+    b = O.spmv(n, ptr, col, val, np.ones(n))
+    x0 = initial_guess("normal", n)
+    B.set_options(tol=TOL, max_iter=1000)
+    order = ["pipe_bicgstab_rr", "bicgstab", "ca_bicgstab", "pipe_bicgstab"]
+    dm = B.DeviceMatrix(blk)
+    try:
+        shared = [_solve_bits(B, dm, m, x0, b) for m in order]
+    finally:
+        dm.destroy()
+    for method, got in zip(order, shared):
+        dm = B.DeviceMatrix(blk)
+        try:
+            want = _solve_bits(B, dm, method, x0, b)
+        finally:
+            dm.destroy()
+        assert got == want, method
+
+
+def _circulant(n, rho):
+    """A = I + rho S, S the cyclic shift: its eigenvalues lie on a circle of radius rho around 1, so BiCGStab's residual falls
+    by about rho^2 per iteration, steadily.  At rho = 0.992 it needs about 1200 iterations for 1e-10, and the oracle and its
+    long-double evaluation stop a few iterations apart, inside the C-level rule (a 1-D Laplacian needing as many stops 300
+    iterations apart: its count says nothing about the kernels)."""
+    import scipy.sparse as sp
+    A = sp.csr_matrix(sp.identity(n) + rho * sp.diags([np.ones(n - 1), np.ones(1)], [1, -(n - 1)]))
+    A.sort_indices()
+    return A.indptr, A.indices, A.data
+
+
+_LONG = {}
+
+
+def test_max_iter_raised_past_the_handle_history(B, O, _fixed_plan, request):
+    """A handle keeps max(max_iter, 1000) + 2 history entries in its arena.  Raising max_iter past that on an existing handle
+    moves the history out of the arena and drops the captured graphs, whose kernels hold the old pointer: after a solve on
+    each loop path at max_iter = 1000 (the kernel-per-phase graph is captured then), a solve of more than 1000 iterations at
+    max_iter = 2000 gives the bits of a handle created at 2000, and the oracle's count and early history.  Lowering max_iter
+    again, a short solve (50 iterations) still gives a fresh handle's bits and the oracle's history."""
+    mega = request.node.callspec.params["_quiet"]
+    n = 20000
+    ptr, col, val = _circulant(n, 0.992)
+    # x* of seed 1: the oracle's first ten history entries lie 2e-12 from their long-double evaluation (seed 0: 1.4e-8, beyond
+    # the H-level rule), and the two stop 1 iteration apart at 1e-10
+    b = O.spmv(n, ptr, col, val, initial_guess("normal", n, seed=1))
+    method = "bicgstab"
+    if "ref" not in _LONG:
+        _LONG["ref"] = O.solve(method, n, ptr, col, val, b, tol=TOL, max_iter=2000)
+    assert 1000 < _LONG["ref"]["iters"] < 1900, _LONG["ref"]["iters"]
+    blk = B.blocks_from_csr(n, ptr, col, val)
+    zero = np.zeros(n)
+    B.set_options(max_iter=1000)
+    old = B.DeviceMatrix(blk)
+    try:
+        B.set_options(tol=0.0, max_iter=50)
+        for path in (1 - mega, mega):
+            B.set_options(mega=path)
+            _solve_bits(B, old, method, zero, b)
+        B.set_options(tol=TOL, max_iter=2000)
+        got = _solve_bits(B, old, method, zero, b)
+        fresh = B.DeviceMatrix(blk)
+        try:
+            want = _solve_bits(B, fresh, method, zero, b)
+        finally:
+            fresh.destroy()
+        assert got[0] > 1000 and got == want, (got[0], want[0])
+        x = np.frombuffer(got[1]); hist = np.frombuffer(got[3])
+        assert hist.size == got[0] + 1
+        _hold_to_oracle(O, n, ptr, col, val, b, method, None, TOL, 2000, got[0], hist, x, "max_iter 2000")
+        B.set_options(tol=0.0, max_iter=50)
+        got = _solve_bits(B, old, method, zero, b)
+    finally:
+        old.destroy()
+    fresh = B.DeviceMatrix(blk)
+    try:
+        want = _solve_bits(B, fresh, method, zero, b)
+    finally:
+        fresh.destroy()
+    assert got[0] == 50 and got == want
+    ref = O.solve(method, n, ptr, col, val, b, tol=0.0, max_iter=10)
+    hist, want = np.sqrt(np.frombuffer(got[3])[1:11]), np.sqrt(ref["hist"][1:11])
+    assert np.all(np.abs(hist - want) <= 1e-10 * want + H_FLOOR), np.abs(hist - want) / want

@@ -1,5 +1,5 @@
 """GPU: the shifted solvers on device-resident vectors (bicg_shifted_solve_dev, DeviceMatrix.shifted_solve with CUDA tensors) and
-DeviceMatrix.solve with CUDA tensors (bicg_solve, device_vectors = 1).
+DeviceMatrix.solve with CUDA tensors (bicg_solve, device_vectors = 1), from zero and from nonzero initial guesses.
 
 For each of the four shifted methods the same problem runs through the host path (numpy) and the device path (tensors updated in
 place), with BICG_SHIFT_ERROR=1 and rank 0's printout on.  These must be bitwise equal: x_set, r, the return value,
@@ -14,7 +14,7 @@ import re
 import numpy as np
 import pytest
 
-from helpers import SMALL_CASES, RR, global_csr
+from helpers import SMALL_CASES, RR, global_csr, initial_guess
 from shifted_fixed_cases import FIXED_CASES
 from shifted_lop_cases import SHIFTED_LOP_CASES, shifted_lop_problem
 
@@ -137,23 +137,27 @@ def test_misaligned_view(B, O, capfd, method, case):
 @pytest.mark.parametrize("method", PLAIN)
 @pytest.mark.parametrize("case", [SMALL_CASES[0], SMALL_CASES[3]], ids=lambda c: c[0])
 def test_plain_solve_tensors_match_numpy(B, O, method, case):
+    """From x0 = 0 and from a nonzero x0 (r0 = b - A x0 then differs from b): the tensor path is the numpy path, bit for bit."""
     import torch
     B.set_options(quiet=1, tol=1e-10, max_iter=1000)
     blk, n, ptr, col, val = global_csr(B, *case[1:4])
     b = O.spmv(n, ptr, col, val, np.ones(n))
     kw = RR if method == "pipe_bicgstab_rr" else {}
     dm = B.DeviceMatrix(blk)
-    x = np.zeros(n); r = b.copy()
-    it_h, st_h = dm.solve(method, x, r, **kw)
-    hist_h = B.last_history()
-    xt = torch.zeros(n, dtype=torch.float64, device="cuda"); rt = torch.from_numpy(b.copy()).cuda()
-    ptrs = (xt.data_ptr(), rt.data_ptr())
-    it_d, st_d = dm.solve(method, xt, rt, **kw)
-    hist_d = B.last_history()
-    dm.destroy()
-    assert (xt.data_ptr(), rt.data_ptr()) == ptrs
-    assert it_d == it_h and st_d["iters"] == st_h["iters"] and st_d["converged"] == st_h["converged"]
-    assert _bits(st_d["final_res"]) == _bits(st_h["final_res"])
-    assert _bits(xt.cpu().numpy()) == _bits(x) and _bits(rt.cpu().numpy()) == _bits(r) and _bits(hist_d) == _bits(hist_h)
-    assert st_d["h2d_bytes"] == 0 and st_d["d2h_bytes"] == 0
-    assert np.abs(x - 1.0).max() < 1e-6
+    try:
+        for x0 in (np.zeros(n), initial_guess("normal", n)):
+            x = x0.copy(); r = b.copy()
+            it_h, st_h = dm.solve(method, x, r, **kw)
+            hist_h = B.last_history()
+            xt = torch.from_numpy(x0.copy()).cuda(); rt = torch.from_numpy(b.copy()).cuda()
+            ptrs = (xt.data_ptr(), rt.data_ptr())
+            it_d, st_d = dm.solve(method, xt, rt, **kw)
+            hist_d = B.last_history()
+            assert (xt.data_ptr(), rt.data_ptr()) == ptrs
+            assert it_d == it_h and st_d["iters"] == st_h["iters"] and st_d["converged"] == st_h["converged"]
+            assert _bits(st_d["final_res"]) == _bits(st_h["final_res"])
+            assert _bits(xt.cpu().numpy()) == _bits(x) and _bits(rt.cpu().numpy()) == _bits(r) and _bits(hist_d) == _bits(hist_h)
+            assert st_d["h2d_bytes"] == 0 and st_d["d2h_bytes"] == 0
+            assert np.abs(x - 1.0).max() < 1e-6
+    finally:
+        dm.destroy()

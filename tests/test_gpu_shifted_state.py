@@ -20,7 +20,7 @@ epilogue under the 0-, 1- and 2-dot epilogues) and a 216 k-row matrix with 64 sh
 import numpy as np
 import pytest
 
-from helpers import global_csr, shifted_problem
+from helpers import global_csr, initial_x_set, shifted_problem
 from shifted_fixed_cases import FIXED_CASES
 from shifted_loop_reference import METHODS, shifted_reference_states
 from state_check import MATRICES, STANDALONE, _hold, _rel, matrix
@@ -63,13 +63,15 @@ def _problem(O, n, ptr, col, val, L, scale, seed):
 _REF = {}
 
 
-def reference(B, O, spec, method, L, scale, seed, tol, ks, keep_p=True):
-    """(restatement states, exact-evaluation states) for ks, once per matrix, method, tolerance, shift set and seed."""
-    key = (str(spec), method, L, scale, seed, tol, tuple(ks))
+def reference(B, O, spec, method, L, scale, seed, tol, ks, keep_p=True, x0=False):
+    """(restatement states, exact-evaluation states) for ks, once per matrix, method, tolerance, shift set, seed and initial
+    x_set (x0: helpers.initial_x_set instead of zero)."""
+    key = (str(spec), method, L, scale, seed, tol, tuple(ks), x0)
     if key not in _REF:
         n, ptr, col, val = _matrix(B, spec)
         sigma, b = _problem(O, n, ptr, col, val, L, scale, seed)
-        _REF[key] = tuple(shifted_reference_states(O, method, ptr, col, val, b, sigma, seed, ks, tol=tol, exact=e, keep_p=keep_p)
+        xs = initial_x_set(L, n) if x0 else None
+        _REF[key] = tuple(shifted_reference_states(O, method, ptr, col, val, b, sigma, seed, ks, tol=tol, exact=e, keep_p=keep_p, x0=xs)
                           for e in (False, True))
         if n * L > 1 << 22:                        # the 216 k-row case: its states are not kept
             return _REF.pop(key)
@@ -115,11 +117,12 @@ def check_state(method, k, got, want, exact, what):
 
 
 def solve_k(B, dm, method, k, sigma, seed, b, tol, x0=None):
-    """One solve with shift_max_iter = k on host vectors (x0: a CUDA tensor x_set to solve in place instead)."""
+    """One solve with shift_max_iter = k on host vectors from x0 (a numpy (L, n) initial x_set; None: zero), or in place on x0
+    if it is a CUDA tensor."""
     L, n = sigma.size, b.size
     B.set_options(shift_tol=tol, shift_max_iter=k)
-    if x0 is None:
-        x, r = np.zeros((L, n)), b.copy()
+    if x0 is None or isinstance(x0, np.ndarray):
+        x, r = np.zeros((L, n)) if x0 is None else x0.copy(), b.copy()
         ret, st = dm.shifted_solve(method, x, r, sigma, seed)
     else:
         import torch
@@ -129,6 +132,17 @@ def solve_k(B, dm, method, k, sigma, seed, b, tol, x0=None):
     seed_out, stop = B.last_shift_info(L)
     assert st["iters"] == B.last_history().size - 1, (st["iters"], B.last_history().size)
     return dict(ret=ret, iters=st["iters"], x=x, r=r, hist=B.last_history(), seed=seed_out, stop=stop)
+
+
+def _device_x_set(x0, offset):
+    """x0 (L, n) as a CUDA tensor: contiguous, or a view one element into a larger tensor (every row misaligned for even n)."""
+    import torch
+    t = torch.from_numpy(x0).cuda()
+    if not offset:
+        return t
+    big = torch.zeros(x0.size + 1, dtype=torch.float64, device="cuda")
+    big[1:].view(x0.shape).copy_(t)
+    return big[1:].view(x0.shape)
 
 
 def check_stopped_shifts(method, outs, what):
@@ -145,18 +159,22 @@ def check_stopped_shifts(method, outs, what):
             assert outs[k]["x"][j].tobytes() == outs[after[0]]["x"][j].tobytes(), (what, "stopped shift moved", j, s, after[0], k)
 
 
-def run_states(B, O, spec, method, L, scale, seed, tol=1e-12, ks=KS, label=None, keep_p=True):
-    """Solve for every k in ks on one handle, hold each state to the restatement.  Returns {k: the solve's results}."""
+def run_states(B, O, spec, method, L, scale, seed, tol=1e-12, ks=KS, label=None, keep_p=True, x0=False, device=None):
+    """Solve for every k in ks on one handle, hold each state to the restatement.  x0: start from helpers.initial_x_set instead
+    of zero; device: solve in place on a CUDA tensor, "aligned" or at a one-element "offset".  Returns {k: the solve's results}."""
     label = label or f"{spec} {method} L={L} seed={seed} tol={tol:g}"
+    label += (" x0" if x0 else "") + (f" device-{device}" if device else "")
     n, ptr, col, val = _matrix(B, spec)
     sigma, b = _problem(O, n, ptr, col, val, L, scale, seed)
-    ref, ex = reference(B, O, spec, method, L, scale, seed, tol, ks, keep_p)
+    ref, ex = reference(B, O, spec, method, L, scale, seed, tol, ks, keep_p, x0)
+    xs = initial_x_set(L, n) if x0 else np.zeros((L, n))
     check_decisions(ref, ex, ks, label)
     dm = B.DeviceMatrix(B.blocks_from_csr(n, ptr, col, val))
     worst, outs = (0.0, ""), {}
     try:
         for k in ks:
-            outs[k] = solve_k(B, dm, method, k, sigma, seed, b, tol)
+            start = xs if device is None else _device_x_set(xs, device == "offset")
+            outs[k] = solve_k(B, dm, method, k, sigma, seed, b, tol, start)
             worst = max(worst, check_state(method, k, outs[k], ref[k], ex[k], label))
     finally:
         dm.destroy()
@@ -303,3 +321,36 @@ def test_many_shifts_match_512(B, O, method):
         assert res.max() <= 1e-10, (method, int(res.argmax()), res.max())
     finally:
         dm.destroy()
+
+
+# ---- nonzero initial x_set ------------------------------------------------------------------------------------------------
+# None of the four solvers forms b - A x0: they add corrections to each x_j, so x_j = x0_j + correction.  x0 = 0.1 standard
+# normal keeps |x0| no larger than the corrections, which set max|x_j| in the max-norm rule: a large x0 would hide their error.
+X0_CASES = [c for c in CASES if c[0] in ("sh_convdiff_g40_L6_switch", "fx_stencil15_g12_L5_seed2")] + [
+    ("small_n17", "small_n17", 5, 0.05, 2, 1e-12)]
+
+
+@pytest.mark.parametrize("method", METHODS)
+@pytest.mark.parametrize("case", X0_CASES, ids=[c[0] for c in X0_CASES])
+def test_nonzero_x0_state(B, O, case, method):
+    _, spec, L, scale, seed, tol = case
+    run_states(B, O, spec, method, L, scale, seed, tol, _ks(B, O, case, method), label=f"{case[0]} {method}", x0=True)
+
+
+X0_EDGES = [(m, L) for m, L in EDGES if L in (945, 946, 970, 971)]
+
+
+@pytest.mark.parametrize("method,L", X0_EDGES, ids=[f"{m}-L{L}" for m, L in X0_EDGES])
+def test_nonzero_x0_table_edges_state(B, O, method, L):
+    """The update kernels' coefficient tables in one pass and in two, adding to a nonzero x_j on either side of the seed."""
+    run_states(B, O, "small_n17", method, L, 0.5 / L, L // 2, ks=tuple(k for k in KS if k <= kmax("table_edges", method)), x0=True)
+
+
+@pytest.mark.parametrize("device", ["aligned", "offset"])
+@pytest.mark.parametrize("method", METHODS)
+def test_nonzero_x0_device_path_state(B, O, method, device):
+    """bicg_shifted_solve_dev in place on the caller's nonzero x_set, through the seed switch: held to the restatement itself,
+    not only to the host path."""
+    case = next(c for c in X0_CASES if c[0] == "sh_convdiff_g40_L6_switch")
+    _, spec, L, scale, seed, tol = case
+    run_states(B, O, spec, method, L, scale, seed, tol, _ks(B, O, case, method), label=f"{case[0]} {method}", x0=True, device=device)

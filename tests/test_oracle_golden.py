@@ -1,12 +1,14 @@
 """CPU: the oracle restatement (oracle/bicg_oracle.c) against the golden vectors the REFERENCE produced
 (tests/golden/ref_histories_P*.npz, generator tests/golden/make_golden.py) -- bit for bit, for 1, 2 and 3 ranks --
-and against further outputs of the compiled reference (tests/golden/ref_live.npz, tests/golden/make_golden_live.py)."""
+and against further outputs of the compiled reference (tests/golden/ref_live.npz, tests/golden/make_golden_live.py; from
+nonzero initial guesses tests/golden/ref_x0.npz, tests/golden/make_golden_x0.py)."""
 import os
 
 import numpy as np
 import pytest
 
-from helpers import METHODS, RR, SMALL_CASES, global_csr
+from helpers import (METHODS, RR, SMALL_CASES, X0_GOLDEN, X0_KINDS, X0_PLAIN, X0_PLAIN_MAX_ITER, X0_PLAIN_TOL, X0_RR, global_csr,
+                     initial_guess)
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 TOL, MAX_ITER = 1e-10, 600
@@ -52,6 +54,29 @@ def test_oracle_against_compiled_reference_live(B, O, gold_live):
         assert np.array_equal(o["x"], r["x"]) and np.array_equal(o["r"], r["r"])
 
 
+@pytest.fixture(scope="module")
+def gold_x0():
+    return np.load(X0_GOLDEN)
+
+
+@pytest.mark.parametrize("x0_kind", X0_KINDS)
+def test_oracle_from_nonzero_x0_against_compiled_reference(B, O, gold_x0, x0_kind):
+    """From x0 != 0 (solver.c:74-83: r0 = b - A x0, r# = r0, dot_zero = (r0, r0); pipe_bicgstab_rr keeps the caller's b for its
+    replacements, :475 / :524) the oracle gives the reference's iteration count, every printed residual, x and r bit for bit."""
+    kind, g, p0, gseed = X0_PLAIN
+    _, n, ptr, col, val = global_csr(B, kind, g, p0, seed=gseed)
+    b = O.spmv(n, ptr, col, val, np.ones(n))
+    x0 = gold_x0[f"plain|{x0_kind}|x0"]
+    assert np.array_equal(x0, initial_guess(x0_kind, n))
+    for method in METHODS:
+        kw = X0_RR if method == "pipe_bicgstab_rr" else {}
+        o = O.solve(method, n, ptr, col, val, b, x0=x0, tol=X0_PLAIN_TOL, max_iter=X0_PLAIN_MAX_ITER, **kw)
+        r = {k: gold_x0[f"plain|{x0_kind}|{method}|{k}"] for k in ("iters", "res", "x", "r")}
+        assert 0 < o["iters"] == r["iters"] < X0_PLAIN_MAX_ITER, (method, o["iters"], r["iters"])
+        assert np.array_equal(np.sqrt(o["hist"][1:]), r["res"]), method
+        assert np.array_equal(o["x"], r["x"]) and np.array_equal(o["r"], r["r"]), method
+
+
 def test_oracle_rhs_ones_multi_rank_live(B, O, gold_live):
     """README / BASELINE wording "right-hand side = all ones" (main.c itself uses b = A*1): the oracle follows the
     compiled reference for that rhs too, with 1 and 3 ranks."""
@@ -88,7 +113,7 @@ def test_manufactured_solution(B, O):
 
 
 # ---- shifted family (SURVEY.md 8(f) N4) --------------------------------------------------------------------------
-from helpers import SHIFTED_CASES, shifted_problem
+from helpers import SHIFTED_CASES, X0_SHIFTED_MAX_ITER, X0_SHIFTED_TOL, shifted_problem, x0_shifted_problem
 
 
 @pytest.fixture(scope="module")
@@ -129,3 +154,14 @@ def test_reference_noovlp_twin_is_the_same_solve(B, O, gold_shifted, gold_live, 
     assert np.array_equal(np.sqrt(o["hist"][1:]), c["res"])
     assert a["ret"] == c["ret"] and np.array_equal(a["x"], c["x"]) and np.array_equal(a["r"], c["r"])
     assert np.array_equal(a["res"], c["res"])
+
+
+def test_shifted_oracle_from_nonzero_x0_against_compiled_reference(B, O, gold_x0):
+    """orc_shifted_lopbicg_switching from a nonzero x_set, through a seed switch: the reference's return value, every x_j, r and
+    printed residual, bit for bit.  The solver only adds to each x_j, so x0 reaches the result."""
+    n, ptr, col, val, b, sigma, seed, x0 = x0_shifted_problem(B, O, gold_x0)
+    o = O.shifted_solve(n, ptr, col, val, b, sigma, seed, tol=X0_SHIFTED_TOL, max_iter=X0_SHIFTED_MAX_ITER, x0=x0)
+    want = {k: gold_x0[f"shifted|shifted_lopbicg_switching|{k}"] for k in ("ret", "res", "x", "r")}
+    assert o["ret"] == want["ret"] and o["seed"] != seed
+    assert np.array_equal(o["x"], want["x"]) and np.array_equal(o["r"], want["r"])
+    assert np.array_equal(np.sqrt(o["hist"][1:]), want["res"])

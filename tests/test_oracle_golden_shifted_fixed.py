@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 import shifted_fixed_oracle as OF
 
-from helpers import global_csr
+from helpers import X0_GOLDEN, X0_SHIFTED_MAX_ITER, X0_SHIFTED_TOL, global_csr, x0_shifted_problem
 from shifted_fixed_cases import FIXED_CASES, FIXED_LARGE_CASES, GOLDEN_FIXED, fixed_problem
 
 
@@ -73,3 +73,14 @@ def test_fixed_solves_every_shifted_system(B, O, case):
     for j in range(sigma.size):
         res = O.spmv(n, ptr, col, val, x[j]) + sigma[j] * x[j] - b
         assert np.linalg.norm(res) <= 10 * tol * np.linalg.norm(b), (j, np.linalg.norm(res) / np.linalg.norm(b))
+
+
+def test_oracle_from_nonzero_x0_matches_reference_bitwise(B, O):
+    """From a nonzero x_set (tests/golden/ref_x0.npz): the reference's return value, every x_j, r and printed residual."""
+    gold = np.load(X0_GOLDEN)
+    n, ptr, col, val, b, sigma, seed, x0 = x0_shifted_problem(B, O, gold)
+    got = OF.shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, tol=X0_SHIFTED_TOL, max_iter=X0_SHIFTED_MAX_ITER, x0=x0)
+    want = {k: gold[f"shifted|shifted_lopbicg|{k}"] for k in ("ret", "res", "x", "r")}
+    assert got["ret"] == want["ret"]
+    assert np.array_equal(got["x"], want["x"]) and np.array_equal(got["r"], want["r"])
+    assert np.array_equal(np.sqrt(got["hist"][1:]), want["res"])

@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 import shifted_lop_oracle as OL
 
-from helpers import global_csr
+from helpers import X0_GOLDEN, X0_SHIFTED_MAX_ITER, X0_SHIFTED_TOL, global_csr, x0_shifted_problem
 from shifted_lop_cases import SHIFTED_LOP_CASES, SHIFTED_LOP_VARIANTS, golden_path, shifted_lop_problem
 
 LOP = ["shifted_lopbicgstab", "shifted_lopbicgstab_v2", "shifted_lopbicgstab_nooverlap"]
@@ -51,6 +51,18 @@ def test_lop_solves_every_shifted_system(B, O, case):
     for j in range(sigma.size):
         res = O.spmv(n, ptr, col, val, x[j]) + sigma[j] * x[j] - b
         assert np.linalg.norm(res) <= 1e-10 * np.linalg.norm(b), (j, np.linalg.norm(res) / np.linalg.norm(b))
+
+
+@pytest.mark.parametrize("pipe", [False, True], ids=["lop", "pipe_lop"])
+def test_oracle_from_nonzero_x0_matches_reference_bitwise(B, O, pipe):
+    """From a nonzero x_set (tests/golden/ref_x0.npz): the reference's return value, every x_j, r and printed residual."""
+    gold = np.load(X0_GOLDEN)
+    n, ptr, col, val, b, sigma, seed, x0 = x0_shifted_problem(B, O, gold)
+    got = OL.shifted_lop_solve(n, ptr, col, val, b, sigma, seed, pipe=pipe, tol=X0_SHIFTED_TOL, max_iter=X0_SHIFTED_MAX_ITER, x0=x0)
+    want = {k: gold[f"shifted|{PIPE[0] if pipe else LOP[0]}|{k}"] for k in ("ret", "res", "x", "r")}
+    assert got["ret"] == want["ret"]
+    assert np.array_equal(got["x"], want["x"]) and np.array_equal(got["r"], want["r"])
+    assert np.array_equal(np.sqrt(got["hist"][1:]), want["res"])
 
 
 def test_golden_covers_every_reference_function():

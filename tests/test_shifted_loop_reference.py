@@ -7,7 +7,7 @@ import pytest
 import shifted_fixed_oracle as OF
 import shifted_lop_oracle as OL
 
-from helpers import global_csr
+from helpers import global_csr, initial_x_set
 from shifted_fixed_cases import FIXED_CASES, FIXED_LARGE_CASES, fixed_problem
 from shifted_loop_reference import METHODS, shifted_reference_solve, shifted_reference_states
 
@@ -19,16 +19,17 @@ def _bits(a):
     return np.ascontiguousarray(np.asarray(a, dtype=np.float64)).tobytes()
 
 
-def oracle_solve(O, method, n, ptr, col, val, b, sigma, seed, tol, max_iter):
-    """The C oracle of `method` at P = 1: dict(ret, x, r, hist, seed, stop_iter); seed / stop_iter are None where the oracle
-    does not report them (the LOP family neither switches nor stops single shifts)."""
+def oracle_solve(O, method, n, ptr, col, val, b, sigma, seed, tol, max_iter, x0=None):
+    """The C oracle of `method` at P = 1 from the initial x_set x0 (None: zero): dict(ret, x, r, hist, seed, stop_iter); seed /
+    stop_iter are None where the oracle does not report them (the LOP family neither switches nor stops single shifts)."""
     if method == "shifted_lopbicg_switching":
-        out = O.shifted_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter)
+        out = O.shifted_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter, x0=x0)
         return dict(ret=out["ret"], x=out["x"], r=out["r"], hist=out["hist"], seed=out["seed"], stop_iter=out["stop_iter"])
     if method == "shifted_lopbicg":
-        out = OF.shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter)
+        out = OF.shifted_fixed_solve(n, ptr, col, val, b, sigma, seed, tol=tol, max_iter=max_iter, x0=x0)
         return dict(ret=out["ret"], x=out["x"], r=out["r"], hist=out["hist"], seed=seed, stop_iter=out["stop_iter"])
-    out = OL.shifted_lop_solve(n, ptr, col, val, b, sigma, seed, pipe=method == "shifted_pipe_lopbicgstab", tol=tol, max_iter=max_iter)
+    out = OL.shifted_lop_solve(n, ptr, col, val, b, sigma, seed, pipe=method == "shifted_pipe_lopbicgstab", tol=tol, max_iter=max_iter,
+                               x0=x0)
     return dict(ret=out["ret"], x=out["x"], r=out["r"], hist=out["hist"], seed=None, stop_iter=None)
 
 
@@ -53,6 +54,27 @@ def test_restatement_bitwise_equal_to_oracle(B, O, case, method):
     assert_same_as_oracle(got, ret, want, (case[0], method))
     if method == "shifted_lopbicg_switching" and case[0].endswith("_switch"):
         assert any(d[0] == "switch" for d in got["decisions"]), got["decisions"]      # the seed does switch here
+
+
+X0_CASES = [c for c in FIXED_CASES if c[0] in ("sh_stencil15_g12_L5", "sh_convdiff_g40_L6_switch", "fx_stencil15_g12_L5_seed2")]
+
+
+@pytest.mark.parametrize("method", METHODS)
+@pytest.mark.parametrize("case", X0_CASES, ids=[c[0] for c in X0_CASES])
+def test_restatement_from_nonzero_x0_bitwise_equal_to_oracle(B, O, case, method):
+    """The shifted solvers never form b - A x0: they only add to each x_j, so a nonzero initial x_set carries through to the
+    result, and the restatement must still give the oracles' bits, through the seed switch of the _switch case too."""
+    _, n, ptr, col, val = global_csr(B, *case[1:4])
+    sigma, b, seed, tol = fixed_problem(O, n, ptr, col, val, case)
+    x0 = initial_x_set(sigma.size, n)
+    want = oracle_solve(O, method, n, ptr, col, val, b, sigma, seed, tol, MAX_ITER, x0=x0)
+    got, ret = shifted_reference_solve(O, method, ptr, col, val, b, sigma, seed, tol, MAX_ITER, x0=x0)
+    assert_same_as_oracle(got, ret, want, (case[0], method, "x0"))
+    zero = oracle_solve(O, method, n, ptr, col, val, b, sigma, seed, tol, MAX_ITER)
+    assert want["ret"] == zero["ret"] and _bits(want["hist"]) == _bits(zero["hist"])     # x0 changes nothing but x
+    assert not np.array_equal(want["x"], zero["x"])
+    if method == "shifted_lopbicg_switching" and case[0].endswith("_switch"):
+        assert any(d[0] == "switch" for d in got["decisions"]), got["decisions"]
 
 
 def _switch_iteration(O, B, case, tol):
