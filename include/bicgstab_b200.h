@@ -245,7 +245,12 @@ int bicg_profile_solve(bicg_matrix *m, int method, int iters, double class_ms[3]
  *   bicg_debug_coded_ctas: how many CTAs of the last persistent-kernel launch on this handle streamed 16-bit column codes
  *                         instead of 32-bit columns (csrc/mega.cu).
  *   bicg_debug_stream_codes: on = 0 makes every streaming CTA of later launches on this handle stream 32-bit columns,
- *                         on = 1 restores the default; returns the previous setting.  Both formats give bit-identical results. */
+ *                         on = 1 restores the default; returns the previous setting.  Both formats give bit-identical results.
+ *   bicg_debug_packed_ctas: how many CTAs of the last persistent-kernel launch on this handle streamed 7-byte packed values
+ *                         (a per-CTA sign / exponent table index + the 52 mantissa bits) instead of 8-byte values (csrc/mega.cu).
+ *   bicg_debug_stream_values: on = 0 makes every streaming CTA of later launches on this handle stream 8-byte values (the
+ *                         column codes stay), on = 1 restores the default; returns the previous setting.  Both formats give
+ *                         bit-identical results. */
 int bicg_debug_vec_phase(bicg_matrix *m, int phase, const double coef[3], double *vecs, double dots[8]);
 int bicg_debug_spmv_epi(bicg_matrix *m, int epi, double *vecs, double dots[8]);
 int bicg_debug_get_vec(bicg_matrix *m, int id, double *out);
@@ -253,6 +258,8 @@ int bicg_debug_get_scalars(bicg_matrix *m, double out[13]);
 int bicg_debug_resident_ctas(bicg_matrix *m);
 int bicg_debug_coded_ctas(bicg_matrix *m);
 int bicg_debug_stream_codes(bicg_matrix *m, int on);
+int bicg_debug_packed_ctas(bicg_matrix *m);
+int bicg_debug_stream_values(bicg_matrix *m, int on);
 
 /* full-precision history of the last solve on this rank: out[k] = dot_r/dot_zero after iteration k
  * (out[0] = 1).  Returns the number of entries available (iters + 1). */

@@ -416,6 +416,15 @@ class DeviceMatrix:
         (the results are bit-identical); returns the previous setting."""
         return bool(lib.bicg_debug_stream_codes(self.h, 1 if on else 0))
 
+    def packed_ctas(self):
+        """CTAs of the last persistent-kernel launch that streamed 7-byte packed values instead of 8-byte values."""
+        return int(lib.bicg_debug_packed_ctas(self.h))
+
+    def stream_values(self, on):
+        """Test hook: on=False makes later persistent-kernel launches on this handle stream 8-byte values everywhere while
+        keeping the column codes (the results are bit-identical); returns the previous setting."""
+        return bool(lib.bicg_debug_stream_values(self.h, 1 if on else 0))
+
     def spmv_time(self, reps=20):
         ms, by = C.c_double(), C.c_double()
         lib.bicg_spmv_time(self.h, reps, C.byref(ms), C.byref(by))

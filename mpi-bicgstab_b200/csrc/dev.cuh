@@ -252,27 +252,29 @@ __device__ __forceinline__ TileWindow tile_window(int row0, int row1, unsigned p
 
 // One row's product with x over the staged entries [j, e) (j already includes the thread's offset in its group of
 // LANES), summed over the group.  This loop decides the bits of y: entries in storage order, one fma each, then
-// lanes_sum.  UNR gathers are in flight per thread; `column(idx)` returns the column of staged entry idx.
-template <int LANES, int UNR, class Column>
-__device__ __forceinline__ double row_product(const double *sval, Column column, const double *x, int j, int e)
+// lanes_sum.  UNR gathers are in flight per thread; `column(idx)` and `value(idx)` return the column and the value of
+// staged entry idx (a value may come as an object that converts to double: it is converted where it is multiplied).
+template <int LANES, int UNR, class Value, class Column>
+__device__ __forceinline__ double row_product(Value value, Column column, const double *x, int j, int e)
 {
     double acc = 0.0;
     while (j < e) {
         unsigned c[UNR];
-        double v[UNR], xv[UNR];
+        decltype(value(0)) v[UNR];
+        double xv[UNR];
 #pragma unroll
         for (int u = 0; u < UNR; ++u) {
             // clamp instead of predicating: unconditional loads batch freely (a predicated load per slot runs out
             // of predicate registers after 7); the FMA below is what is predicated
             const int idx = min(j + u * LANES, e - 1);
             c[u] = column(idx);
-            v[u] = sval[idx];
+            v[u] = value(idx);
         }
 #pragma unroll
         for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
 #pragma unroll
         for (int u = 0; u < UNR; ++u)
-            if (j + u * LANES < e) acc = fma(v[u], xv[u], acc);
+            if (j + u * LANES < e) acc = fma((double)v[u], xv[u], acc);
         j += UNR * LANES;
     }
     return lanes_sum<LANES>(acc);

@@ -152,6 +152,11 @@ struct MegaPlan {
     int4 *d_cta_dep = nullptr;
     unsigned short *d_col16 = nullptr;   // nnz + 16: 16-bit column codes of the CTAs whose column window fits them (mega.cu)
     bool stream_codes = true;    // streaming CTAs use d_col16 where they can (false: 32-bit columns; bicg_debug_stream_codes)
+    ValTable *d_vtab = nullptr;  // grid: every CTA's value table (mega.cu: mega_value_kernel)
+    unsigned char *d_vhi = nullptr;      // nnz + 16 each: the packed values of the CTAs that have codes and a value table
+    unsigned short *d_vmid = nullptr;
+    unsigned *d_vlo = nullptr;
+    bool stream_values = true;   // those CTAs stream the packed values (false: 8-byte values; bicg_debug_stream_values)
     int *d_tile_flag = nullptr;  // only when rows longer than a stage were cut into chunk tiles
     bool chunked = false;
     std::vector<int> cta_row;    // grid + 1: first row of every CTA

@@ -481,6 +481,9 @@ static void choose_spmv_plan(bicg_matrix *m, const unsigned *h_ptr)
                 m->plan.kind, m->plan.lanes, m->plan.threads, m->plan.stages, m->plan.ctas_per_sm, m->plan.ms);
 }
 
+// mean entries per row from which the persistent kernel's plan packs the values it streams (mega.cu: streams_values)
+constexpr double PACK_MIN_MEAN_ROW = 8.0;
+
 // lanes per row of the persistent kernel's SpMV (instantiated: 1, 4, 8, 32)
 static int mega_lanes_for(double mean_row)
 {
@@ -514,11 +517,12 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
         std::vector<unsigned> tile_nz;
         // a stage must hold one tile; at least two stages must fit.  Tiles (or single rows) with more entries than that
         // are cut by the planner: greedy tiles + chunked long rows (plan.cpp).  The producer loads a tile's entries from a
-        // window aligned to 8 entries at both ends (16-byte bulk copies of 2-byte column codes): up to 14 more than the tile.
-        const int cap_limit = (int)(((SMEM_MAX / 2 - (long long)(rpt + 8) * 4) / 12) / 32 * 32) - 64;   // cap = roundup(max + 16, 32) must still fit twice
+        // window aligned to 16 entries at both ends (16-byte bulk copies of the 1-byte plane of packed values): up to 30
+        // more than the tile.
+        const int cap_limit = (int)(((SMEM_MAX / 2 - (long long)(rpt + 8) * 4) / 12) / 32 * 32) - 64;   // cap = roundup(max + 30, 32) must still fit twice
         const unsigned max_tile_nnz = plan_cta_tiles(h_ptr, m->n_loc, G, rpt, row_extra.empty() ? nullptr : row_extra.data(),
                                                      c.cfg.boundary_weight, tile_row, cta_tile, cap_limit, &tile_nz, &tile_flag, c.cfg.row_weight);
-        const int cap = round_up((long long)max_tile_nnz + 16, 32);
+        const int cap = round_up((long long)max_tile_nnz + 30, 32);
         const long long stage = (long long)cap * 12 + (long long)(rpt + 8) * 4;
         int stages = (int)std::min<long long>(4, SMEM_MAX / stage);
         if (stages < 2) continue;                       // cannot happen with the cap-limited plan; kept as a guard
@@ -561,6 +565,23 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
         BICG_CUDA(cudaMemsetAsync(mp.d_col16 + m->nnz, 0, pad * sizeof(unsigned short), c.stream));
         launch_mega_code(m->d_col, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, G, m->ghost_off, mp.d_cta_dep, mp.d_col16, c.stream);
         BICG_CUDA(cudaGetLastError());
+        // value tables and packed values (streamed by the CTAs that also stream codes), padded like d_col16.  Not on
+        // short rows: a thread-per-row pass loads 16 slots per row, clamped at its end, and with 5-point rows the three
+        // plane loads per slot cost more shared-memory issue than the byte they save (5-point Laplacian 2000^2: 2.6 %
+        // slower on one H100 80GB HBM3 at 700 W).  Without the tables every CTA streams 8-byte values.
+        mp.d_vtab = nullptr; mp.d_vhi = nullptr; mp.d_vmid = nullptr; mp.d_vlo = nullptr;
+        if (m->mean_row >= PACK_MIN_MEAN_ROW) {
+            mp.d_vtab = (ValTable *)c.dev_alloc((size_t)G * sizeof(ValTable));
+            mp.d_vhi = (unsigned char *)c.dev_alloc(m->nnz + pad);
+            mp.d_vmid = (unsigned short *)c.dev_alloc((m->nnz + pad) * sizeof(unsigned short));
+            mp.d_vlo = (unsigned *)c.dev_alloc((m->nnz + pad) * sizeof(unsigned));
+            BICG_CUDA(cudaMemsetAsync(mp.d_vhi + m->nnz, 0, pad, c.stream));
+            BICG_CUDA(cudaMemsetAsync(mp.d_vmid + m->nnz, 0, pad * sizeof(unsigned short), c.stream));
+            BICG_CUDA(cudaMemsetAsync(mp.d_vlo + m->nnz, 0, pad * sizeof(unsigned), c.stream));
+            launch_mega_values(m->d_val, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, G, m->ghost_off, mp.d_cta_dep, mp.d_vtab, mp.d_vhi,
+                               mp.d_vmid, mp.d_vlo, c.stream);
+            BICG_CUDA(cudaGetLastError());
+        }
         mp.ok = true;
         if (c.cfg.verbose)
             fprintf(stderr, "[bicg mega r%d] threads=%d lanes=%d stages=%d cap=%d tiles=%d smem=%zu resident_smem=%zu\n", m->rank, threads, lanes,
@@ -901,6 +922,7 @@ void matrix_destroy(bicg_matrix *m)
     c.dev_free(m->d_trace);
     c.dev_free(m->mega.d_tile_row); c.dev_free(m->mega.d_tile_nz); c.dev_free(m->mega.d_cta_tile); c.dev_free(m->mega.d_cta_dep);
     c.dev_free(m->mega.d_col16); c.dev_free(m->mega.d_tile_flag);
+    c.dev_free(m->mega.d_vtab); c.dev_free(m->mega.d_vhi); c.dev_free(m->mega.d_vmid); c.dev_free(m->mega.d_vlo);
     if (m->hist_extra) cudaFree(m->hist_extra);
     c.dev_free(m->d_val); c.dev_free(m->d_col); c.dev_free(m->d_ptr);
     if (m->world > 1) c.arena_pool.emplace(m->arena_bytes, Context::ArenaRec{m->arena, m->arena_bytes, m->arena_id, m->arena_handle});

@@ -96,6 +96,7 @@ struct MegaShared {
     double scratch[32 * MAX_DOTS];
     unsigned long long full_bar[4], empty_bar[4];
     StageHdr hdr[4];
+    unsigned vadj[VAL_TABLE_MAX];             // the CTA's value table as PackedVal adds it (packed CTAs only)
     volatile int flags[4];                    // [1] producer stop, [2] consumed visits, [3] a wait timed out
 };
 
@@ -150,6 +151,39 @@ __device__ __forceinline__ bool streams_codes(const MegaArgs &a, const ResidentP
 {
     return a.stream_codes && a.col16 != nullptr && my_tiles > 0 && !rp.on && rp.w.ok;
 }
+// a CTA that streams codes and has a value table (mega_value_kernel) streams its values packed: 7 bytes instead of 8.
+// Decided like streams_codes, by the producer thread and by every consumer thread from the same inputs.
+__device__ __forceinline__ bool streams_values(const MegaArgs &a, bool coded)
+{
+    return coded && a.stream_values && a.vtab != nullptr && a.vtab[blockIdx.x].n > 0;
+}
+// A packed value is hi = table index << 4 | mantissa bits 51..48, mid = mantissa bits 47..32, lo = bits 31..0.
+// adj[i] = (field i << 20) - (i << 20) (mod 2^32), so hi << 16 = i << 20 | (bits 51..48) << 16 plus adj[i] is the high word
+// without bits 47..32, and mid fills those: the 64-bit pattern comes back exactly, with no floating-point operation.
+__device__ __forceinline__ unsigned val_adj(const ValTable &t, int i)
+{
+    return i < t.n ? ((unsigned)t.field[i] << 20) - ((unsigned)i << 20) : 0u;
+}
+// As loaded from a stage, a packed value is hm = hi << 16 | mid and lo; it is put together where it is multiplied, after
+// the gathers, so that it holds two registers while they are in flight, like an 8-byte value.  The planes and the table
+// are read through 32-bit shared-memory addresses: one register per base instead of a 64-bit generic pointer, which is
+// what keeps the 512-thread kernels within their register budget.
+__device__ __forceinline__ unsigned lds_u32(unsigned p) { unsigned v; asm volatile("ld.shared.u32 %0, [%1];" : "=r"(v) : "r"(p)); return v; }
+__device__ __forceinline__ unsigned lds_u16(unsigned p) { unsigned v; asm volatile("ld.shared.u16 %0, [%1];" : "=r"(v) : "r"(p)); return v; }
+__device__ __forceinline__ unsigned lds_u8(unsigned p) { unsigned v; asm volatile("ld.shared.u8 %0, [%1];" : "=r"(v) : "r"(p)); return v; }
+struct PackedVal {
+    unsigned hm, lo, adj;                         // adj: shared address of the table (MegaShared::vadj)
+    __device__ __forceinline__ operator double() const
+    {
+        return __hiloint2double((int)(hm + lds_u32(adj + (hm >> 20) * 4u)), (int)lo);
+    }
+};
+// entry idx of the planes of a stage that starts at shared address st and holds cap entries (spmv_impl<..., PACKED>)
+__device__ __forceinline__ PackedVal val_load(unsigned adj, unsigned st, unsigned cap, unsigned idx)
+{
+    const unsigned lo = lds_u32(st + idx * 4u), mid = lds_u16(st + cap * 4u + idx * 2u), hi = lds_u8(st + cap * 6u + idx);
+    return PackedVal{(hi << 16) | mid, lo, adj};
+}
 
 template <int CT, int LANES>
 struct Mega {
@@ -175,6 +209,7 @@ struct Mega {
     int trace_it, trace_who;
     bool resident;                // this CTA keeps its matrix slice in shared memory (ResidentPlan)
     bool coded;                   // this CTA streams 16-bit column codes (streams_codes)
+    bool packed;                  // this CTA streams 7-byte packed values (streams_values)
     ResidentPlan rp;
     const double *rs_val; const unsigned short *rs_col; const unsigned *rs_ptr;
 
@@ -434,8 +469,9 @@ struct Mega {
         if constexpr (LANES == 1) {
             if (resident) { spmv_res<EPI>(x, y, dot); return; }
         }
-        if (coded) spmv_impl<EPI, true>(x, y, dot);
-        else spmv_impl<EPI, false>(x, y, dot);
+        if (packed) spmv_impl<EPI, true, true>(x, y, dot);
+        else if (coded) spmv_impl<EPI, true, false>(x, y, dot);
+        else spmv_impl<EPI, false, false>(x, y, dot);
     }
     // one row's epilogue operands (EPI_RH_Y: r#; EPI_QY_YY: q, kept in v.r; EPI_CA4: r#, r, s, z), loaded before its gathers
     template <int EPI>
@@ -496,8 +532,10 @@ struct Mega {
     }
 
     // CODED: the stage's column area holds the CTA's 16-bit column codes (its first half; the stage layout is the same for
-    // both formats), each turned back into the column with one select and one add before its gather
-    template <int EPI, bool CODED>
+    // both formats), each turned back into the column with one select and one add before its gather.
+    // PACKED (CODED CTAs only): the stage's value area holds the three planes of the packed values -- vlo at 0, vmid at
+    // 4 cap bytes, vhi at 6 cap bytes -- each value put back together by PackedVal.
+    template <int EPI, bool CODED, bool PACKED>
     __device__ void spmv_impl(const double *x, double *y, double (&dot)[4])
     {
         const int stages = a.stages, cap = a.cap;
@@ -512,7 +550,12 @@ struct Mega {
             const unsigned *scol = reinterpret_cast<const unsigned *>(sval + cap);
             const unsigned short *scode = reinterpret_cast<const unsigned short *>(scol);
             const unsigned *sptr = scol + cap;
+            const unsigned sts = PACKED ? smem_u32(st) : 0u, adj = PACKED ? smem_u32(sh.vadj) : 0u;
             auto column = [&](unsigned idx) { return CODED ? col_decode(w, scode[idx]) : scol[idx]; };
+            auto value = [&](unsigned idx) {
+                if constexpr (PACKED) return val_load(adj, sts, (unsigned)cap, idx);
+                else return sval[idx];
+            };
             const StageHdr h = sh.hdr[s];
             if (h.flag != 0) {
                 // one chunk of a row longer than a stage: the whole CTA multiplies it, the row's partial sum is carried
@@ -523,7 +566,7 @@ struct Mega {
 #pragma unroll
                     for (int u = 0; u < 4; ++u) {
                         const unsigned idx = min(jj + (unsigned)(u * CT), h.hi - 1u);
-                        pv[u] = sval[idx]; px[u] = ld_coherent(x + column(idx));
+                        pv[u] = (double)value(idx); px[u] = ld_coherent(x + column(idx));
                     }
 #pragma unroll
                     for (int u = 0; u < 4; ++u)
@@ -554,7 +597,7 @@ struct Mega {
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
                 if (sub == 0) epi_load<EPI>(row, e0, e1, e2, e3);
             }
-            const double acc = row_product<LANES, UNR>(sval, column, x, j, e);
+            const double acc = row_product<LANES, UNR>(value, column, x, j, e);
             if (valid && sub == 0) row_done<EPI>(row, acc, e0, e1, e2, e3, y, dot);
             __syncwarp();
             if (lane == 0) mbar_arrive(smem_u32(&sh.empty_bar[s]));
@@ -772,7 +815,9 @@ struct Mega {
         }
     }
     // ---------------------------------------------------------------- solver.c:216-259 ----------------------
-    __device__ void run_ca()
+    // __noinline__: inlined into the kernel body next to the packed-value SpMV, it makes the 512-thread kernels with
+    // LANES > 1 spill
+    __device__ __noinline__ void run_ca()
     {
         double d5[5], d4[4], d2[2], d1[1], d0[1];
         d0[0] = 0.0;
@@ -873,9 +918,11 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
             volatile int *flags = sh.flags;
             const unsigned long long pol = l2_evict_first_policy();
             // 16-bit codes: 2 bytes per entry; a bulk copy moves whole 16-byte units, so the entry window of a tile is
-            // aligned to 8 entries (4 suffice for 4-byte columns); the plan's stage capacity covers the wider window
+            // aligned to 8 entries (4 suffice for 4-byte columns), and to 16 for the 1-byte plane of packed values; the
+            // plan's stage capacity covers the widest window
             const bool coded = streams_codes(a, rp, my_tiles);
-            const unsigned al = coded ? 7u : 3u, cbytes = coded ? 2u : 4u;
+            const bool packed = streams_values(a, coded);
+            const unsigned al = packed ? 15u : (coded ? 7u : 3u), cbytes = coded ? 2u : 4u, vbytes = packed ? 7u : 8u;
             const void *cols = coded ? (const void *)a.col16 : (const void *)a.col;
             unsigned v = 0;
             bool stop = false;
@@ -898,10 +945,16 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
                 unsigned *sptr = scol + cap;
                 sh.hdr[s] = StageHdr{row0, row1, a0, rowa, p0 - a0, p1 - a0, a.tile_flag ? a.tile_flag[t] : 0, 0};
                 const unsigned bar = smem_u32(&sh.full_bar[s]);
-                mbar_arrive_expect_tx(bar, cnt * (8u + cbytes) + (unsigned)cntp * 4u);
+                mbar_arrive_expect_tx(bar, cnt * (vbytes + cbytes) + (unsigned)cntp * 4u);
                 if (cnt) {
                     const void *csrc = (const char *)cols + (size_t)a0 * cbytes;
-                    tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
+                    if (packed) {                               // the stage layout of spmv_impl<..., PACKED>
+                        tma_load_1d_hint(smem_u32(st), a.vlo + a0, cnt * 4u, bar, pol);
+                        tma_load_1d_hint(smem_u32(st + (size_t)cap * 4u), a.vmid + a0, cnt * 2u, bar, pol);
+                        tma_load_1d_hint(smem_u32(st + (size_t)cap * 6u), a.vhi + a0, cnt, bar, pol);
+                    } else {
+                        tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
+                    }
                     tma_load_1d_hint(smem_u32(scol), csrc, cnt * cbytes, bar, pol);
                 }
                 tma_load_1d(smem_u32(sptr), a.ptr + rowa, (unsigned)cntp * 4u, bar);
@@ -959,6 +1012,8 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
         m.rp = resident_plan(a, t0, t1, LANES);
         m.resident = m.rp.on;
         m.coded = streams_codes(a, m.rp, my_tiles);
+        m.packed = streams_values(a, m.coded);
+        if (m.packed && tid < VAL_TABLE_MAX) sh.vadj[tid] = val_adj(a.vtab[blockIdx.x], tid);
         if (m.resident) {
             const size_t nnzp = ((size_t)m.rp.nnz + 7u) & ~(size_t)7u;
             double *sv = reinterpret_cast<double *>(dyn_smem);
@@ -973,6 +1028,7 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
             if (tid == 0) atomicAdd(&a.sync->st.resident_ctas, 1);
         }
         if (m.coded && tid == 0) atomicAdd(&a.sync->st.coded_ctas, 1);
+        if (m.packed && tid == 0) atomicAdd(&a.sync->st.packed_ctas, 1);
         nbar(1, CT);
         if (a.comm.world > 1 && (m.reads_ghost || m.gs_hi > m.gs_lo)) {
             // the vectors the first phases read were pushed by the init kernels (kernel-per-phase protocol)
@@ -1031,6 +1087,53 @@ __global__ void __launch_bounds__(256) mega_code_kernel(const unsigned *__restri
     if (r1 <= r0) return;
     const unsigned e0 = ptr[r0], e1 = ptr[r1];
     for (unsigned j = e0 + threadIdx.x; j < e1; j += blockDim.x) col16[j] = col_encode(w, ghost_off, col[j]);
+}
+
+// The value table of every CTA: the distinct sign / exponent fields (bits 63..52) of its entries, ascending -- a set, so
+// it does not depend on the order in which threads find them -- or n = 0 beyond VAL_TABLE_MAX fields.  A CTA that has a
+// table and column codes (col_window) also gets its entries packed; the entries of the other CTAs are not written.  The
+// split works on the bit pattern, so +-0.0, subnormals and every other value round-trip exactly.
+__global__ void __launch_bounds__(256) mega_value_kernel(const double *__restrict__ val, const unsigned *__restrict__ ptr,
+                                                         const int *__restrict__ tile_row, const int *__restrict__ cta_tile,
+                                                         int ghost_off, const int4 *__restrict__ dep, ValTable *__restrict__ vtab,
+                                                         unsigned char *__restrict__ vhi, unsigned short *__restrict__ vmid,
+                                                         unsigned *__restrict__ vlo)
+{
+    constexpr int W = 4096 / 32;
+    __shared__ unsigned seen[W];                  // bit f: some entry of the CTA has field f
+    __shared__ int below[W];                      // fields in the words before: the table index of field f is
+    __shared__ int total;                         // below[f / 32] + the bits of seen[f / 32] under f
+    for (int i = threadIdx.x; i < W; i += blockDim.x) seen[i] = 0u;
+    __syncthreads();
+    const int r0 = tile_row[cta_tile[blockIdx.x]], r1 = tile_row[cta_tile[blockIdx.x + 1]];
+    const unsigned e0 = r1 > r0 ? ptr[r0] : 0u, e1 = r1 > r0 ? ptr[r1] : 0u;
+    for (unsigned j = e0 + threadIdx.x; j < e1; j += blockDim.x) {
+        const unsigned f = (unsigned)((unsigned long long)__double_as_longlong(val[j]) >> 52), b = 1u << (f & 31u);
+        if (!(seen[f >> 5] & b)) atomicOr(&seen[f >> 5], b);       // a plain read first: the set is small and soon complete
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int n = 0;
+        for (int i = 0; i < W; ++i) { below[i] = n; n += __popc(seen[i]); }
+        total = n;
+        ValTable t;
+        t.n = n <= VAL_TABLE_MAX ? n : 0;
+        for (int k = 0; k < VAL_TABLE_MAX; ++k) t.field[k] = 0;
+        int k = 0;
+        for (int i = 0; i < W && t.n > 0; ++i)
+            for (unsigned b = seen[i]; b; b &= b - 1u) t.field[k++] = (unsigned short)(i * 32 + __ffs((int)b) - 1);
+        vtab[blockIdx.x] = t;
+    }
+    __syncthreads();
+    if (total == 0 || total > VAL_TABLE_MAX || !col_window(dep[blockIdx.x], ghost_off).ok) return;
+    for (unsigned j = e0 + threadIdx.x; j < e1; j += blockDim.x) {
+        const unsigned long long bits = (unsigned long long)__double_as_longlong(val[j]);
+        const unsigned f = (unsigned)(bits >> 52);
+        const unsigned idx = (unsigned)below[f >> 5] + __popc(seen[f >> 5] & ((1u << (f & 31u)) - 1u));
+        vhi[j] = (unsigned char)((idx << 4) | ((unsigned)(bits >> 48) & 15u));
+        vmid[j] = (unsigned short)(bits >> 32);
+        vlo[j] = (unsigned)bits;
+    }
 }
 
 template <int CT, int LANES>
@@ -1096,6 +1199,13 @@ void launch_mega_code(const unsigned *col, const unsigned *ptr, const int *tile_
                       int ghost_off, const int4 *dep, unsigned short *col16, cudaStream_t st)
 {
     mega_code_kernel<<<grid, 256, 0, st>>>(col, ptr, tile_row, cta_tile, ghost_off, dep, col16);
+}
+
+void launch_mega_values(const double *val, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
+                        int ghost_off, const int4 *dep, ValTable *vtab, unsigned char *vhi, unsigned short *vmid,
+                        unsigned *vlo, cudaStream_t st)
+{
+    mega_value_kernel<<<grid, 256, 0, st>>>(val, ptr, tile_row, cta_tile, ghost_off, dep, vtab, vhi, vmid, vlo);
 }
 
 } // namespace bicg

@@ -22,6 +22,7 @@ struct alignas(128) MegaState {
     int plan_ok[MAX_RANKS];             // written by rank p at plan time: its persistent-kernel plan is usable
     int resident_ctas;                  // CTAs of the last launch that kept their matrix slice in shared memory (test / trace aid)
     int coded_ctas;                     // CTAs of the last launch that streamed 16-bit column codes (test / trace aid)
+    int packed_ctas;                    // CTAs of the last launch that streamed 7-byte packed values (test / trace aid)
 };
 
 // Lives in the IPC-shared arena: `mail` and `st.plan_ok` are written by the peers.
@@ -44,6 +45,12 @@ struct PushPlan {
 // LL halo regions (one per pushed vector; s has two because the multi-GPU BiCGStab loop double-buffers it)
 enum LLRegion : int { LL_S0 = 0, LL_S1, LL_R, LL_P, LL_Z, LL_X, LL_W, LL_REGIONS };
 
+// A CTA's value table (mega_value_kernel): the distinct sign / exponent fields (value bits 63..52) of its entries in
+// ascending order; n = 0 when there are more than VAL_TABLE_MAX of them (or no entries).  With a table every value is
+// its 4-bit table index plus its 52 mantissa bits: 7 bytes, lossless on the bit pattern.
+constexpr int VAL_TABLE_MAX = 16;
+struct ValTable { int n; unsigned short field[VAL_TABLE_MAX]; };
+
 constexpr int MEGA_TRACE_ITERS = 256, MEGA_TRACE_SLOTS = 16;
 
 struct MegaArgs {
@@ -58,6 +65,12 @@ struct MegaArgs {
     const unsigned *col;
     const unsigned short *col16;   // per entry: 16-bit code of the column in its CTA's column window (mega_code_kernel),
                                    // filled for the CTAs whose window fits 16 bits; what the resident load copies
+    const ValTable *vtab;       // [grid]: the CTA's value table (mega_value_kernel)
+    // per entry, for the CTAs that stream codes and have a value table: the value as table index | mantissa bits 51..48
+    // (vhi), mantissa bits 47..32 (vmid) and 31..0 (vlo) -- 7 bytes instead of 8
+    const unsigned char  *vhi;
+    const unsigned short *vmid;
+    const unsigned       *vlo;
     const unsigned *ptr;
     const int      *tile_row;   // ntiles + 1
     const unsigned *tile_nz;    // ntiles + 1
@@ -70,6 +83,8 @@ struct MegaArgs {
                                 //    through the TMA ring in every SpMV
     int stream_codes;           // 1: a streaming CTA whose column window fits 16 bits streams col16 (10 bytes per entry
                                 //    instead of 12); 0: every streaming CTA streams the 32-bit columns
+    int stream_values;          // 1: a CTA that streams codes and has a value table streams the packed values (9 bytes per
+                                //    entry with the codes instead of 10); 0: every streaming CTA streams the 8-byte values
     int smem_bytes;             // dynamic shared memory of this launch
     double *vec_base; long long vstride;   // arena vectors: vec(id) = vec_base + id * vstride
     VecPtrs v;
@@ -99,5 +114,10 @@ void   launch_mega_dep(const unsigned *col, const unsigned *ptr, const int *tile
 // 16-bit column codes of the CTAs whose column window fits them (one launch at plan time, behind launch_mega_dep)
 void   launch_mega_code(const unsigned *col, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
                         int ghost_off, const int4 *dep, unsigned short *col16, cudaStream_t st);
+// value table of every CTA and, where the CTA also has column codes, its packed values (one launch at plan time, behind
+// launch_mega_dep)
+void   launch_mega_values(const double *val, const unsigned *ptr, const int *tile_row, const int *cta_tile, int grid,
+                          int ghost_off, const int4 *dep, ValTable *vtab, unsigned char *vhi, unsigned short *vmid,
+                          unsigned *vlo, cudaStream_t st);
 
 } // namespace bicg

@@ -159,6 +159,8 @@ struct Seq : PhaseLauncher {
         a.n_ghost = m->n_ghost; a.cta_dep = m->mega.d_cta_dep;
         a.val = m->d_val; a.col = m->d_col; a.col16 = m->mega.d_col16; a.ptr = m->d_ptr;
         a.stream_codes = m->mega.stream_codes ? 1 : 0;
+        a.vtab = m->mega.d_vtab; a.vhi = m->mega.d_vhi; a.vmid = m->mega.d_vmid; a.vlo = m->mega.d_vlo;
+        a.stream_values = m->mega.stream_values ? 1 : 0;
         a.tile_row = m->mega.d_tile_row; a.tile_nz = m->mega.d_tile_nz; a.cta_tile = m->mega.d_cta_tile;
         a.tile_flag = m->mega.d_tile_flag;
         a.cap = m->mega.cap; a.stages = m->mega.stages;
@@ -185,6 +187,7 @@ struct Seq : PhaseLauncher {
         a.snap_iter = 50;
         BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.resident_ctas, 0, sizeof(int), c.stream));
         BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.coded_ctas, 0, sizeof(int), c.stream));
+        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.packed_ctas, 0, sizeof(int), c.stream));
         int rc = launch_mega(m->mega.threads, m->mega.lanes, m->mega.grid, smem, a, c.stream);
         if (rc) {
             // e.g. the grid cannot be co-resident because something else holds SMs.  Single rank: not an error, the
@@ -646,6 +649,24 @@ extern "C" int bicg_debug_stream_codes(bicg_matrix *m, int on)
 {
     const int was = m->mega.stream_codes ? 1 : 0;
     m->mega.stream_codes = on != 0;
+    return was;
+}
+
+extern "C" int bicg_debug_packed_ctas(bicg_matrix *m)
+{
+    using namespace bicg;
+    Context &c = ctx();
+    c.ensure();
+    int n = 0;
+    BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.packed_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    return n;
+}
+
+extern "C" int bicg_debug_stream_values(bicg_matrix *m, int on)
+{
+    const int was = m->mega.stream_values ? 1 : 0;
+    m->mega.stream_values = on != 0;
     return was;
 }
 

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
                 j = (int)(sptr[row - h.rowa] - h.a0) + lane;
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
             }
-            double acc = row_product<LANES, UNR>(sval, [&](int idx) { return scol[idx]; }, x, j, e);
+            double acc = row_product<LANES, UNR>([&](int idx) { return sval[idx]; }, [&](int idx) { return scol[idx]; }, x, j, e);
             if (valid && lane == 0) {
                 if (a.shift_sigma) acc = fma(*a.shift_sigma, ld_coherent(x + row), acc);     // s += sigma p (daxpy after the SpMV)
                 a.y[row] = acc;
