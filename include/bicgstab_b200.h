@@ -184,6 +184,47 @@ typedef struct {
 int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors,
                bicg_stats *stats);
 
+/* Written by the device at the end of an asynchronous solve, in stream order (24 bytes): the iters, converged and
+ * final_res that bicg_solve reports in bicg_stats for the same solve, and error = 1 if a bounded wait for a peer GPU or
+ * another CTA timed out (BICG_PEER_TIMEOUT_S). */
+typedef struct {
+    int    iters;
+    int    converged;
+    int    error;
+    int    reserved;
+    double final_res;
+} bicg_result;
+
+/* bicg_solve with device vectors, enqueued on the caller's CUDA stream `stream` (a cudaStream_t; 0 is CUDA's default
+ * stream, not the library's).  x and r are device pointers to n_loc doubles, updated in place, with the meaning of
+ * bicg_solve.  `result`, if not null, is device memory that receives the solve's bicg_result.  Returns 0 once the work is
+ * enqueued, with no host synchronisation, allocation, pageable copy or output; -1 for a null x / r or an unknown method
+ * (PIPE_RR with krr <= 0 runs PIPE, as in bicg_solve); -2 inside a stream capture when bicg_solve_async_prepare has not
+ * been called for this handle and method under the current options (the capture stays valid).  Options (TOL, MAX_ITER,
+ * MEGA, RESIDENT, UNROLL, ...) are read at enqueue time; a captured solve keeps the values it was captured with.
+ * The x, r and history it computes are bit-identical to bicg_solve's.
+ *
+ * Ordering: every call on a handle shares its device state, so each asynchronous call waits for the handle's previous
+ * asynchronous work and every synchronous entry point waits for it too.  A captured solve orders its replays the same
+ * way, but a replay must not run concurrently with other work on the same handle that was not enqueued after it.
+ * Not updated by asynchronous solves: bicg_last_stats, bicg_last_history and the stdout lines (BICG_MEGA_TRACE and
+ * bicg_profile_solve stay synchronous).  With several ranks the call is collective like bicg_solve: every rank enqueues,
+ * or replays, the same sequence on the handle.
+ *
+ * bicg_solve_async_prepare builds, outside any capture, what the asynchronous path needs on this handle and method: the
+ * graphs of the device-side loop and a history for the current MAX_ITER.  It may synchronise and allocate; an uncaptured
+ * bicg_solve_async calls it itself.  The handle's first prepare also orders every later asynchronous call on it behind the
+ * work already enqueued on the library's stream (the upload of bicg_matrix_create).  Raising MAX_ITER past the handle's
+ * history capacity moves its history: a solve captured before that keeps writing the old one, so prepare and capture again.
+ * Returns 0, or -1 for an unknown method.
+ *
+ * bicg_matrix_history waits for the last work enqueued on m and copies that solve's history (dot_r/dot_zero after every
+ * iteration, out[0] = 1) like bicg_last_history; returns the number of entries.  A peer timeout of that solve is fatal
+ * here, as it is in bicg_solve. */
+int bicg_solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, void *stream, bicg_result *result);
+int bicg_solve_async_prepare(bicg_matrix *m, int method);
+int bicg_matrix_history(bicg_matrix *m, double *out, int cap);
+
 /* shifted_lopbicg_switching on a resident matrix; bicg_last_shift_info: the seed the last shifted solve ended with and the
  * iteration at which every shift stopped (returns sigma_len).  The stop iteration is 1-based (the iteration after whose
  * convergence test the shift stopped), 0 for a shift that never stopped; for shifted_lopbicg the seed is the one passed in.

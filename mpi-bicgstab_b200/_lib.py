@@ -30,6 +30,12 @@ class bicg_stats(C.Structure):
                 ("spmv_lanes", C.c_int), ("spmv_kind", C.c_int)]
 
 
+class bicg_result(C.Structure):
+    """What an asynchronous solve writes to device memory at its end (24 bytes)."""
+    _fields_ = [("iters", C.c_int), ("converged", C.c_int), ("error", C.c_int), ("reserved", C.c_int),
+                ("final_res", C.c_double)]
+
+
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 
 # every symbol include/bicgstab_b200.h declares: (restype, argtypes)
@@ -69,6 +75,9 @@ SYMBOLS = {
     "bicg_matrix_destroy": (None, [C.c_void_p]),
     "bicg_matrix_invalidate": (None, [_P(CSR_Matrix)]),
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
+    "bicg_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "bicg_solve_async_prepare": (C.c_int, [C.c_void_p, C.c_int]),
+    "bicg_matrix_history": (C.c_int, [C.c_void_p, _P(C.c_double), C.c_int]),
     "bicg_shifted_solve": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_last_shift_info": (C.c_int, [_P(C.c_int), _P(C.c_int), C.c_int]),
     "bicg_shifted_solve_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),

@@ -13,7 +13,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_stats, lib
+from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_result, bicg_stats, lib
 
 METHODS = {"bicgstab": 0, "ca_bicgstab": 1, "pipe_bicgstab": 2, "pipe_bicgstab_rr": 3}
 SHIFTED_METHODS = {"shifted_lopbicg_switching": 0, "shifted_lopbicgstab": 1, "shifted_pipe_lopbicgstab": 2}
@@ -266,9 +266,18 @@ def shifted_pipe_lopbicgstab(blk, x_set, r_loc, sigma, seed):
 
 
 def _cuda_vectors(*args):
+    """Device pointers of CUDA float64 torch tensors, given as (name, tensor, expected shape) triples, checked by
+    _checked_cuda_vectors.  Then torch's current stream is synchronised, because the library works on its own stream."""
+    import torch
+    ptrs = _checked_cuda_vectors(*args)
+    torch.cuda.current_stream(args[0][1].device).synchronize()
+    return ptrs
+
+
+def _checked_cuda_vectors(*args):
     """Device pointers of CUDA float64 torch tensors, given as (name, tensor, expected shape) triples.  Everything the library
     cannot check itself is checked here, before it is called: all are torch tensors, float64, contiguous, of the expected shape,
-    on the library's GPU.  Then torch's current stream is synchronised, because the library works on its own stream."""
+    on the library's GPU."""
     import torch
     checks = [(lambda t, s: isinstance(t, torch.Tensor), TypeError,
                lambda t, s: f"numpy arrays and torch tensors cannot be mixed in one call (got {type(t).__name__})"),
@@ -284,7 +293,6 @@ def _cuda_vectors(*args):
     for name, t, _ in args:
         if t.device.index != dev:
             raise ValueError(f"{name}: tensor on {t.device}, the library runs on cuda:{dev}")
-    torch.cuda.current_stream(args[0][1].device).synchronize()
     return [C.c_void_p(t.data_ptr()) for _, t, _ in args]
 
 
@@ -329,6 +337,19 @@ def last_history():
     return out[:n]
 
 
+def decode_result(t, stream=None):
+    """The bicg_result an asynchronous solve wrote into the 24-byte tensor `t`, as a dict with iters, converged, error and
+    final_res.  The copy to the host is ordered after torch's current stream only: pass the stream the solve was enqueued on
+    when it was another one, and it is synchronised first (or synchronise it yourself)."""
+    if stream is not None:
+        stream.synchronize()
+    raw = bytes(t.detach().cpu().numpy().tobytes()) if hasattr(t, "detach") else bytes(np.asarray(t, dtype=np.uint8))
+    if len(raw) != C.sizeof(bicg_result):
+        raise ValueError(f"a bicg_result has {C.sizeof(bicg_result)} bytes, got {len(raw)}")
+    r = bicg_result.from_buffer_copy(raw)
+    return {f: getattr(r, f) for f, _ in bicg_result._fields_ if f != "reserved"}
+
+
 def _stats_dict(s):
     return {f: getattr(s, f) for f, _ in bicg_stats._fields_}
 
@@ -357,6 +378,45 @@ class DeviceMatrix:
         st = bicg_stats()
         it = lib.bicg_solve(self.h, METHODS[method], xp, rp, krr, nrr, dev, C.byref(st))
         return it, _stats_dict(st)
+
+    def solve_async(self, method, x, r, krr=0, nrr=0, result=None, stream=None):
+        """bicg_solve_async: the solve of solve() on CUDA tensors, enqueued on `stream` (default: torch's current stream) without
+        waiting for it or for anything before it.  x (initial guess in, solution out) and r (b in, final residual out) are
+        contiguous CUDA float64 tensors of shape (n_loc,), updated in place in stream order.  `result`: a 24-byte uint8 CUDA
+        tensor that receives the bicg_result (decode_result reads it); allocated when not given.  Works inside
+        torch.cuda.graph once prepare_async(method) has been called.  Returns the result tensor."""
+        import torch
+        n = self.blk.n_loc
+        xp, rp = _checked_cuda_vectors(("x", x, (n,)), ("r", r, (n,)))
+        nbytes = C.sizeof(bicg_result)
+        if stream is None:
+            stream = torch.cuda.current_stream(x.device)
+        if result is None:
+            result = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+            result.record_stream(stream)          # written on `stream`, which need not be the one it was allocated on
+        elif not (isinstance(result, torch.Tensor) and result.is_cuda and result.dtype == torch.uint8 and result.is_contiguous()
+                  and result.numel() == nbytes and result.device == x.device and result.data_ptr() % 8 == 0):
+            raise ValueError(f"result: need a contiguous, 8-byte aligned uint8 CUDA tensor of {nbytes} elements on {x.device}")
+        rc = lib.bicg_solve_async(self.h, METHODS[method], xp, rp, int(krr), int(nrr), C.c_void_p(stream.cuda_stream),
+                                  C.c_void_p(result.data_ptr()))
+        if rc == -2:
+            raise RuntimeError(f"solve_async inside a stream capture needs prepare_async({method!r}) first")
+        if rc != 0:
+            raise ValueError(f"bicg_solve_async failed with {rc}")
+        return result
+
+    def prepare_async(self, method):
+        """bicg_solve_async_prepare: build what solve_async needs for `method` under the current options, outside any capture."""
+        if lib.bicg_solve_async_prepare(self.h, METHODS[method]) != 0:
+            raise ValueError(f"bicg_solve_async_prepare({method}) failed")
+
+    def history(self):
+        """bicg_matrix_history: dot_r/dot_zero after every iteration of the last solve enqueued on this handle, synchronous or
+        asynchronous (waits for it; entry 0 = 1)."""
+        n = lib.bicg_matrix_history(self.h, None, 0)
+        out = np.empty(max(n, 1))
+        n = lib.bicg_matrix_history(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), n)
+        return out[:n]
 
     def shifted_solve(self, method, x_set, r, sigma, seed):
         """bicg_shifted_solve_ex: method is a key of SHIFTED_SOLVE_EX; returns (that solver's return value, stats).  x_set

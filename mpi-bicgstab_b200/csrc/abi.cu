@@ -15,6 +15,9 @@ static_assert(offsetof(CSR_Matrix, col) == 8 && offsetof(CSR_Matrix, ptr) == 16 
 static_assert(sizeof(INFO_Matrix) == 32, "INFO_Matrix layout must match matrix.h:28-33");
 static_assert(offsetof(INFO_Matrix, code) == 12 && offsetof(INFO_Matrix, recvcounts) == 16 &&
               offsetof(INFO_Matrix, displs) == 24, "INFO_Matrix layout");
+static_assert(sizeof(bicg_result) == 24 && offsetof(bicg_result, iters) == 0 && offsetof(bicg_result, converged) == 4 &&
+              offsetof(bicg_result, error) == 8 && offsetof(bicg_result, reserved) == 12 &&
+              offsetof(bicg_result, final_res) == 16, "bicg_result layout of include/bicgstab_b200.h");
 
 namespace {
 
@@ -207,6 +210,12 @@ int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nr
 {
     return solve(m, method, x, r, krr, nrr, device_vectors, stats);
 }
+int bicg_solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, void *stream, bicg_result *result)
+{
+    return solve_async(m, method, x, r, krr, nrr, (cudaStream_t)stream, result);
+}
+int bicg_solve_async_prepare(bicg_matrix *m, int method) { return solve_async_prepare(m, method); }
+int bicg_matrix_history(bicg_matrix *m, double *out, int cap) { return matrix_history(m, out, cap); }
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_host(m, x_loc, y_loc, nullptr); }
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {

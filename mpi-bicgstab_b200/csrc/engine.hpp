@@ -162,6 +162,16 @@ struct MegaPlan {
     std::vector<int> cta_row;    // grid + 1: first row of every CTA
 };
 
+// The loop of an asynchronous solve on the kernel-per-phase path (solve.cu): templates captured from the same sequence as
+// ensure_graph, and the executable graph of one WHILE node around them that an uncaptured call launches.
+struct AsyncLoopState { int count, batches, krr, nrr; };   // device memory: bodies run, their bound, PIPE_RR's schedule
+struct AsyncLoop {
+    cudaGraph_t iters = nullptr;      // `unroll` iterations (PIPE_RR: one pipe_iter)
+    cudaGraph_t rr = nullptr;         // PIPE_RR: one rr_replace_iter
+    cudaGraphExec_t exec = nullptr;
+    int unroll = 0;
+};
+
 } // namespace bicg
 
 // the opaque handle of the C ABI
@@ -221,6 +231,13 @@ struct bicg_matrix {
     double upload_ms = 0.0;
     cudaEvent_t ev_upload0 = nullptr, ev_upload1 = nullptr;   // around upload + planning; read lazily (matrix_upload_ms)
     uint64_t upload_bytes = 0;
+    // asynchronous solves (bicg_solve_async): the last work they enqueued on this handle, which every later call waits for,
+    // the device state of their loop, and per method what bicg_solve_async_prepare built
+    cudaEvent_t ev_last = nullptr;
+    bicg::AsyncLoopState *d_loop = nullptr;
+    bicg::AsyncLoop async[4];
+    bool captured = false;                // a caller has captured a solve on this handle into a graph
+    std::vector<double *> hist_retired;   // histories replaced while such a graph may still write them
 
     double *vec(int id) const { return vec_base + (long long)id * vstride; }
 };
@@ -234,11 +251,20 @@ double matrix_upload_ms(bicg_matrix *m);
 bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, bool *fresh);
 // solve.cu
 int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *st);
+// bicg_solve_async / bicg_solve_async_prepare / bicg_matrix_history (include/bicgstab_b200.h)
+int  solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, cudaStream_t st, bicg_result *result);
+int  solve_async_prepare(bicg_matrix *m, int method);
+int  matrix_history(bicg_matrix *m, double *out, int cap);
+// every synchronous entry point that touches a handle first makes the library's stream wait for the handle's last
+// asynchronous work (free when there is none)
+void wait_handle(bicg_matrix *m);
+void drop_async_loop(AsyncLoop &L);        // frees what bicg_solve_async_prepare built for one method
 int  spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full_or_null);
 int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);
 void print_times(double seconds, double iters);          // "Total time" / "Avg time/iter" (= seconds / iters), then flush
 void reset_scalars(bicg_matrix *m, double tol, int max_iter);   // Scalars of a new solve (enqueued on the stream)
+void reset_scalars(bicg_matrix *m, double tol, int max_iter, cudaStream_t st);
 // The host side of every kernel-per-phase loop: enqueues batch b = 0, 1, ... of U iterations (max_iter / U rounded up)
 // and reads the device's done flag *d_done after each; from batch `depth` on it first waits for batch b - depth and
 // stops once the flag was raised by its end.  The loop test runs on the device, which returns from every kernel after it.
@@ -255,7 +281,7 @@ std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long 
 std::vector<double> shift_relative_errors(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
-void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, int prof_class = 0);
+void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class = 0);
 
 // reduction tails of the kernel-per-phase kernels
 inline TailDesc tail_none() { return TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0}; }
@@ -272,8 +298,10 @@ struct PhaseLauncher {
     Context &c;
     const double *shift_sigma = nullptr;   // device scalar sigma: every SpMV computes y = (A + sigma I) x; null: y = A x
     int launches = 0;                      // kernels launched through vec / spmv (a graph capture takes them back out)
+    cudaStream_t stream;                   // where they go: the library's stream unless an asynchronous solve names another
 
-    explicit PhaseLauncher(bicg_matrix *mm) : m(mm), c(ctx()) {}
+    explicit PhaseLauncher(bicg_matrix *mm) : m(mm), c(ctx()), stream(c.stream) {}
+    PhaseLauncher(bicg_matrix *mm, cudaStream_t st) : m(mm), c(ctx()), stream(st) {}
     VecPtrs ptrs() const;
     KernelCommon common(TailDesc tail) const;
     // the boundary runs of arena vector `id` into its ghost slots on the peers; push_src: take the values from there instead

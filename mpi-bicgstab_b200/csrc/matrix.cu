@@ -355,20 +355,20 @@ SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y
     return a;
 }
 
-void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, int prof_class)
+void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class)
 {
     Context &c = ctx();
     (void)m;
     if (c.prof_on) {
         cudaEvent_t e0, e1;
         BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
-        BICG_CUDA(cudaEventRecord(e0, c.stream));
-        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, c.stream);
+        BICG_CUDA(cudaEventRecord(e0, st));
+        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, st);
         if (rc) fatal("bicgstab_b200: SpMV launch failed: %s", cudaGetErrorString((cudaError_t)rc));
-        BICG_CUDA(cudaEventRecord(e1, c.stream));
+        BICG_CUDA(cudaEventRecord(e1, st));
         c.prof_ev.push_back(e0); c.prof_ev.push_back(e1); c.prof_class.push_back(prof_class);
     } else {
-        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, c.stream);
+        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, st);
         if (rc) fatal("bicgstab_b200: SpMV launch failed (kind %d lanes %d threads %d grid %d smem %zu): %s",
                       p.kind, p.lanes, p.threads, p.grid, p.smem, cudaGetErrorString((cudaError_t)rc));
     }
@@ -384,9 +384,9 @@ static double time_plan(bicg_matrix *m, const SpmvPlan &p, int reps)
     epi_add_dot(a.epi, m->vec(V_RH), nullptr);
     cudaEvent_t e0, e1;
     BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
-    for (int i = 0; i < 2; ++i) launch_spmv_plan(m, p, a);
+    for (int i = 0; i < 2; ++i) launch_spmv_plan(m, p, a, c.stream);
     BICG_CUDA(cudaEventRecord(e0, c.stream));
-    for (int i = 0; i < reps; ++i) launch_spmv_plan(m, p, a);
+    for (int i = 0; i < reps; ++i) launch_spmv_plan(m, p, a, c.stream);
     BICG_CUDA(cudaEventRecord(e1, c.stream));
     BICG_CUDA(cudaEventSynchronize(e1));
     float ms = 0.f;
@@ -909,11 +909,15 @@ void matrix_destroy(bicg_matrix *m)
     if (!m) return;
     Context &c = ctx();
     if (c.ready) cudaStreamSynchronize(c.stream);
+    if (m->ev_last) { cudaEventSynchronize(m->ev_last); cudaEventDestroy(m->ev_last); }
     (void)matrix_upload_ms(m);
     for (auto it = c.cache.begin(); it != c.cache.end();) {
         if (it->second == m) it = c.cache.erase(it); else ++it;
     }
     for (int g = 0; g < 4; ++g) if (m->graph[g]) cudaGraphExecDestroy(m->graph[g]);
+    for (AsyncLoop &L : m->async) drop_async_loop(L);
+    c.dev_free(m->d_loop);
+    for (double *h : m->hist_retired) cudaFree(h);
     // world > 1: nothing collective here.  The arena is parked, not freed (the peers keep their mappings), and a rank
     // that has finished its solve has received everything its peers will ever write into this arena: the last
     // reduction completes only after every rank's last push and post (DESIGN.md 4).

@@ -145,6 +145,7 @@ std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long 
 {
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     const int n = m->n_loc, W = L + 1;
     const bool peers = m->world > 1;
     const int nj_max = std::min(L, peers ? SC_B : SC_LAUNCH);  // shifts per launch

@@ -447,6 +447,7 @@ int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const do
 {
     ctx().ensure();
     if (L <= 0 || seed < 0 || seed >= L) return -1;
+    wait_handle(m);
     switch (method) {
     case BICG_SHIFTED_SWITCHING: return switching_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter, dev);
     case BICG_SHIFTED_LOPBICG:   return switching_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);

@@ -41,11 +41,57 @@ __global__ void fill_kernel(double *p, int n, double v)
 
 __global__ void set_coef_kernel(Scalars *s, double al, double be, double om) { s->alpha = al; s->beta = be; s->omega = om; }
 
+// ---- the device-side loop of the asynchronous solves (one thread each) ------------------------------------------
+__global__ void loop_begin_kernel(AsyncLoopState *st, int batches, int krr, int nrr)
+{
+    st->count = 0; st->batches = batches; st->krr = krr; st->nrr = nrr;
+}
+
+// end of a WHILE body: run the next batch unless the loop test has failed or max_iter / U batches have run (run_batches' bound)
+__global__ void loop_next_kernel(cudaGraphConditionalHandle loop, const Scalars *sc, AsyncLoopState *st)
+{
+    const int b = ++st->count;
+    cudaGraphSetConditional(loop, (!sc->done && b < st->batches) ? 1u : 0u);
+}
+
+// PIPE_RR: iteration k = bodies run so far is a replacement iteration where solve() schedules one (solver.c:498, 522)
+__global__ void rr_choose_kernel(cudaGraphConditionalHandle replace, cudaGraphConditionalHandle plain, const AsyncLoopState *st)
+{
+    const int k = st->count;
+    const bool rep = (k % st->krr == 0) && k > 0 && k <= st->krr * st->nrr;
+    cudaGraphSetConditional(replace, rep ? 1u : 0u);
+    cudaGraphSetConditional(plain, rep ? 0u : 1u);
+}
+
+// what bicg_solve reports in bicg_stats, with the same IEEE operations as the host (solve(): st.final_res)
+__global__ void result_kernel(const Scalars *sc, bicg_result *out)
+{
+    out->iters = sc->k;
+    out->converged = sc->converged;
+    out->error = sc->error;
+    out->reserved = 0;
+    out->final_res = sqrt(sc->dot_r / sc->dot_zero);
+}
+
 } // namespace
 
-void reset_scalars(bicg_matrix *m, double tol, int max_iter)
+void reset_scalars(bicg_matrix *m, double tol, int max_iter, cudaStream_t st)
 {
-    reset_state_kernel<<<1, 1, 0, ctx().stream>>>(m->d_sc, tol, max_iter);
+    reset_state_kernel<<<1, 1, 0, st>>>(m->d_sc, tol, max_iter);
+}
+void reset_scalars(bicg_matrix *m, double tol, int max_iter) { reset_scalars(m, tol, max_iter, ctx().stream); }
+
+void drop_async_loop(AsyncLoop &L)
+{
+    if (L.exec) cudaGraphExecDestroy(L.exec);
+    if (L.iters) cudaGraphDestroy(L.iters);
+    if (L.rr) cudaGraphDestroy(L.rr);
+    L = AsyncLoop();
+}
+
+void wait_handle(bicg_matrix *m)
+{
+    if (m && m->ev_last) BICG_CUDA(cudaStreamWaitEvent(ctx().stream, m->ev_last, 0));
 }
 
 VecPtrs PhaseLauncher::ptrs() const
@@ -95,11 +141,11 @@ void PhaseLauncher::vec(int phase, TailDesc tail, int push_vec, const double *pu
         return;                                   // single rank: nothing to exchange
     }
     cudaEvent_t e0 = nullptr, e1 = nullptr;
-    if (c.prof_on) { BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1)); BICG_CUDA(cudaEventRecord(e0, c.stream)); }
-    int rc = launch_vec(phase, m->vgrid, a, c.stream);
+    if (c.prof_on) { BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1)); BICG_CUDA(cudaEventRecord(e0, stream)); }
+    int rc = launch_vec(phase, m->vgrid, a, stream);
     if (rc) fatal("bicgstab_b200: vector kernel launch failed (phase %d): %s", phase, cudaGetErrorString((cudaError_t)rc));
     if (c.prof_on) {
-        BICG_CUDA(cudaEventRecord(e1, c.stream));
+        BICG_CUDA(cudaEventRecord(e1, stream));
         c.prof_ev.push_back(e0); c.prof_ev.push_back(e1); c.prof_class.push_back(phase == PH_PUSH ? 2 : 1);
     }
     ++launches; ++c.launches;
@@ -113,7 +159,7 @@ void PhaseLauncher::spmv(int x_id, int y_id, TailDesc tail, int ndot, const doub
     a.shift_sigma = shift_sigma;
     const double *as[4] = {a0, a1, a2, a3}, *bs[4] = {b0, b1, b2, b3};
     for (int k = 0; k < ndot; ++k) epi_add_dot(a.epi, as[k], bs[k]);
-    launch_spmv_plan(m, m->plan, a, 0);
+    launch_spmv_plan(m, m->plan, a, stream, 0);
     ++launches;
 }
 
@@ -185,10 +231,10 @@ struct Seq : PhaseLauncher {
         a.trace = m->d_trace;
         a.snap = m->d_trace ? m->d_trace + (size_t)2 * MEGA_TRACE_ITERS * MEGA_TRACE_SLOTS : nullptr;
         a.snap_iter = 50;
-        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.resident_ctas, 0, sizeof(int), c.stream));
-        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.coded_ctas, 0, sizeof(int), c.stream));
-        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.packed_ctas, 0, sizeof(int), c.stream));
-        int rc = launch_mega(m->mega.threads, m->mega.lanes, m->mega.grid, smem, a, c.stream);
+        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.resident_ctas, 0, sizeof(int), stream));
+        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.coded_ctas, 0, sizeof(int), stream));
+        BICG_CUDA(cudaMemsetAsync(&m->d_msync->st.packed_ctas, 0, sizeof(int), stream));
+        int rc = launch_mega(m->mega.threads, m->mega.lanes, m->mega.grid, smem, a, stream);
         if (rc) {
             // e.g. the grid cannot be co-resident because something else holds SMs.  Single rank: not an error, the
             // kernel-per-phase path below does the same job.  With peers the ranks must agree on the loop
@@ -285,24 +331,133 @@ int kernels_per_iter(int method, int world)
     }
 }
 
-void ensure_graph(bicg_matrix *m, int method, int unroll)
+// `count` iterations of `method`'s loop body (rr: PIPE_RR's replacement iteration instead), captured on the library's stream
+cudaGraph_t capture_iters(bicg_matrix *m, int method, int count, bool rr)
 {
     Context &c = ctx();
-    if (m->graph[method] && m->graph_unroll[method] == unroll) return;
-    if (m->graph[method]) { cudaGraphExecDestroy(m->graph[method]); m->graph[method] = nullptr; }
     cudaGraph_t g = nullptr;
     BICG_CUDA(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
     Seq s(m);
-    for (int u = 0; u < unroll; ++u) {
-        if (method == BICG_METHOD_BICGSTAB) s.bicgstab_iter();
+    for (int u = 0; u < count; ++u) {
+        if (rr) s.rr_replace_iter();
+        else if (method == BICG_METHOD_BICGSTAB) s.bicgstab_iter();
         else if (method == BICG_METHOD_CA) s.ca_iter();
         else s.pipe_iter();
     }
     BICG_CUDA(cudaStreamEndCapture(c.stream, &g));
+    c.launches -= s.launches;       // capture is not execution
+    return g;
+}
+
+void ensure_graph(bicg_matrix *m, int method, int unroll)
+{
+    if (m->graph[method] && m->graph_unroll[method] == unroll) return;
+    if (m->graph[method]) { cudaGraphExecDestroy(m->graph[method]); m->graph[method] = nullptr; }
+    cudaGraph_t g = capture_iters(m, method, unroll, false);
     BICG_CUDA(cudaGraphInstantiate(&m->graph[method], g, 0));
     BICG_CUDA(cudaGraphDestroy(g));
     m->graph_unroll[method] = unroll;
-    c.launches -= s.launches;       // capture is not execution
+}
+
+// a history for max_iter iterations.  Growing it synchronises and allocates, and drops every graph that holds the old pointer
+void ensure_hist(bicg_matrix *m, int max_iter)
+{
+    if (max_iter + 2 <= m->hist_cap) return;
+    Context &c = ctx();
+    // BICG_MAX_ITER was raised after the handle was created: move the history out of the arena and drop the captured graphs
+    // (their kernel arguments hold the old pointer).  Once a caller has captured a solve on this handle the old one stays
+    // allocated until the handle is destroyed, because that graph may still be replayed and write it.
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    if (m->ev_last) BICG_CUDA(cudaEventSynchronize(m->ev_last));
+    if (m->hist_extra && m->captured) m->hist_retired.push_back(m->hist_extra);
+    else if (m->hist_extra) cudaFree(m->hist_extra);
+    BICG_CUDA(cudaMalloc((void **)&m->hist_extra, ((size_t)max_iter + 2) * sizeof(double)));
+    m->d_hist = m->hist_extra; m->hist_cap = max_iter + 2;
+    for (int g = 0; g < 4; ++g) if (m->graph[g]) { cudaGraphExecDestroy(m->graph[g]); m->graph[g] = nullptr; }
+    for (AsyncLoop &L : m->async) drop_async_loop(L);
+}
+
+// iterations per WHILE body: PIPE_RR chooses every iteration's kind on the device, the others run BICG_UNROLL per body
+int async_unroll(int method) { return method == BICG_METHOD_PIPE_RR ? 1 : std::max(1, ctx().cfg.unroll); }
+
+cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args)
+{
+    cudaKernelNodeParams p{};
+    p.func = (void *)fn; p.gridDim = dim3(1); p.blockDim = dim3(1); p.sharedMemBytes = 0; p.kernelParams = args;
+    cudaGraphNode_t n = nullptr;
+    BICG_CUDA(cudaGraphAddKernelNode(&n, g, deps, ndeps, &p));
+    return n;
+}
+
+cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
+                                     cudaGraphConditionalNodeType type, cudaGraph_t *body)
+{
+    cudaGraphNodeParams p{};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = h; p.conditional.type = type; p.conditional.size = 1;
+    cudaGraphNode_t n = nullptr;
+    BICG_CUDA(cudaGraphAddNode(&n, g, deps, ndeps, &p));
+    *body = p.conditional.phGraph_out[0];
+    return n;
+}
+
+// The kernel-per-phase loop as one WHILE node of `g` behind `deps`: its body is the prepared batch of iterations (PIPE_RR:
+// one iteration, its kind chosen by two IF nodes), then loop_next_kernel, which decides on the device whether the body runs again
+cudaGraphNode_t add_device_loop(bicg_matrix *m, int method, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps)
+{
+    const AsyncLoop &L = m->async[method];
+    cudaGraphConditionalHandle loop;
+    BICG_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
+    cudaGraph_t body = nullptr;
+    const cudaGraphNode_t node = add_conditional_node(g, deps, ndeps, loop, cudaGraphCondTypeWhile, &body);
+    cudaGraphNode_t tail[2] = {};
+    size_t ntail = 1;
+    if (method != BICG_METHOD_PIPE_RR) {
+        BICG_CUDA(cudaGraphAddChildGraphNode(&tail[0], body, nullptr, 0, L.iters));
+    } else {
+        cudaGraphConditionalHandle rep, plain;
+        BICG_CUDA(cudaGraphConditionalHandleCreate(&rep, body, 0, 0));
+        BICG_CUDA(cudaGraphConditionalHandleCreate(&plain, body, 0, 0));
+        const AsyncLoopState *st = m->d_loop;
+        void *cargs[3] = {&rep, &plain, (void *)&st};
+        const cudaGraphNode_t choose = add_kernel_node(body, nullptr, 0, (const void *)rr_choose_kernel, cargs);
+        cudaGraph_t b_rep = nullptr, b_plain = nullptr;
+        tail[0] = add_conditional_node(body, &choose, 1, rep, cudaGraphCondTypeIf, &b_rep);
+        tail[1] = add_conditional_node(body, &choose, 1, plain, cudaGraphCondTypeIf, &b_plain);
+        cudaGraphNode_t n;
+        BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_rep, nullptr, 0, L.rr));
+        BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_plain, nullptr, 0, L.iters));
+        ntail = 2;
+    }
+    const Scalars *sc = m->d_sc;
+    AsyncLoopState *st = m->d_loop;
+    void *largs[3] = {&loop, (void *)&sc, (void *)&st};
+    add_kernel_node(body, tail, ntail, (const void *)loop_next_kernel, largs);
+    return node;
+}
+
+bool async_prepared(const bicg_matrix *m, int method)
+{
+    const AsyncLoop &L = m->async[method];
+    return m->ev_last && m->d_loop && L.exec && L.unroll == async_unroll(method) && ctx().cfg.max_iter + 2 <= m->hist_cap;
+}
+
+// the kernel-per-phase loop on `st` without the host: into the caller's capture as a WHILE node, else the prepared graph
+void enqueue_device_loop(bicg_matrix *m, int method, int krr, int nrr, cudaStream_t st)
+{
+    const int U = m->async[method].unroll;
+    loop_begin_kernel<<<1, 1, 0, st>>>(m->d_loop, (ctx().cfg.max_iter + U - 1) / U, krr, nrr);
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t *deps = nullptr;
+    size_t ndeps = 0;
+    BICG_CUDA(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &ndeps));
+    if (cs == cudaStreamCaptureStatusActive) {
+        cudaGraphNode_t node = add_device_loop(m, method, g, deps, ndeps);
+        BICG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+    } else {
+        BICG_CUDA(cudaGraphLaunch(m->async[method].exec, st));
+    }
 }
 
 } // namespace
@@ -320,6 +475,87 @@ void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist
     print_times(t, st.iters);
 }
 
+namespace {
+
+[[noreturn]] void timeout_fatal(const bicg_matrix *m)
+{
+    fatal("bicgstab_b200: rank %d timed out after %d s waiting for a peer GPU / another CTA (halo flag or reduction "
+          "mailbox; BICG_PEER_TIMEOUT_S raises the bound)", m->rank, ctx().cfg.peer_timeout_s);
+}
+
+// The enqueue half of a solve on stream `st`: inputs, scalars, the init phases, the loop, the outputs.  marks: four events
+// recorded before and after the inputs, after the loop and after the outputs (bicg_solve's timing), or null.  device_loop:
+// the kernel-per-phase loop runs as a WHILE node (asynchronous solves); otherwise the host polls it as it always has.
+// Returns whether the persistent kernel ran the loop.
+bool enqueue_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, bool device_vectors, cudaStream_t st,
+                   const cudaEvent_t *marks, bool device_loop)
+{
+    Context &c = ctx();
+    const Config &cfg = c.cfg;
+    const int max_iter = cfg.max_iter;
+    const size_t vbytes = (size_t)m->n_loc * sizeof(double);
+    const cudaMemcpyKind in_kind = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const cudaMemcpyKind out_kind = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+
+    // ---- inputs (outside the reference's timed region, solver.c:61-71) ---------------------------------
+    if (marks) BICG_CUDA(cudaEventRecord(marks[0], st));
+    BICG_CUDA(cudaMemcpyAsync(m->vec(V_X), x, vbytes, in_kind, st));
+    BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, vbytes, in_kind, st));
+    reset_scalars(m, cfg.tol, max_iter, st);
+    if (method != BICG_METHOD_BICGSTAB) {
+        // p, s, z, v, t start at zero: the defined version of the reference's uninitialised reads (SURVEY 5)
+        const int zero_ids[5] = {(int)V_P, (int)V_S, (int)V_Z, (int)V_V, (int)V_T};
+        for (int id : zero_ids)
+            BICG_CUDA(cudaMemsetAsync(m->vec(id), 0, (size_t)m->ghost_off * sizeof(double), st));   // own part only:
+            // the ghost tail belongs to the peers, who may already be pushing into it
+    }
+    if (method == BICG_METHOD_PIPE_RR)
+        BICG_CUDA(cudaMemcpyAsync(m->vec(V_B), m->vec(V_R), vbytes, cudaMemcpyDeviceToDevice, st));   // solver.c:475
+    if (marks) BICG_CUDA(cudaEventRecord(marks[1], st));
+
+    // ---- the reference's timed region a14 (solver.c:69-132) ------------------------------------------------
+    Seq seq(m, st);
+    if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_init();
+    else seq.capipe_init(method != BICG_METHOD_CA);
+
+    bool use_mega = cfg.mega && m->mega.ok && !c.prof_on;
+    if (use_mega) use_mega = seq.mega(method, krr, nrr);
+    if (!use_mega && device_loop) {
+        enqueue_device_loop(m, method, krr, nrr, st);
+    } else if (!use_mega) {
+        const bool use_graph = cfg.graph && !c.prof_on && method != BICG_METHOD_PIPE_RR;   // replacement iterations are host-scheduled
+        const int U = std::max(1, cfg.unroll);
+        if (use_graph) ensure_graph(m, method, U);
+        run_batches(max_iter, U, 3, &m->d_sc->done, [&](int b) {
+            if (use_graph) {
+                BICG_CUDA(cudaGraphLaunch(m->graph[method], c.stream));
+                c.launches += U * kernels_per_iter(method, m->world);
+                return;
+            }
+            for (int u = 0; u < U; ++u) {
+                const int k = b * U + u;
+                if (k >= max_iter) break;
+                if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_iter();
+                else if (method == BICG_METHOD_CA) seq.ca_iter();
+                else if (method == BICG_METHOD_PIPE) seq.pipe_iter();
+                else {
+                    const bool replace = (k % krr == 0) && k > 0 && k <= krr * nrr;       // solver.c:498, 522
+                    if (replace) seq.rr_replace_iter(); else seq.pipe_iter();
+                }
+            }
+        });
+    }
+    if (marks) BICG_CUDA(cudaEventRecord(marks[2], st));
+
+    // ---- outputs ---------------------------------------------------------------------------------------
+    BICG_CUDA(cudaMemcpyAsync(x, m->vec(V_X), vbytes, out_kind, st));
+    BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), vbytes, out_kind, st));
+    if (marks) BICG_CUDA(cudaEventRecord(marks[3], st));
+    return use_mega;
+}
+
+} // namespace
+
 int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *out)
 {
     Context &c = ctx();
@@ -327,81 +563,21 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     if (method < 0 || method > 3) return -1;
     if (method == BICG_METHOD_PIPE_RR && krr <= 0) method = BICG_METHOD_PIPE;
     const Config &cfg = c.cfg;
-    const int max_iter = cfg.max_iter;
-    if (max_iter + 2 > m->hist_cap) {
-        // BICG_MAX_ITER was raised after the handle was created: move the history out of the arena and
-        // drop the captured graphs (their kernel arguments hold the old pointer)
-        BICG_CUDA(cudaStreamSynchronize(c.stream));
-        if (m->hist_extra) cudaFree(m->hist_extra);
-        BICG_CUDA(cudaMalloc((void **)&m->hist_extra, ((size_t)max_iter + 2) * sizeof(double)));
-        m->d_hist = m->hist_extra; m->hist_cap = max_iter + 2;
-        for (int g = 0; g < 4; ++g) if (m->graph[g]) { cudaGraphExecDestroy(m->graph[g]); m->graph[g] = nullptr; }
-    }
+    ensure_hist(m, cfg.max_iter);
+    wait_handle(m);
     const size_t vbytes = (size_t)m->n_loc * sizeof(double);
-    const cudaMemcpyKind in_kind = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
-    const cudaMemcpyKind out_kind = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
 
-    cudaEvent_t e_in0, e_in1, e_loop1, e_out1;
-    BICG_CUDA(cudaEventCreate(&e_in0)); BICG_CUDA(cudaEventCreate(&e_in1));
-    BICG_CUDA(cudaEventCreate(&e_loop1)); BICG_CUDA(cudaEventCreate(&e_out1));
-
-    // ---- inputs (outside the reference's timed region, solver.c:61-71) ---------------------------------
-    BICG_CUDA(cudaEventRecord(e_in0, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(m->vec(V_X), x, vbytes, in_kind, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(m->vec(V_R), r, vbytes, in_kind, c.stream));
-    reset_scalars(m, cfg.tol, max_iter);
-    if (method != BICG_METHOD_BICGSTAB) {
-        // p, s, z, v, t start at zero: the defined version of the reference's uninitialised reads (SURVEY 5)
-        const int zero_ids[5] = {(int)V_P, (int)V_S, (int)V_Z, (int)V_V, (int)V_T};
-        for (int id : zero_ids)
-            BICG_CUDA(cudaMemsetAsync(m->vec(id), 0, (size_t)m->ghost_off * sizeof(double), c.stream));   // own part only:
-            // the ghost tail belongs to the peers, who may already be pushing into it
-    }
-    if (method == BICG_METHOD_PIPE_RR)
-        BICG_CUDA(cudaMemcpyAsync(m->vec(V_B), m->vec(V_R), vbytes, cudaMemcpyDeviceToDevice, c.stream));   // solver.c:475
-    BICG_CUDA(cudaEventRecord(e_in1, c.stream));
-
-    // ---- the reference's timed region a14 (solver.c:69-132) ------------------------------------------------
+    cudaEvent_t ev[4];     // before / after the inputs, after the loop, after the outputs
+    for (cudaEvent_t &e : ev) BICG_CUDA(cudaEventCreate(&e));
     const int launches0 = c.launches;
-    Seq seq(m);
-    if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_init();
-    else seq.capipe_init(method != BICG_METHOD_CA);
+    const bool use_mega = enqueue_solve(m, method, x, r, krr, nrr, device_vectors != 0, c.stream, ev, false);
 
-    bool use_mega = cfg.mega && m->mega.ok && !c.prof_on;
-    if (use_mega) use_mega = seq.mega(method, krr, nrr);
-    const bool use_graph = cfg.graph && !c.prof_on && method != BICG_METHOD_PIPE_RR;   // replacement iterations are host-scheduled
-    const int U = std::max(1, cfg.unroll);
-    if (use_graph && !use_mega) ensure_graph(m, method, U);
-    if (!use_mega) run_batches(max_iter, U, 3, &m->d_sc->done, [&](int b) {
-        if (use_graph) {
-            BICG_CUDA(cudaGraphLaunch(m->graph[method], c.stream));
-            c.launches += U * kernels_per_iter(method, m->world);
-            return;
-        }
-        for (int u = 0; u < U; ++u) {
-            const int k = b * U + u;
-            if (k >= max_iter) break;
-            if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_iter();
-            else if (method == BICG_METHOD_CA) seq.ca_iter();
-            else if (method == BICG_METHOD_PIPE) seq.pipe_iter();
-            else {
-                const bool replace = (k % krr == 0) && k > 0 && k <= krr * nrr;       // solver.c:498, 522
-                if (replace) seq.rr_replace_iter(); else seq.pipe_iter();
-            }
-        }
-    });
-    BICG_CUDA(cudaEventRecord(e_loop1, c.stream));
-
-    // ---- outputs ---------------------------------------------------------------------------------------
-    BICG_CUDA(cudaMemcpyAsync(x, m->vec(V_X), vbytes, out_kind, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(r, m->vec(V_R), vbytes, out_kind, c.stream));
-    BICG_CUDA(cudaEventRecord(e_out1, c.stream));
+    // ---- finish: statistics, trace, history --------------------------------------------------------------
     Scalars hs;
     BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
 
-    if (hs.error) fatal("bicgstab_b200: rank %d timed out after %d s waiting for a peer GPU / another CTA (halo flag or reduction "
-                        "mailbox; BICG_PEER_TIMEOUT_S raises the bound)", m->rank, cfg.peer_timeout_s);
+    if (hs.error) timeout_fatal(m);
     if (m->d_trace && use_mega && method == BICG_METHOD_BICGSTAB) {
         // BICG_MEGA_TRACE=1: where CTA 0 and the middle CTA of the persistent kernel spent their time, averaged over the iterations
         const int iters = std::min(hs.k - 1, (int)MEGA_TRACE_ITERS);
@@ -459,14 +635,14 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     st.converged = hs.converged;
     st.final_res = sqrt(hs.dot_r / hs.dot_zero);
     float ms = 0.f;
-    BICG_CUDA(cudaEventElapsedTime(&ms, e_in1, e_loop1)); st.loop_ms = ms;
-    BICG_CUDA(cudaEventElapsedTime(&ms, e_in0, e_in1));   st.h2d_ms = ms;
-    BICG_CUDA(cudaEventElapsedTime(&ms, e_loop1, e_out1)); st.d2h_ms = ms;
+    BICG_CUDA(cudaEventElapsedTime(&ms, ev[1], ev[2])); st.loop_ms = ms;
+    BICG_CUDA(cudaEventElapsedTime(&ms, ev[0], ev[1])); st.h2d_ms = ms;
+    BICG_CUDA(cudaEventElapsedTime(&ms, ev[2], ev[3])); st.d2h_ms = ms;
     st.h2d_bytes = device_vectors ? 0 : 2 * vbytes;
     st.d2h_bytes = device_vectors ? 0 : 2 * vbytes;
     st.kernel_launches = c.launches - launches0;
     st.spmv_lanes = m->plan.lanes; st.spmv_kind = m->plan.kind;
-    cudaEventDestroy(e_in0); cudaEventDestroy(e_in1); cudaEventDestroy(e_loop1); cudaEventDestroy(e_out1);
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
 
     c.last_hist.assign((size_t)st.iters + 1, 0.0);
     BICG_CUDA(cudaMemcpy(c.last_hist.data(), m->d_hist, ((size_t)st.iters + 1) * sizeof(double), cudaMemcpyDeviceToHost));
@@ -475,11 +651,80 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     return st.iters;
 }
 
+int solve_async_prepare(bicg_matrix *m, int method)
+{
+    Context &c = ctx();
+    c.ensure();
+    if (!m || method < 0 || method > 3) return -1;
+    ensure_hist(m, c.cfg.max_iter);
+    if (!m->ev_last) {
+        // the handle's first asynchronous use: matrix_create returns with the upload and the plan's encoding kernels still in
+        // flight on the library's stream, and a synchronous call may have left work there too, so the handle's last work
+        // starts out as everything enqueued on that stream so far
+        BICG_CUDA(cudaEventCreateWithFlags(&m->ev_last, cudaEventDisableTiming));
+        BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
+    }
+    if (!m->d_loop) m->d_loop = (AsyncLoopState *)c.dev_alloc(sizeof(AsyncLoopState));
+    if (method == BICG_METHOD_PIPE_RR) solve_async_prepare(m, BICG_METHOD_PIPE);   // what PIPE_RR with krr <= 0 runs
+    AsyncLoop &L = m->async[method];
+    const int U = async_unroll(method);
+    if (L.exec && L.unroll == U) return 0;
+    drop_async_loop(L);
+    L.iters = capture_iters(m, method, U, false);
+    if (method == BICG_METHOD_PIPE_RR) L.rr = capture_iters(m, method, 1, true);
+    L.unroll = U;
+    cudaGraph_t g = nullptr;
+    BICG_CUDA(cudaGraphCreate(&g, 0));
+    add_device_loop(m, method, g, nullptr, 0);
+    BICG_CUDA(cudaGraphInstantiate(&L.exec, g, 0));
+    BICG_CUDA(cudaGraphDestroy(g));
+    return 0;
+}
+
+int solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, cudaStream_t st, bicg_result *result)
+{
+    Context &c = ctx();
+    c.ensure();
+    if (!m || !x || !r || method < 0 || method > 3) return -1;
+    if (method == BICG_METHOD_PIPE_RR && krr <= 0) method = BICG_METHOD_PIPE;
+    cudaStreamCaptureStatus cs;
+    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
+    const bool captured = cs != cudaStreamCaptureStatusNone;
+    if (!captured) solve_async_prepare(m, method);
+    else if (!async_prepared(m, method)) return -2;
+    // the handle's device state is shared by every call on it; inside a capture the wait and the record become nodes that
+    // order the replays behind the handle's last work at replay time
+    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    if (captured) m->captured = true;
+    enqueue_solve(m, method, x, r, krr, nrr, true, st, nullptr, true);
+    if (result) result_kernel<<<1, 1, 0, st>>>(m->d_sc, result);
+    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    return 0;
+}
+
+int matrix_history(bicg_matrix *m, double *out, int cap)
+{
+    Context &c = ctx();
+    c.ensure();
+    wait_handle(m);
+    Scalars hs;
+    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    if (hs.error) timeout_fatal(m);
+    const int n = hs.k + 1;
+    if (out && cap > 0) {
+        BICG_CUDA(cudaMemcpyAsync(out, m->d_hist, (size_t)std::min(n, cap) * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    return n;
+}
+
 // y_loc = A x_loc with host pointers (the kernel behind MPI_csr_spmv_ovlap, matrix.c:428-441)
 int spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full)
 {
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     const size_t vbytes = (size_t)m->n_loc * sizeof(double);
     BICG_CUDA(cudaMemcpyAsync(m->vec(V_X), x_loc, vbytes, cudaMemcpyHostToDevice, c.stream));
     reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
@@ -515,6 +760,7 @@ int spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
 {
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     reset_scalars(m, c.cfg.tol, c.cfg.max_iter);
     fill_kernel<<<256, 256, 0, c.stream>>>(m->vec(V_P), (int)m->vstride, 1.0);
     fill_kernel<<<256, 256, 0, c.stream>>>(m->vec(V_RH), m->n_loc, 1.0);
@@ -524,9 +770,9 @@ int spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
     a.kc.tail = tail_pend(1, 0);               // full in-kernel reduction of the dot, no peer traffic
     cudaEvent_t e0, e1;
     BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
-    for (int i = 0; i < 3; ++i) launch_spmv_plan(m, m->plan, a);
+    for (int i = 0; i < 3; ++i) launch_spmv_plan(m, m->plan, a, c.stream);
     BICG_CUDA(cudaEventRecord(e0, c.stream));
-    for (int i = 0; i < reps; ++i) launch_spmv_plan(m, m->plan, a);
+    for (int i = 0; i < reps; ++i) launch_spmv_plan(m, m->plan, a, c.stream);
     BICG_CUDA(cudaEventRecord(e1, c.stream));
     BICG_CUDA(cudaEventSynchronize(e1));
     float ms = 0.f;
@@ -548,6 +794,7 @@ extern "C" int bicg_debug_vec_phase(bicg_matrix *m, int phase, const double coef
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     if (m->world != 1 || phase < 0 || phase >= PH_PUSH) return -1;
     const size_t vb = (size_t)m->n_loc * sizeof(double);
     for (int id = 0; id < V_COUNT; ++id)
@@ -577,6 +824,7 @@ extern "C" int bicg_debug_spmv_epi(bicg_matrix *m, int epi, double *vecs, double
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     if (m->world != 1 || epi < 0 || epi > 3) return -1;
     const size_t vb = (size_t)m->n_loc * sizeof(double);
     for (int id = 0; id < V_COUNT; ++id)
@@ -605,6 +853,7 @@ extern "C" int bicg_debug_get_vec(bicg_matrix *m, int id, double *out)
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     if (id < 0 || id >= V_COUNT) return -1;
     BICG_CUDA(cudaMemcpyAsync(out, m->vec(id), (size_t)m->n_loc * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
@@ -615,6 +864,7 @@ extern "C" int bicg_debug_get_scalars(bicg_matrix *m, double out[13])
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     Scalars hs;
     BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
@@ -628,6 +878,7 @@ extern "C" int bicg_debug_resident_ctas(bicg_matrix *m)
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     int n = 0;
     BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.resident_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
@@ -639,6 +890,7 @@ extern "C" int bicg_debug_coded_ctas(bicg_matrix *m)
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     int n = 0;
     BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.coded_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
@@ -657,6 +909,7 @@ extern "C" int bicg_debug_packed_ctas(bicg_matrix *m)
     using namespace bicg;
     Context &c = ctx();
     c.ensure();
+    wait_handle(m);
     int n = 0;
     BICG_CUDA(cudaMemcpyAsync(&n, &m->d_msync->st.packed_ctas, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
