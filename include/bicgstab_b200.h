@@ -250,6 +250,51 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
 int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
                            bicg_stats *stats);
 
+/* Written by the device at the end of an asynchronous shifted solve, in stream order (32 bytes): ret is what
+ * bicg_shifted_solve_dev returns for the same solve (switching: iterations + 1), iters / converged / final_res are its
+ * bicg_stats fields, seed the seed the solve ended with (bicg_last_shift_info's seed), and error = 1 if a bounded wait for a
+ * peer GPU or another CTA timed out (BICG_PEER_TIMEOUT_S). */
+typedef struct {
+    int    ret;
+    int    iters;
+    int    converged;
+    int    seed;
+    int    error;
+    int    reserved;
+    double final_res;
+} bicg_shift_result;
+
+/* bicg_shifted_solve_dev enqueued on the caller's CUDA stream `stream` (a cudaStream_t; 0 is CUDA's default stream).  x_set
+ * (sigma_len blocks of n_loc doubles, any 8-byte alignment), r (b in, seed residual out) and sigma (sigma_len doubles) are all
+ * DEVICE pointers, read and written in stream order: a replay of a captured solve picks up new values in the same buffers.
+ * `result` (a bicg_shift_result) and `stop_iter` (sigma_len ints: what bicg_last_shift_info reports for the same solve) are
+ * optional device memory.  x_set, r, stop_iter and the result are bit-identical to bicg_shifted_solve_dev's.  Returns 0 once the
+ * work is enqueued, with no host synchronisation, allocation, pageable copy or output; -1 for a null pointer, an unknown
+ * method, sigma_len <= 0 or a seed outside [0, sigma_len); -2 inside a stream capture when the handle has not been prepared
+ * for this method and sigma_len under the current BICG_SHIFT_MAX_ITER (the capture stays valid).  BICG_SHIFT_TOL and
+ * BICG_SHIFT_MAX_ITER are read at enqueue time; a captured solve keeps the values it was captured with.
+ *
+ * x_set, r and sigma are staged through buffers on the handle: copied in at the start and x_set, r copied back at the end
+ * (device to device), so the call holds no pointer of the caller beyond its own enqueue.  Ordering is that of
+ * bicg_solve_async: calls on one handle, synchronous or asynchronous, plain or shifted, run in the order they were made.
+ * Not updated by asynchronous shifted solves: bicg_last_stats, bicg_last_history, bicg_last_shift_info and
+ * bicg_last_shift_error; nothing is printed (not the seed-switch report either), and the BICG_SHIFT_ERROR check does not run
+ * (call bicg_shift_residuals after synchronising).  With several ranks the call is collective like bicg_shifted_solve_dev.
+ *
+ * bicg_shifted_solve_async_prepare builds, outside any capture, the handle's workspace of the method's family (switching and
+ * fixed seed; LOP and PIPE-LOP) for sigma_len and the current BICG_SHIFT_MAX_ITER, and the graphs of its device-side loop.  It
+ * may synchronise and allocate; an uncaptured bicg_shifted_solve_async calls it itself.  Collective: every rank returns -1 if
+ * any rank passed a null handle, an unknown method or sigma_len <= 0, or the ranks disagree on method or sigma_len; else 0.
+ * A workspace outgrown by a new sigma_len or a larger BICG_SHIFT_MAX_ITER is replaced; after a capture on the handle the old
+ * one stays allocated until the handle is destroyed, because the captured graph still uses it.
+ *
+ * bicg_matrix_shift_history waits for the handle's last work and copies the seed history of the last asynchronous shifted
+ * solve on m, the entries bicg_last_history returns after the synchronous solve; returns their number (0 if there was none). */
+int bicg_shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                             void *stream, bicg_shift_result *result, int *stop_iter);
+int bicg_shifted_solve_async_prepare(bicg_matrix *m, int method, int sigma_len);
+int bicg_matrix_shift_history(bicg_matrix *m, double *out, int cap);
+
 /* out[j] = ||(A + sigma_j I) x_j - b|| / ||b||, j < sigma_len; x_set: sigma_len blocks of n_loc doubles, b: n_loc doubles, both
  * host pointers, or device pointers when device_vectors != 0.  Collective over the ranks, which pass the same sigma_len: every rank
  * returns -1 when any rank passed sigma_len <= 0 or a null pointer, or the ranks' sigma_len differ.  Any sigma_len > 0 works.

@@ -36,6 +36,12 @@ class bicg_result(C.Structure):
                 ("final_res", C.c_double)]
 
 
+class bicg_shift_result(C.Structure):
+    """What an asynchronous shifted solve writes to device memory at its end (32 bytes)."""
+    _fields_ = [("ret", C.c_int), ("iters", C.c_int), ("converged", C.c_int), ("seed", C.c_int), ("error", C.c_int),
+                ("reserved", C.c_int), ("final_res", C.c_double)]
+
+
 ALLGATHER_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t)
 
 # every symbol include/bicgstab_b200.h declares: (restype, argtypes)
@@ -82,6 +88,10 @@ SYMBOLS = {
     "bicg_last_shift_info": (C.c_int, [_P(C.c_int), _P(C.c_int), C.c_int]),
     "bicg_shifted_solve_ex": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_shifted_solve_dev": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(bicg_stats)]),
+    "bicg_shifted_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]),
+    "bicg_shifted_solve_async_prepare": (C.c_int, [C.c_void_p, C.c_int, C.c_int]),
+    "bicg_matrix_shift_history": (C.c_int, [C.c_void_p, _P(C.c_double), C.c_int]),
     "bicg_shift_residuals": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, _P(C.c_double)]),
     "bicg_last_shift_error": (C.c_int, [_P(C.c_double), C.c_int]),
     "bicg_spmv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -13,7 +13,7 @@ import ctypes as C
 
 import numpy as np
 
-from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_result, bicg_stats, lib
+from ._lib import ALLGATHER_FN, CSR_Matrix, INFO_Matrix, bicg_result, bicg_shift_result, bicg_stats, lib
 
 METHODS = {"bicgstab": 0, "ca_bicgstab": 1, "pipe_bicgstab": 2, "pipe_bicgstab_rr": 3}
 SHIFTED_METHODS = {"shifted_lopbicg_switching": 0, "shifted_lopbicgstab": 1, "shifted_pipe_lopbicgstab": 2}
@@ -337,17 +337,39 @@ def last_history():
     return out[:n]
 
 
+def _decode_record(t, stream, rec):
+    if stream is not None:
+        stream.synchronize()
+    raw = bytes(t.detach().cpu().numpy().tobytes()) if hasattr(t, "detach") else bytes(np.asarray(t, dtype=np.uint8))
+    if len(raw) != C.sizeof(rec):
+        raise ValueError(f"a {rec.__name__} has {C.sizeof(rec)} bytes, got {len(raw)}")
+    r = rec.from_buffer_copy(raw)
+    return {f: getattr(r, f) for f, _ in rec._fields_ if f != "reserved"}
+
+
 def decode_result(t, stream=None):
     """The bicg_result an asynchronous solve wrote into the 24-byte tensor `t`, as a dict with iters, converged, error and
     final_res.  The copy to the host is ordered after torch's current stream only: pass the stream the solve was enqueued on
     when it was another one, and it is synchronised first (or synchronise it yourself)."""
-    if stream is not None:
-        stream.synchronize()
-    raw = bytes(t.detach().cpu().numpy().tobytes()) if hasattr(t, "detach") else bytes(np.asarray(t, dtype=np.uint8))
-    if len(raw) != C.sizeof(bicg_result):
-        raise ValueError(f"a bicg_result has {C.sizeof(bicg_result)} bytes, got {len(raw)}")
-    r = bicg_result.from_buffer_copy(raw)
-    return {f: getattr(r, f) for f, _ in bicg_result._fields_ if f != "reserved"}
+    return _decode_record(t, stream, bicg_result)
+
+
+def decode_shift_result(t, stream=None):
+    """The bicg_shift_result an asynchronous shifted solve wrote into the 32-byte tensor `t`, as a dict with ret, iters,
+    converged, seed, error and final_res; `stream` as in decode_result."""
+    return _decode_record(t, stream, bicg_shift_result)
+
+
+def _result_tensor(result, nbytes, device, stream):
+    """`result` checked, or a new one of nbytes that is written on `stream`"""
+    import torch
+    if result is None:
+        result = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        result.record_stream(stream)          # written on `stream`, which need not be the one it was allocated on
+    elif not (isinstance(result, torch.Tensor) and result.is_cuda and result.dtype == torch.uint8 and result.is_contiguous()
+              and result.numel() == nbytes and result.device == device and result.data_ptr() % 8 == 0):
+        raise ValueError(f"result: need a contiguous, 8-byte aligned uint8 CUDA tensor of {nbytes} elements on {device}")
+    return result
 
 
 def _stats_dict(s):
@@ -388,15 +410,9 @@ class DeviceMatrix:
         import torch
         n = self.blk.n_loc
         xp, rp = _checked_cuda_vectors(("x", x, (n,)), ("r", r, (n,)))
-        nbytes = C.sizeof(bicg_result)
         if stream is None:
             stream = torch.cuda.current_stream(x.device)
-        if result is None:
-            result = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
-            result.record_stream(stream)          # written on `stream`, which need not be the one it was allocated on
-        elif not (isinstance(result, torch.Tensor) and result.is_cuda and result.dtype == torch.uint8 and result.is_contiguous()
-                  and result.numel() == nbytes and result.device == x.device and result.data_ptr() % 8 == 0):
-            raise ValueError(f"result: need a contiguous, 8-byte aligned uint8 CUDA tensor of {nbytes} elements on {x.device}")
+        result = _result_tensor(result, C.sizeof(bicg_result), x.device, stream)
         rc = lib.bicg_solve_async(self.h, METHODS[method], xp, rp, int(krr), int(nrr), C.c_void_p(stream.cuda_stream),
                                   C.c_void_p(result.data_ptr()))
         if rc == -2:
@@ -434,6 +450,55 @@ class DeviceMatrix:
             fn = lib.bicg_shifted_solve_dev
         k = fn(self.h, SHIFTED_SOLVE_EX[method], xp, rp, _dptr(sigma), int(sigma.size), int(seed), C.byref(st))
         return k, _stats_dict(st)
+
+    def shifted_solve_async(self, method, x_set, r, sigma, seed, result=None, stop_iter=None, stream=None):
+        """bicg_shifted_solve_async: the solve of shifted_solve on CUDA tensors, enqueued on `stream` (default: torch's current
+        stream) without waiting for it.  x_set (sigma_len, n_loc; a view at any element offset works), r (n_loc,) and sigma
+        (sigma_len,) are contiguous CUDA float64 tensors, read and written in stream order.  `result`: a 32-byte uint8 CUDA tensor
+        that receives the bicg_shift_result (decode_shift_result reads it), allocated when not given; `stop_iter`: an optional
+        int32 CUDA tensor of sigma_len that receives what last_shift_info reports for the same solve.  Works inside
+        torch.cuda.graph once prepare_shifted_async(method, sigma_len) has been called.  Returns the result tensor."""
+        import torch
+        n = self.blk.n_loc
+        if not isinstance(sigma, torch.Tensor):
+            raise TypeError(f"sigma: need a CUDA float64 tensor, got {type(sigma).__name__}")
+        if sigma.dim() != 1:
+            raise ValueError(f"sigma: need a 1-d tensor, got shape {tuple(sigma.shape)}")
+        L = int(sigma.numel())
+        if isinstance(seed, bool) or not isinstance(seed, (int, np.integer)) or not 0 <= int(seed) < L:
+            raise ValueError(f"seed: need an integer in [0, {L}), got {seed!r}")
+        xp, rp, sp_ = _checked_cuda_vectors(("x_set", x_set, (L, n)), ("r", r, (n,)), ("sigma", sigma, (L,)))
+        if stop_iter is not None and not (isinstance(stop_iter, torch.Tensor) and stop_iter.is_cuda and stop_iter.dtype == torch.int32
+                                          and stop_iter.is_contiguous() and tuple(stop_iter.shape) == (L,)
+                                          and stop_iter.device == x_set.device):
+            raise ValueError(f"stop_iter: need a contiguous int32 CUDA tensor of shape ({L},) on {x_set.device}")
+        if stream is None:
+            stream = torch.cuda.current_stream(x_set.device)
+        result = _result_tensor(result, C.sizeof(bicg_shift_result), x_set.device, stream)
+        if stop_iter is not None:
+            stop_iter.record_stream(stream)
+        rc = lib.bicg_shifted_solve_async(self.h, SHIFTED_SOLVE_EX[method], xp, rp, sp_, L, int(seed), C.c_void_p(stream.cuda_stream),
+                                          C.c_void_p(result.data_ptr()),
+                                          C.c_void_p(stop_iter.data_ptr()) if stop_iter is not None else None)
+        if rc == -2:
+            raise RuntimeError(f"shifted_solve_async inside a stream capture needs prepare_shifted_async({method!r}, {L}) first")
+        if rc != 0:
+            raise ValueError(f"bicg_shifted_solve_async failed with {rc}")
+        return result
+
+    def prepare_shifted_async(self, method, sigma_len):
+        """bicg_shifted_solve_async_prepare: build what shifted_solve_async needs for `method` and sigma_len under the current
+        options, outside any capture.  Collective over the ranks."""
+        if lib.bicg_shifted_solve_async_prepare(self.h, SHIFTED_SOLVE_EX[method], int(sigma_len)) != 0:
+            raise ValueError(f"bicg_shifted_solve_async_prepare({method}, {sigma_len}) failed")
+
+    def shift_history(self):
+        """bicg_matrix_shift_history: the seed history of the last asynchronous shifted solve on this handle (waits for it), the
+        entries last_history returns after the synchronous solve; empty if there was none."""
+        n = lib.bicg_matrix_shift_history(self.h, None, 0)
+        out = np.empty(max(n, 1))
+        n = lib.bicg_matrix_shift_history(self.h, out.ctypes.data_as(C.POINTER(C.c_double)), n)
+        return out[:n]
 
     def shift_residuals(self, x_set, b, sigma):
         """bicg_shift_residuals: ||(A + sigma_j I) x_j - b|| / ||b|| for every row x_j of x_set (sigma_len, n_loc), computed on

@@ -18,6 +18,10 @@ static_assert(offsetof(INFO_Matrix, code) == 12 && offsetof(INFO_Matrix, recvcou
 static_assert(sizeof(bicg_result) == 24 && offsetof(bicg_result, iters) == 0 && offsetof(bicg_result, converged) == 4 &&
               offsetof(bicg_result, error) == 8 && offsetof(bicg_result, reserved) == 12 &&
               offsetof(bicg_result, final_res) == 16, "bicg_result layout of include/bicgstab_b200.h");
+static_assert(sizeof(bicg_shift_result) == 32 && offsetof(bicg_shift_result, ret) == 0 && offsetof(bicg_shift_result, iters) == 4 &&
+              offsetof(bicg_shift_result, converged) == 8 && offsetof(bicg_shift_result, seed) == 12 &&
+              offsetof(bicg_shift_result, error) == 16 && offsetof(bicg_shift_result, reserved) == 20 &&
+              offsetof(bicg_shift_result, final_res) == 24, "bicg_shift_result layout of include/bicgstab_b200.h");
 
 namespace {
 
@@ -251,6 +255,13 @@ int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r,
     if (stats) *stats = c.last_stats;
     return k;
 }
+int bicg_shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                             void *stream, bicg_shift_result *result, int *stop_iter)
+{
+    return shifted_solve_async(m, method, x_set, r, sigma, sigma_len, seed, (cudaStream_t)stream, result, stop_iter);
+}
+int bicg_shifted_solve_async_prepare(bicg_matrix *m, int method, int sigma_len) { return shifted_async_prepare(m, method, sigma_len); }
+int bicg_matrix_shift_history(bicg_matrix *m, double *out, int cap) { return matrix_shift_history(m, out, cap); }
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap)
 {
     Context &c = ctx();

@@ -172,6 +172,23 @@ struct AsyncLoop {
     int unroll = 0;
 };
 
+// What an asynchronous shifted solve of one family (shifted.cu, shifted_lop.cu) keeps on a handle: every device buffer of
+// the solve for sigma_len = L and BICG_SHIFT_MAX_ITER up to cap, its state template, and per variant of the family the
+// captured batch of ShiftedSolve::U iterations and the executable graph of one WHILE node around it.
+struct ShiftWork {
+    int L = 0, cap = 0;
+    std::vector<void *> mem;             // every buffer below and the family's arrays (Context::dev_alloc)
+    void *d_state = nullptr;             // ShiftDev / LopDev
+    void *d_tmpl = nullptr;              // the same with its pointers and L set, copied into d_state at every solve's start
+    std::vector<unsigned char> tmpl;     // host copy of *d_tmpl (the buffers the enqueue stages sigma into and clears)
+    double *d_x = nullptr;               // [L][stride] the caller's x_set, staged
+    double *d_p = nullptr;               // [L][stride] p_j
+    cudaGraph_t iters[2] = {};
+    cudaGraphExec_t exec[2] = {};
+};
+// where the last asynchronous shifted solve on a handle left its history (device memory, written by its result kernel)
+struct ShiftHistRef { const double *hist; int n, pad; };
+
 } // namespace bicg
 
 // the opaque handle of the C ABI
@@ -238,6 +255,11 @@ struct bicg_matrix {
     bicg::AsyncLoop async[4];
     bool captured = false;                // a caller has captured a solve on this handle into a graph
     std::vector<double *> hist_retired;   // histories replaced while such a graph may still write them
+    // asynchronous shifted solves (bicg_shifted_solve_async): one workspace per family (0: switching / fixed seed, 1: LOP),
+    // buffers of workspaces replaced while a captured graph may still use them, and the history of the last such solve
+    bicg::ShiftWork shift_ws[2];
+    std::vector<void *> shift_retired;
+    bicg::ShiftHistRef *d_shift_last = nullptr;
 
     double *vec(int id) const { return vec_base + (long long)id * vstride; }
 };
@@ -259,6 +281,26 @@ int  matrix_history(bicg_matrix *m, double *out, int cap);
 // asynchronous work (free when there is none)
 void wait_handle(bicg_matrix *m);
 void drop_async_loop(AsyncLoop &L);        // frees what bicg_solve_async_prepare built for one method
+// The device-side loop of the asynchronous solves, shared by solve.cu and the shifted solvers.  async_handle_init: the
+// handle's first asynchronous use (its last-work event, recorded on the library's stream, and the loop state).
+void async_handle_init(bicg_matrix *m);
+cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args);
+cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
+                                     cudaGraphConditionalNodeType type, cudaGraph_t *body);
+// A WHILE node of g behind deps: `fill` adds the body's work to `body` and returns its last nodes (at most 2) in `tail`; then
+// loop_next_kernel runs the body again unless *done is set or m->d_loop's bound of bodies has run
+cudaGraphNode_t add_while_node(bicg_matrix *m, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const int *done,
+                               const std::function<size_t(cudaGraph_t body, cudaGraphNode_t *tail)> &fill);
+// the loop on `st` without the host: loop_begin_kernel (`batches` bodies at most), then the node `add` builds into the caller's
+// capture, or else the prepared executable graph `exec` of that node
+void enqueue_while(bicg_matrix *m, cudaStream_t st, int batches, int krr, int nrr, cudaGraphExec_t exec,
+                   const std::function<cudaGraphNode_t(cudaGraph_t, const cudaGraphNode_t *, size_t)> &add);
+// bicg_shifted_solve_async / _prepare / bicg_matrix_shift_history (shifted.cu)
+int  shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                         cudaStream_t st, bicg_shift_result *result, int *stop_iter);
+int  shifted_async_prepare(bicg_matrix *m, int method, int sigma_len);
+int  matrix_shift_history(bicg_matrix *m, double *out, int cap);
+void drop_shift_work(bicg_matrix *m);      // matrix_destroy: every workspace, its graphs and the retired buffers
 int  spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full_or_null);
 int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);

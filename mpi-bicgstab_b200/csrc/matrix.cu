@@ -918,6 +918,7 @@ void matrix_destroy(bicg_matrix *m)
     for (AsyncLoop &L : m->async) drop_async_loop(L);
     c.dev_free(m->d_loop);
     for (double *h : m->hist_retired) cudaFree(h);
+    drop_shift_work(m);
     // world > 1: nothing collective here.  The arena is parked, not freed (the peers keep their mappings), and a rank
     // that has finished its solve has received everything its peers will ever write into this arena: the last
     // reduction completes only after every rank's last push and post (DESIGN.md 4).

@@ -324,9 +324,9 @@ struct ShRun : PhaseLauncher {
     }
     void prologue()
     {
-        sh_vec_init<<<m->vgrid, 256, 0, c.stream>>>(vargs(tail_store(1)));          // :342-354
+        sh_vec_init<<<m->vgrid, 256, 0, stream>>>(vargs(tail_store(1)));            // :342-354
         check_launch("sh_vec_init");
-        sh_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc);
+        sh_scalar_init<<<1, 256, 0, stream>>>(d_sd, m->d_sc);
         check_launch("sh_scalar_init");
         vec(PH_PUSH, tail_none(), V_P);
         c.launches += 2;
@@ -336,40 +336,62 @@ struct ShRun : PhaseLauncher {
         const int G = m->vgrid;
         const double *Y = nullptr;
         spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), Y);                            // s = (A + sigma I) p, (r#,s)   :377-387
-        sh_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
+        sh_scalar_alpha<<<1, 1, 0, stream>>>(d_sd, m->d_sc);
         check_launch("sh_scalar_alpha");
-        sh_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // q, r_old, q_copy            :374, 391-392
+        sh_vec_q<<<G, 256, 0, stream>>>(vargs(tail_none()));                          // q, r_old, q_copy            :374, 391-392
         check_launch("sh_vec_q");
         vec(PH_PUSH, tail_none(), V_R);
         spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), Y);   // y = (A + sigma I) q, (q,q), (q,y)  :395-406
-        sh_scalar_omega<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);
+        sh_scalar_omega<<<1, 1, 0, stream>>>(d_sd, m->d_sc);
         check_launch("sh_scalar_omega");
-        sh_vec_xr<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));                     // x[seed], r, (r,r), (r#,r)   :411-416
+        sh_vec_xr<<<G, 256, 0, stream>>>(vargs(tail_store(2)));                       // x[seed], r, (r,r), (r#,r)   :411-416
         check_launch("sh_vec_xr");
-        sh_scalar_iter<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                       // beta ... loop test          :420, 429-537
+        sh_scalar_iter<<<1, 512, 0, stream>>>(d_sd, m->d_sc);                         // beta ... loop test          :420, 429-537
         check_launch("sh_scalar_iter");
-        sh_vec_shift<<<ugrid, 256, (size_t)base.chunk * SH_ENTRY, c.stream>>>(vargs(tail_none()));   // x_j, p_j   :435-445
+        sh_vec_shift<<<ugrid, 256, (size_t)base.chunk * SH_ENTRY, stream>>>(vargs(tail_none()));     // x_j, p_j   :435-445
         check_launch("sh_vec_shift");
-        sh_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                        // p[seed] (or the switch)     :421-423 / :499
+        sh_vec_p<<<G, 256, 0, stream>>>(vargs(tail_none()));                          // p[seed] (or the switch)     :421-423 / :499
         check_launch("sh_vec_p");
         vec(PH_PUSH, tail_none(), V_P);
         c.launches += 7;
     }
 };
 
-} // namespace
-
-int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
-                    int max_iter_opt, bool dev)
+// The state of a new solve: the template (pointers, L) and the solve's own settings.  Every other field starts at zero, as the
+// host struct it replaces did; sh_scalar_init sets the rest.
+__global__ void sh_begin_kernel(ShiftDev *sd, const ShiftDev *tmpl, int fixed, int seed, double tol, int max_iter)
 {
-    ShiftedSolve s(m, L, dev);
-    Context &c = s.c;
-    const int n = s.n;
-    const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
+    *sd = *tmpl;
+    sd->fixed = fixed; sd->seed = seed; sd->tol = tol; sd->max_iter = max_iter;
+}
 
-    // ---- device state -------------------------------------------------------------------------------------------------
+// what switching_solve reports (its return value, bicg_stats, bicg_last_shift_info), with the same IEEE operations
+__global__ void sh_result_kernel(const ShiftDev *sd, const Scalars *sc, bicg_shift_result *out, int *stop_iter, ShiftHistRef *last)
+{
+    const int k = sd->k;
+    if (threadIdx.x == 0) {
+        last->hist = sd->hist; last->n = max(k, 1);
+        if (out) {
+            out->ret = sd->fixed ? k - 1 : k;
+            out->iters = k - 1;
+            out->converged = sd->stop_count >= sd->L;
+            out->seed = sd->seed;
+            out->error = sc->error;
+            out->reserved = 0;
+            out->final_res = sqrt(sd->dot_r / sd->dot_zero);
+        }
+    }
+    if (stop_iter)
+        for (int j = threadIdx.x; j < sd->L; j += blockDim.x) stop_iter[j] = sd->stop_iter[j];
+}
+
+// every device buffer of a solve with s.L shifts and max_iter (= SHIFT_MAX_ITER + 1) iterations, as the template of its state;
+// p_set in *d_p
+ShiftDev sh_buffers(ShiftedSolve &s, int max_iter, double **d_p)
+{
+    const int L = s.L;
     ShiftDev h{};
-    h.L = L; h.max_iter = max_iter; h.fixed = fixed ? 1 : 0; h.tol = tol; h.seed = seed;
+    h.L = L;
     h.sigma = s.alloc<double>(L);
     h.alpha_set = s.alloc<double>(L); h.beta_set = s.alloc<double>(L);
     h.omega_set = s.alloc<double>(L); h.eta_set = s.alloc<double>(L);
@@ -383,26 +405,55 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
     h.ev_k = s.alloc<int>(SH_EVENTS); h.ev_seed = s.alloc<int>(SH_EVENTS);
     h.ev_remain = s.alloc<int>(SH_EVENTS);
     h.ev_vals = s.alloc<double>((size_t)SH_EVENTS * L * 3);
-    ShiftDev *d_sd = s.alloc<ShiftDev>(1);
-    double *d_p = s.alloc<double>((size_t)L * s.stride);
-    BICG_CUDA(cudaMemcpyAsync(d_sd, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(h.sigma, sigma, L * sizeof(double), cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemsetAsync(h.pi_arch, 0, (size_t)L * max_iter * sizeof(double), c.stream));
-    BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), c.stream));
-    s.upload(x_set, r);
+    *d_p = s.alloc<double>((size_t)L * s.stride);
+    return h;
+}
 
-    ShRun run(m);
+// the launcher of a solve on s's stream with state d_sd and p_set d_p
+ShRun sh_run(ShiftedSolve &s, ShiftDev *d_sd, double *d_p)
+{
+    bicg_matrix *m = s.m;
+    ShRun run(m, s.st);
     run.d_sd = d_sd;
     run.shift_sigma = &d_sd->sigma_seed;
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);
     run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
-    run.base.n = n; run.base.L = L;
+    run.base.n = s.n; run.base.L = s.L;
     run.ugrid = s.update_grid();
-    run.base.chunk = std::min(L, table_chunk(sh_vec_shift, SH_ENTRY));
+    run.base.chunk = std::min(s.L, table_chunk(sh_vec_shift, SH_ENTRY));
+    return run;
+}
 
-    s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :364
+// The enqueue half of every switching / fixed-seed solve on s.st, synchronous or asynchronous: the state from the template
+// d_tmpl (host copy h), the inputs, the reference's timed region (:364).  The outputs are s.finish / s.finish_async.
+void sh_enqueue(ShiftedSolve &s, ShiftDev *d_sd, const ShiftDev *d_tmpl, const ShiftDev &h, double *d_p, double *x_set, double *r,
+                const double *sigma, bool fixed, int seed, double tol, int max_iter)
+{
+    BICG_CUDA(cudaMemsetAsync(h.pi_arch, 0, (size_t)s.L * max_iter * sizeof(double), s.st));
+    BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), s.st));
+    s.upload(x_set, r, sigma, h.sigma);
+    sh_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, d_tmpl, fixed ? 1 : 0, seed, tol, max_iter);
+    check_launch("sh_begin_kernel");
+    ShRun run = sh_run(s, d_sd, d_p);
+    s.run(run, max_iter, &d_sd->done, 0);
+}
+
+} // namespace
+
+int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
+                    int max_iter_opt, bool dev)
+{
+    ShiftedSolve s(m, L, dev);
+    Context &c = s.c;
+    const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
+
+    double *d_p = nullptr;
+    const ShiftDev h = sh_buffers(s, max_iter, &d_p);
+    ShiftDev *d_sd = s.alloc<ShiftDev>(2);                                            // the state, its template
+    BICG_CUDA(cudaMemcpyAsync(d_sd + 1, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
+    sh_enqueue(s, d_sd, d_sd + 1, h, d_p, x_set, r, sigma, fixed, seed, tol, max_iter);
     const ShiftDev out = s.finish(x_set, r, d_sd);
 
     // ---- results ------------------------------------------------------------------------------------------------------
@@ -455,6 +506,164 @@ int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const do
     case BICG_SHIFTED_PIPE_LOP:  return lop_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);
     default: return -1;
     }
+}
+
+void switching_prepare(bicg_matrix *m, ShiftWork &ws, int L)
+{
+    Context &c = ctx();
+    ShiftedSolve s(m, L, ws, c.stream);
+    ShiftDev *d_sd = nullptr;
+    if (ws.mem.empty()) {
+        ws.L = L; ws.cap = c.cfg.shift_max_iter;
+        ws.d_x = s.d_x = s.alloc<double>((size_t)L * s.stride);
+        const ShiftDev h = sh_buffers(s, ws.cap + 1, &ws.d_p);
+        d_sd = s.alloc<ShiftDev>(2);
+        ws.d_state = d_sd; ws.d_tmpl = d_sd + 1;
+        ws.tmpl.assign((const unsigned char *)&h, (const unsigned char *)&h + sizeof(ShiftDev));
+        BICG_CUDA(cudaMemcpyAsync(ws.d_tmpl, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
+    }
+    d_sd = (ShiftDev *)ws.d_state;
+    if (!ws.exec[0]) {                              // the body is the same for both methods: `fixed` is a device flag
+        ShRun run = sh_run(s, d_sd, ws.d_p);
+        s.capture_loop(run, &d_sd->done, 0);
+    }
+}
+
+void switching_solve_async(bicg_matrix *m, ShiftWork &ws, bool fixed, double *x_set, double *r, const double *sigma, int seed,
+                           double tol, int max_iter_opt, cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+{
+    ShiftedSolve s(m, ws.L, ws, st);
+    ShiftDev h;
+    memcpy(&h, ws.tmpl.data(), sizeof(ShiftDev));
+    ShiftDev *d_sd = (ShiftDev *)ws.d_state;
+    sh_enqueue(s, d_sd, (const ShiftDev *)ws.d_tmpl, h, ws.d_p, x_set, r, sigma, fixed, seed, tol, max_iter_opt + 1);
+    s.finish_async(x_set, r);
+    sh_result_kernel<<<1, 256, 0, st>>>(d_sd, m->d_sc, result, stop_iter, m->d_shift_last);
+    check_launch("sh_result_kernel");
+}
+
+namespace {
+
+// the workspace of a method's family (0: switching and fixed seed, 1: LOP and PIPE-LOP) and its variant of the captured loop
+int shift_family(int method) { return method == BICG_SHIFTED_LOP || method == BICG_SHIFTED_PIPE_LOP ? 1 : 0; }
+int shift_variant(int method) { return method == BICG_SHIFTED_PIPE_LOP ? 1 : 0; }
+
+bool shift_method_known(int method)
+{
+    return method == BICG_SHIFTED_SWITCHING || method == BICG_SHIFTED_LOP || method == BICG_SHIFTED_PIPE_LOP ||
+           method == BICG_SHIFTED_LOPBICG;
+}
+
+bool shift_async_prepared(const bicg_matrix *m, int method, int L)
+{
+    const ShiftWork &ws = m->shift_ws[shift_family(method)];
+    return m->ev_last && m->d_loop && m->d_shift_last && ws.L == L && ws.cap >= ctx().cfg.shift_max_iter &&
+           ws.exec[shift_variant(method)];
+}
+
+// frees a workspace's graphs; its buffers go back to the pool, or are kept until the handle is destroyed (retire: a captured
+// graph may still use them)
+void drop_work(bicg_matrix *m, ShiftWork &ws, bool retire)
+{
+    Context &c = ctx();
+    for (int v = 0; v < 2; ++v) {
+        if (ws.exec[v]) cudaGraphExecDestroy(ws.exec[v]);
+        if (ws.iters[v]) cudaGraphDestroy(ws.iters[v]);
+    }
+    for (void *p : ws.mem) {
+        if (retire) m->shift_retired.push_back(p);
+        else c.dev_free(p);
+    }
+    ws = ShiftWork();
+}
+
+} // namespace
+
+int shifted_async_prepare(bicg_matrix *m, int method, int L)
+{
+    Context &c = ctx();
+    // collective, as bicg_shifted_solve_dev: every rank learns every rank's verdict, method and sigma_len
+    struct Args { int bad, method, len; } mine{!m || !shift_method_known(method) || L <= 0, method, L};
+    std::vector<Args> all((size_t)c.world);
+    c.host_allgather(&mine, all.data(), sizeof(Args));
+    for (const Args &a : all)
+        if (a.bad || a.method != method || a.len != L) return -1;
+    c.ensure();
+    async_handle_init(m);
+    ShiftWork &ws = m->shift_ws[shift_family(method)];
+    if (!ws.mem.empty() && (ws.L != L || ws.cap < c.cfg.shift_max_iter)) {
+        // outgrown: nothing may still run on the old buffers when they return to the pool
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+        BICG_CUDA(cudaEventSynchronize(m->ev_last));
+        drop_work(m, ws, m->captured);
+    }
+    // what this enqueues on the library's stream (the history record's and the template's initial values) goes behind the
+    // handle's last work and ahead of the next call on it
+    wait_handle(m);
+    if (!m->d_shift_last) {
+        m->d_shift_last = (ShiftHistRef *)c.dev_alloc(sizeof(ShiftHistRef));
+        BICG_CUDA(cudaMemsetAsync(m->d_shift_last, 0, sizeof(ShiftHistRef), c.stream));
+    }
+    if (shift_family(method) == 0) switching_prepare(m, ws, L);
+    else lop_prepare(m, ws, L, method == BICG_SHIFTED_PIPE_LOP);
+    BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
+    return 0;
+}
+
+int shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed,
+                        cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+{
+    Context &c = ctx();
+    c.ensure();
+    if (!m || !x_set || !r || !sigma || !shift_method_known(method) || L <= 0 || seed < 0 || seed >= L) return -1;
+    cudaStreamCaptureStatus cs;
+    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
+    const bool captured = cs != cudaStreamCaptureStatusNone;
+    if (!shift_async_prepared(m, method, L)) {
+        if (captured) return -2;
+        if (shifted_async_prepare(m, method, L) != 0) return -1;
+    }
+    // the order of the plain asynchronous solve (solve_async): behind the handle's last work, which this call then is
+    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    if (captured) m->captured = true;
+    ShiftWork &ws = m->shift_ws[shift_family(method)];
+    const double tol = c.cfg.shift_tol;
+    const int max_iter = c.cfg.shift_max_iter;
+    switch (method) {
+    case BICG_SHIFTED_SWITCHING: switching_solve_async(m, ws, false, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
+    case BICG_SHIFTED_LOPBICG:   switching_solve_async(m, ws, true, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
+    case BICG_SHIFTED_LOP:       lop_solve_async(m, ws, false, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
+    default:                     lop_solve_async(m, ws, true, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
+    }
+    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    return 0;
+}
+
+int matrix_shift_history(bicg_matrix *m, double *out, int cap)
+{
+    Context &c = ctx();
+    c.ensure();
+    if (!m) return -1;
+    if (!m->d_shift_last) return 0;
+    wait_handle(m);
+    ShiftHistRef ref{};
+    BICG_CUDA(cudaMemcpyAsync(&ref, m->d_shift_last, sizeof(ShiftHistRef), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    if (out && cap > 0 && ref.n > 0) {
+        BICG_CUDA(cudaMemcpyAsync(out, ref.hist, (size_t)std::min(ref.n, cap) * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    return ref.n;
+}
+
+void drop_shift_work(bicg_matrix *m)
+{
+    Context &c = ctx();
+    for (ShiftWork &ws : m->shift_ws) drop_work(m, ws, false);
+    for (void *p : m->shift_retired) c.dev_free(p);
+    m->shift_retired.clear();
+    if (m->d_shift_last) c.dev_free(m->d_shift_last);
+    m->d_shift_last = nullptr;
 }
 
 } // namespace bicg

@@ -20,6 +20,7 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
 
 namespace bicg {
 
@@ -298,15 +299,15 @@ struct LopRun : PhaseLauncher {
     void prologue()
     {
         const int G = m->vgrid;
-        lop_vec_init<<<G, 256, 0, c.stream>>>(vargs(tail_store(1)), pipe ? 1 : 0);
+        lop_vec_init<<<G, 256, 0, stream>>>(vargs(tail_store(1)), pipe ? 1 : 0);
         check_launch("lop_vec_init");
-        lop_scalar_init<<<1, 256, 0, c.stream>>>(d_sd, m->d_sc, pipe ? 1 : 0);
+        lop_scalar_init<<<1, 256, 0, stream>>>(d_sd, m->d_sc, pipe ? 1 : 0);
         check_launch("lop_scalar_init");
         c.launches += 2;
         if (!pipe) { vec(PH_PUSH, tail_none(), V_P); return; }
         vec(PH_PUSH, tail_none(), V_R);
         spmv(V_R, V_W, tail_store(1), 1, m->vec(V_R), nullptr);                         // w = (A + sigma I) r, (r,w)  :765-767
-        lop_scalar_pipe_init<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                       :787
+        lop_scalar_pipe_init<<<1, 1, 0, stream>>>(d_sd, m->d_sc);                      // alpha                       :787
         check_launch("lop_scalar_pipe_init");
         vec(PH_PUSH, tail_none(), V_W);
         spmv(V_W, V_T, tail_none());                                                   // t = (A + sigma I) w          :769-770
@@ -318,66 +319,89 @@ struct LopRun : PhaseLauncher {
         const size_t smem = (size_t)base.chunk * LOP_COEF * sizeof(double);
         if (!pipe) {
             spmv(V_P, V_S, tail_store(1), 1, m->vec(V_RH), nullptr);                    // s = (A + sigma I) p, (r#,s)   :261-263
-            lop_scalar_alpha<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc);                    // alpha                        :276
+            lop_scalar_alpha<<<1, 1, 0, stream>>>(d_sd, m->d_sc);                      // alpha                        :276
             check_launch("lop_scalar_alpha");
-            lop_vec_q<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // r_old, q                     :271, 277
+            lop_vec_q<<<G, 256, 0, stream>>>(vargs(tail_none()));                      // r_old, q                     :271, 277
             check_launch("lop_vec_q");
             vec(PH_PUSH, tail_none(), V_R);
             spmv(V_R, V_Y, tail_store(2), 2, m->vec(V_R), m->vec(V_R), m->vec(V_R), nullptr);   // y = (A + sigma I) q, (q,q), (q,y)  :278-282
-            lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            lop_scalar_shift<<<1, 512, 0, stream>>>(d_sd, m->d_sc);                    // omega, every shift's scalars
             check_launch("lop_scalar_shift");
-            lop_vec_update<false><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(2)));
+            lop_vec_update<false><<<ugrid, 256, smem, stream>>>(vargs(tail_store(2)));
             check_launch("lop_vec_update");
-            lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 0);                   // beta, loop test              :312-318
+            lop_scalar_end<<<1, 1, 0, stream>>>(d_sd, m->d_sc, 0);                     // beta, loop test              :312-318
             check_launch("lop_scalar_end");
-            lop_vec_p<<<G, 256, 0, c.stream>>>(vargs(tail_none()));                    // p[seed]                      :319-321
+            lop_vec_p<<<G, 256, 0, stream>>>(vargs(tail_none()));                      // p[seed]                      :319-321
             check_launch("lop_vec_p");
             vec(PH_PUSH, tail_none(), V_P);
             c.launches += 6;
         } else {
-            lop_vec_pipe1<<<G, 256, 0, c.stream>>>(vargs(tail_store(2)));              // p, s, z, q, y, (q,y), (y,y)   :795-814
+            lop_vec_pipe1<<<G, 256, 0, stream>>>(vargs(tail_store(2)));                // p, s, z, q, y, (q,y), (y,y)   :795-814
             check_launch("lop_vec_pipe1");
             vec(PH_PUSH, tail_none(), V_Z);
             spmv(V_Z, V_V, tail_none());                                               // v = (A + sigma I) z           :815-816
-            lop_scalar_shift<<<1, 512, 0, c.stream>>>(d_sd, m->d_sc);                  // omega, every shift's scalars
+            lop_scalar_shift<<<1, 512, 0, stream>>>(d_sd, m->d_sc);                    // omega, every shift's scalars
             check_launch("lop_scalar_shift");
-            lop_vec_update<true><<<ugrid, 256, smem, c.stream>>>(vargs(tail_store(5)));
+            lop_vec_update<true><<<ugrid, 256, smem, stream>>>(vargs(tail_store(5)));
             check_launch("lop_vec_update");
             vec(PH_PUSH, tail_none(), V_W);
             spmv(V_W, V_T, tail_none());                                               // t = (A + sigma I) w           :850-851
-            lop_scalar_end<<<1, 1, 0, c.stream>>>(d_sd, m->d_sc, 1);                   // beta, alpha, loop test       :857-865
+            lop_scalar_end<<<1, 1, 0, stream>>>(d_sd, m->d_sc, 1);                     // beta, alpha, loop test       :857-865
             check_launch("lop_scalar_end");
             c.launches += 4;
         }
     }
 };
 
-} // namespace
-
-int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
-              bool dev)
+// The state of a new solve: the template (pointers, L) and the solve's own settings, sigma_seed from the staged sigma (read by the
+// SpMV epilogue from the first kernel on).  Every other field starts at zero; lop_scalar_init sets the rest.
+__global__ void lop_begin_kernel(LopDev *sd, const LopDev *tmpl, int seed, double tol, int max_iter)
 {
-    ShiftedSolve s(m, L, dev);
-    Context &c = s.c;
-    const int n = s.n;
+    *sd = *tmpl;
+    sd->seed = seed; sd->tol = tol; sd->max_iter = max_iter;
+    sd->sigma_seed = sd->sigma[seed];
+}
 
-    // ---- device state -------------------------------------------------------------------------------------------------
+// what lop_solve reports (its return value, bicg_stats, bicg_last_shift_info), with the same IEEE operations
+__global__ void lop_result_kernel(const LopDev *sd, const Scalars *sc, bicg_shift_result *out, int *stop_iter, ShiftHistRef *last)
+{
+    const int k = sd->k;
+    if (threadIdx.x == 0) {
+        last->hist = sd->hist; last->n = k + 1;
+        if (out) {
+            out->ret = k;
+            out->iters = k;
+            out->converged = sd->max_zeta_pi * sd->max_zeta_pi * sd->dot_r <= sd->tol * sd->tol * sd->dot_zero;
+            out->seed = sd->seed;
+            out->error = sc->error;
+            out->reserved = 0;
+            out->final_res = sqrt(sd->dot_r / sd->dot_zero);
+        }
+    }
+    if (stop_iter)                                      // no shift stops on its own
+        for (int j = threadIdx.x; j < sd->L; j += blockDim.x) stop_iter[j] = 0;
+}
+
+// every device buffer of a solve with s.L shifts and max_iter iterations, as the template of its state; p_set in *d_p
+LopDev lop_buffers(ShiftedSolve &s, int max_iter, double **d_p)
+{
+    const int L = s.L;
     LopDev h{};
-    h.L = L; h.max_iter = max_iter; h.tol = tol; h.seed = seed; h.sigma_seed = sigma[seed];
+    h.L = L;
     h.sigma = s.alloc<double>(L);
     h.eta = s.alloc<double>(L); h.zeta = s.alloc<double>(L);
     h.pi_old = s.alloc<double>(L); h.pi_new = s.alloc<double>(L);
     h.coef = s.alloc<double>((size_t)(L - 1) * LOP_COEF);
     h.hist = s.alloc<double>((size_t)max_iter + 1);
-    LopDev *d_sd = s.alloc<LopDev>(1);
-    double *d_p = s.alloc<double>((size_t)L * s.stride);
-    BICG_CUDA(cudaMemcpyAsync(d_sd, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemcpyAsync(h.sigma, sigma, L * sizeof(double), cudaMemcpyHostToDevice, c.stream));
-    BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), c.stream));
-    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)L * s.stride * sizeof(double), c.stream));        // p_loc_set = calloc(...)  :226
-    s.upload(x_set, r);
+    *d_p = s.alloc<double>((size_t)L * s.stride);
+    return h;
+}
 
-    LopRun run(m);
+// the launcher of a solve on s's stream with state d_sd and p_set d_p
+LopRun lop_run(ShiftedSolve &s, bool pipe, LopDev *d_sd, double *d_p)
+{
+    bicg_matrix *m = s.m;
+    LopRun run(m, s.st);
     run.pipe = pipe;
     run.d_sd = d_sd;
     run.shift_sigma = &d_sd->sigma_seed;
@@ -386,12 +410,40 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     run.base.y = m->vec(V_Y); run.base.z = m->vec(V_Z); run.base.w = m->vec(V_W); run.base.v = m->vec(V_V); run.base.t = m->vec(V_T);
     run.base.rold = m->vec(pipe ? V_AX : V_V);
     run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
-    run.base.n = n; run.base.L = L;
+    run.base.n = s.n; run.base.L = s.L;
     run.ugrid = s.update_grid();
     constexpr size_t entry = LOP_COEF * sizeof(double);
-    run.base.chunk = std::min(L - 1, pipe ? table_chunk(lop_vec_update<true>, entry) : table_chunk(lop_vec_update<false>, entry));
+    run.base.chunk = std::min(s.L - 1, pipe ? table_chunk(lop_vec_update<true>, entry) : table_chunk(lop_vec_update<false>, entry));
+    return run;
+}
 
-    s.run(run, max_iter, &d_sd->done);                                                // the reference's timed region :237 / :759
+// The enqueue half of every LOP / PIPE-LOP solve on s.st, synchronous or asynchronous: the state from the template d_tmpl
+// (host copy h), the inputs, the reference's timed region (:237 / :759).  The outputs are s.finish / s.finish_async.
+void lop_enqueue(ShiftedSolve &s, bool pipe, LopDev *d_sd, const LopDev *d_tmpl, const LopDev &h, double *d_p, double *x_set,
+                 double *r, const double *sigma, int seed, double tol, int max_iter)
+{
+    BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), s.st));
+    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)s.L * s.stride * sizeof(double), s.st));        // p_loc_set = calloc(...)  :226
+    s.upload(x_set, r, sigma, h.sigma);
+    lop_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, d_tmpl, seed, tol, max_iter);
+    check_launch("lop_begin_kernel");
+    LopRun run = lop_run(s, pipe, d_sd, d_p);
+    s.run(run, max_iter, &d_sd->done, pipe ? 1 : 0);
+}
+
+} // namespace
+
+int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
+              bool dev)
+{
+    ShiftedSolve s(m, L, dev);
+    Context &c = s.c;
+
+    double *d_p = nullptr;
+    const LopDev h = lop_buffers(s, max_iter, &d_p);
+    LopDev *d_sd = s.alloc<LopDev>(2);                                                // the state, its template
+    BICG_CUDA(cudaMemcpyAsync(d_sd + 1, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
+    lop_enqueue(s, pipe, d_sd, d_sd + 1, h, d_p, x_set, r, sigma, seed, tol, max_iter);
     const LopDev out = s.finish(x_set, r, d_sd);
 
     // ---- results ------------------------------------------------------------------------------------------------------
@@ -414,6 +466,40 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     }
     s.report_error(sigma, seed);
     return k;                                                                         // :352 / :894
+}
+
+void lop_prepare(bicg_matrix *m, ShiftWork &ws, int L, bool pipe)
+{
+    Context &c = ctx();
+    ShiftedSolve s(m, L, ws, c.stream);
+    if (ws.mem.empty()) {
+        ws.L = L; ws.cap = c.cfg.shift_max_iter;
+        ws.d_x = s.d_x = s.alloc<double>((size_t)L * s.stride);
+        const LopDev h = lop_buffers(s, ws.cap, &ws.d_p);
+        LopDev *d_sd = s.alloc<LopDev>(2);
+        ws.d_state = d_sd; ws.d_tmpl = d_sd + 1;
+        ws.tmpl.assign((const unsigned char *)&h, (const unsigned char *)&h + sizeof(LopDev));
+        BICG_CUDA(cudaMemcpyAsync(ws.d_tmpl, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
+    }
+    const int v = pipe ? 1 : 0;
+    if (!ws.exec[v]) {
+        LopDev *d_sd = (LopDev *)ws.d_state;
+        LopRun run = lop_run(s, pipe, d_sd, ws.d_p);
+        s.capture_loop(run, &d_sd->done, v);
+    }
+}
+
+void lop_solve_async(bicg_matrix *m, ShiftWork &ws, bool pipe, double *x_set, double *r, const double *sigma, int seed, double tol,
+                     int max_iter, cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+{
+    ShiftedSolve s(m, ws.L, ws, st);
+    LopDev h;
+    memcpy(&h, ws.tmpl.data(), sizeof(LopDev));
+    LopDev *d_sd = (LopDev *)ws.d_state;
+    lop_enqueue(s, pipe, d_sd, (const LopDev *)ws.d_tmpl, h, ws.d_p, x_set, r, sigma, seed, tol, max_iter);
+    s.finish_async(x_set, r);
+    lop_result_kernel<<<1, 256, 0, st>>>(d_sd, m->d_sc, result, stop_iter, m->d_shift_last);
+    check_launch("lop_result_kernel");
 }
 
 } // namespace bicg

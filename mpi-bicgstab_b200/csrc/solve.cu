@@ -47,11 +47,12 @@ __global__ void loop_begin_kernel(AsyncLoopState *st, int batches, int krr, int 
     st->count = 0; st->batches = batches; st->krr = krr; st->nrr = nrr;
 }
 
-// end of a WHILE body: run the next batch unless the loop test has failed or max_iter / U batches have run (run_batches' bound)
-__global__ void loop_next_kernel(cudaGraphConditionalHandle loop, const Scalars *sc, AsyncLoopState *st)
+// end of a WHILE body: run the next batch unless the loop test has failed (*done: Scalars::done, or a shifted solver's own)
+// or max_iter / U batches have run (run_batches' bound)
+__global__ void loop_next_kernel(cudaGraphConditionalHandle loop, const int *done, AsyncLoopState *st)
 {
     const int b = ++st->count;
-    cudaGraphSetConditional(loop, (!sc->done && b < st->batches) ? 1u : 0u);
+    cudaGraphSetConditional(loop, (!*done && b < st->batches) ? 1u : 0u);
 }
 
 // PIPE_RR: iteration k = bodies run so far is a replacement iteration where solve() schedules one (solver.c:498, 522)
@@ -92,6 +93,72 @@ void drop_async_loop(AsyncLoop &L)
 void wait_handle(bicg_matrix *m)
 {
     if (m && m->ev_last) BICG_CUDA(cudaStreamWaitEvent(ctx().stream, m->ev_last, 0));
+}
+
+void async_handle_init(bicg_matrix *m)
+{
+    Context &c = ctx();
+    if (!m->ev_last) {
+        // the handle's first asynchronous use: matrix_create returns with the upload and the plan's encoding kernels still in
+        // flight on the library's stream, and a synchronous call may have left work there too, so the handle's last work
+        // starts out as everything enqueued on that stream so far
+        BICG_CUDA(cudaEventCreateWithFlags(&m->ev_last, cudaEventDisableTiming));
+        BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
+    }
+    if (!m->d_loop) m->d_loop = (AsyncLoopState *)c.dev_alloc(sizeof(AsyncLoopState));
+}
+
+cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args)
+{
+    cudaKernelNodeParams p{};
+    p.func = (void *)fn; p.gridDim = dim3(1); p.blockDim = dim3(1); p.sharedMemBytes = 0; p.kernelParams = args;
+    cudaGraphNode_t n = nullptr;
+    BICG_CUDA(cudaGraphAddKernelNode(&n, g, deps, ndeps, &p));
+    return n;
+}
+
+cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
+                                     cudaGraphConditionalNodeType type, cudaGraph_t *body)
+{
+    cudaGraphNodeParams p{};
+    p.type = cudaGraphNodeTypeConditional;
+    p.conditional.handle = h; p.conditional.type = type; p.conditional.size = 1;
+    cudaGraphNode_t n = nullptr;
+    BICG_CUDA(cudaGraphAddNode(&n, g, deps, ndeps, &p));
+    *body = p.conditional.phGraph_out[0];
+    return n;
+}
+
+cudaGraphNode_t add_while_node(bicg_matrix *m, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const int *done,
+                               const std::function<size_t(cudaGraph_t body, cudaGraphNode_t *tail)> &fill)
+{
+    cudaGraphConditionalHandle loop;
+    BICG_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
+    cudaGraph_t body = nullptr;
+    const cudaGraphNode_t node = add_conditional_node(g, deps, ndeps, loop, cudaGraphCondTypeWhile, &body);
+    cudaGraphNode_t tail[2] = {};
+    const size_t ntail = fill(body, tail);
+    AsyncLoopState *st = m->d_loop;
+    void *largs[3] = {&loop, (void *)&done, (void *)&st};
+    add_kernel_node(body, tail, ntail, (const void *)loop_next_kernel, largs);
+    return node;
+}
+
+void enqueue_while(bicg_matrix *m, cudaStream_t st, int batches, int krr, int nrr, cudaGraphExec_t exec,
+                   const std::function<cudaGraphNode_t(cudaGraph_t, const cudaGraphNode_t *, size_t)> &add)
+{
+    loop_begin_kernel<<<1, 1, 0, st>>>(m->d_loop, batches, krr, nrr);
+    cudaStreamCaptureStatus cs;
+    cudaGraph_t g = nullptr;
+    const cudaGraphNode_t *deps = nullptr;
+    size_t ndeps = 0;
+    BICG_CUDA(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &ndeps));
+    if (cs == cudaStreamCaptureStatusActive) {
+        cudaGraphNode_t node = add(g, deps, ndeps);
+        BICG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+    } else {
+        BICG_CUDA(cudaGraphLaunch(exec, st));
+    }
 }
 
 VecPtrs PhaseLauncher::ptrs() const
@@ -380,41 +447,16 @@ void ensure_hist(bicg_matrix *m, int max_iter)
 // iterations per WHILE body: PIPE_RR chooses every iteration's kind on the device, the others run BICG_UNROLL per body
 int async_unroll(int method) { return method == BICG_METHOD_PIPE_RR ? 1 : std::max(1, ctx().cfg.unroll); }
 
-cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args)
-{
-    cudaKernelNodeParams p{};
-    p.func = (void *)fn; p.gridDim = dim3(1); p.blockDim = dim3(1); p.sharedMemBytes = 0; p.kernelParams = args;
-    cudaGraphNode_t n = nullptr;
-    BICG_CUDA(cudaGraphAddKernelNode(&n, g, deps, ndeps, &p));
-    return n;
-}
-
-cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
-                                     cudaGraphConditionalNodeType type, cudaGraph_t *body)
-{
-    cudaGraphNodeParams p{};
-    p.type = cudaGraphNodeTypeConditional;
-    p.conditional.handle = h; p.conditional.type = type; p.conditional.size = 1;
-    cudaGraphNode_t n = nullptr;
-    BICG_CUDA(cudaGraphAddNode(&n, g, deps, ndeps, &p));
-    *body = p.conditional.phGraph_out[0];
-    return n;
-}
-
 // The kernel-per-phase loop as one WHILE node of `g` behind `deps`: its body is the prepared batch of iterations (PIPE_RR:
 // one iteration, its kind chosen by two IF nodes), then loop_next_kernel, which decides on the device whether the body runs again
 cudaGraphNode_t add_device_loop(bicg_matrix *m, int method, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps)
 {
     const AsyncLoop &L = m->async[method];
-    cudaGraphConditionalHandle loop;
-    BICG_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
-    cudaGraph_t body = nullptr;
-    const cudaGraphNode_t node = add_conditional_node(g, deps, ndeps, loop, cudaGraphCondTypeWhile, &body);
-    cudaGraphNode_t tail[2] = {};
-    size_t ntail = 1;
-    if (method != BICG_METHOD_PIPE_RR) {
-        BICG_CUDA(cudaGraphAddChildGraphNode(&tail[0], body, nullptr, 0, L.iters));
-    } else {
+    return add_while_node(m, g, deps, ndeps, &m->d_sc->done, [&](cudaGraph_t body, cudaGraphNode_t *tail) -> size_t {
+        if (method != BICG_METHOD_PIPE_RR) {
+            BICG_CUDA(cudaGraphAddChildGraphNode(&tail[0], body, nullptr, 0, L.iters));
+            return 1;
+        }
         cudaGraphConditionalHandle rep, plain;
         BICG_CUDA(cudaGraphConditionalHandleCreate(&rep, body, 0, 0));
         BICG_CUDA(cudaGraphConditionalHandleCreate(&plain, body, 0, 0));
@@ -427,13 +469,8 @@ cudaGraphNode_t add_device_loop(bicg_matrix *m, int method, cudaGraph_t g, const
         cudaGraphNode_t n;
         BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_rep, nullptr, 0, L.rr));
         BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_plain, nullptr, 0, L.iters));
-        ntail = 2;
-    }
-    const Scalars *sc = m->d_sc;
-    AsyncLoopState *st = m->d_loop;
-    void *largs[3] = {&loop, (void *)&sc, (void *)&st};
-    add_kernel_node(body, tail, ntail, (const void *)loop_next_kernel, largs);
-    return node;
+        return 2;
+    });
 }
 
 bool async_prepared(const bicg_matrix *m, int method)
@@ -446,18 +483,8 @@ bool async_prepared(const bicg_matrix *m, int method)
 void enqueue_device_loop(bicg_matrix *m, int method, int krr, int nrr, cudaStream_t st)
 {
     const int U = m->async[method].unroll;
-    loop_begin_kernel<<<1, 1, 0, st>>>(m->d_loop, (ctx().cfg.max_iter + U - 1) / U, krr, nrr);
-    cudaStreamCaptureStatus cs;
-    cudaGraph_t g = nullptr;
-    const cudaGraphNode_t *deps = nullptr;
-    size_t ndeps = 0;
-    BICG_CUDA(cudaStreamGetCaptureInfo(st, &cs, nullptr, &g, &deps, &ndeps));
-    if (cs == cudaStreamCaptureStatusActive) {
-        cudaGraphNode_t node = add_device_loop(m, method, g, deps, ndeps);
-        BICG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
-    } else {
-        BICG_CUDA(cudaGraphLaunch(m->async[method].exec, st));
-    }
+    enqueue_while(m, st, (ctx().cfg.max_iter + U - 1) / U, krr, nrr, m->async[method].exec,
+                  [&](cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps) { return add_device_loop(m, method, g, deps, ndeps); });
 }
 
 } // namespace
@@ -657,14 +684,7 @@ int solve_async_prepare(bicg_matrix *m, int method)
     c.ensure();
     if (!m || method < 0 || method > 3) return -1;
     ensure_hist(m, c.cfg.max_iter);
-    if (!m->ev_last) {
-        // the handle's first asynchronous use: matrix_create returns with the upload and the plan's encoding kernels still in
-        // flight on the library's stream, and a synchronous call may have left work there too, so the handle's last work
-        // starts out as everything enqueued on that stream so far
-        BICG_CUDA(cudaEventCreateWithFlags(&m->ev_last, cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
-    }
-    if (!m->d_loop) m->d_loop = (AsyncLoopState *)c.dev_alloc(sizeof(AsyncLoopState));
+    async_handle_init(m);
     if (method == BICG_METHOD_PIPE_RR) solve_async_prepare(m, BICG_METHOD_PIPE);   // what PIPE_RR with krr <= 0 runs
     AsyncLoop &L = m->async[method];
     const int U = async_unroll(method);

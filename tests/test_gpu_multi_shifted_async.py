@@ -1,0 +1,23 @@
+"""GPU, N > 1 (skipped on boxes with fewer GPUs): asynchronous shifted solves and their captured replays row-partitioned over
+peer memory, bitwise equal to bicg_shifted_solve_dev on every rank, for every shifted method (tests/_mgpu_shifted_async_worker.py)."""
+import os
+import subprocess
+import sys
+
+import pytest
+
+pytestmark = pytest.mark.gpu
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.mark.parametrize("world", [2, 4])
+def test_multi_gpu_shifted_async(world):
+    import torch
+    if torch.cuda.device_count() < world:
+        pytest.skip(f"needs {world} GPUs")
+    port = 29860 + world
+    cmd = ["timeout", "600", sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}",
+           "--master-addr", "127.0.0.1", "--master-port", str(port), os.path.join(ROOT, "tests", "_mgpu_shifted_async_worker.py")]
+    p = subprocess.run(cmd, capture_output=True, text=True, timeout=700)
+    assert p.returncode == 0, p.stdout[-4000:] + p.stderr[-4000:]
+    assert f"MGPU_SHIFTED_ASYNC_OK {world}" in p.stdout
