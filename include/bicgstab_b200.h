@@ -129,8 +129,7 @@ int bicg_abi_version(void);
  *   BICG_TOL       (1e-15, solver.c:3)   BICG_MAX_ITER (1000, solver.c:4)   BICG_OUT_ITER (100, solver.c:9)
  *   BICG_QUIET=1   suppress the solver.c:124,135-139 stdout lines
  *   BICG_SPMV      auto | tma | rowsplit        BICG_SPMV_LANES  lanes per row (1,2,4,...,32; 0 = choose)
- *   BICG_GRAPH     1 (CUDA-graph replay of iteration batches) | 0 (plain stream launches)
- *   BICG_UNROLL    iterations per graph (default 10)
+ *   BICG_UNROLL    iterations per body of the kernel-per-phase loop's CUDA-graph WHILE node (default 10)
  *   BICG_CACHE     1 keep uploaded matrices keyed by host pointer (default) | 0 re-upload on every call
  *   BICG_DEVICE    CUDA device ordinal (default: LOCAL_RANK if set, else 0)
  *   BICG_MEGA      1 persistent solver kernel where it wins (thread-per-row plans; default) | 2 always | 0 kernel-per-phase graph
@@ -174,7 +173,10 @@ typedef struct {
     double h2d_ms, d2h_ms; /* host<->device copies of x, b / x, r done by this call        */
     double upload_ms;      /* matrix upload + planning done by this call (0 when cached)   */
     uint64_t h2d_bytes, d2h_bytes;
-    int    kernel_launches;/* kernels launched inside the timed region                      */
+    int    kernel_launches;/* kernels launched inside the timed region.  Kernel-per-phase loop: the init kernels plus
+                              every kernel of every WHILE body that ran, including those of the last body that
+                              returned at once after the loop test; far above the <= 8 of a persistent-kernel
+                              solve (its init kernels and the one loop kernel)                */
     int    spmv_lanes;     /* lanes per row the SpMV plan chose                             */
     int    spmv_kind;      /* 0 = tma tile kernel, 1 = rowsplit kernel                      */
 } bicg_stats;
@@ -243,8 +245,8 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
 /* bicg_shifted_solve_ex on DEVICE memory: x_set is sigma_len contiguous blocks of n_loc doubles (initial guesses in, solutions
  * out, updated in place; no padding or alignment required), r is n_loc doubles (b in, seed residual out). sigma stays a host
  * array. Same methods, return values, stdout, statistics, bicg_last_* results and BICG_SHIFT_ERROR report as
- * bicg_shifted_solve_ex, except that h2d_bytes and d2h_bytes are 0: x_set is never copied and no second copy of it is
- * allocated. Returns once the library's stream has synchronised, with the results in the caller's buffers. Collective:
+ * bicg_shifted_solve_ex, except that h2d_bytes and d2h_bytes are 0: x_set never crosses PCIe (it is staged device to device
+ * through the handle's workspace, as in bicg_shifted_solve_async). Returns once the library's stream has synchronised, with the results in the caller's buffers. Collective:
  * every rank returns -1 if any rank passed a null pointer, an unknown method, sigma_len <= 0 or a seed outside
  * [0, sigma_len), or if the ranks disagree on method, sigma_len or seed. */
 int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
@@ -314,9 +316,10 @@ int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc);
  * algorithmic bytes of one launch (12 nnz + 28 n_loc, SURVEY.md 8(d) phase P1) in *bytes. */
 int bicg_spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 
-/* per-kernel-class device time of one solve run WITHOUT graphs, each launch bracketed by events.
+/* per-kernel-class device time of one kernel-per-phase solve of exactly `iters` iterations (tol = 0) from x = 0, b = 1,
+ * every kernel launched from the host and bracketed by events (krr/nrr as in bicg_solve).
  * classes: 0 = SpMV(+dots), 1 = fused vector updates, 2 = other.  ms are totals over the solve. */
-int bicg_profile_solve(bicg_matrix *m, int method, int iters, double class_ms[3], int class_launches[3]);
+int bicg_profile_solve(bicg_matrix *m, int method, int iters, int krr, int nrr, double class_ms[3], int class_launches[3]);
 
 /* Test hooks for kernel-level parity (tests/test_gpu_kernels.py); single rank.  `vecs` holds the 11 arena vectors
  * x r r# p s y|z w v t b ax (n_loc doubles each), in and out.

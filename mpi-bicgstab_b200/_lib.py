@@ -96,7 +96,7 @@ SYMBOLS = {
     "bicg_last_shift_error": (C.c_int, [_P(C.c_double), C.c_int]),
     "bicg_spmv": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "bicg_spmv_time": (C.c_int, [C.c_void_p, C.c_int, _P(C.c_double), _P(C.c_double)]),
-    "bicg_profile_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_int, _P(C.c_double), _P(C.c_int)]),
+    "bicg_profile_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, _P(C.c_double), _P(C.c_int)]),
     "bicg_debug_vec_phase": (C.c_int, [C.c_void_p, C.c_int, _P(C.c_double), C.c_void_p, _P(C.c_double)]),
     "bicg_debug_spmv_epi": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, _P(C.c_double)]),
     "bicg_debug_get_vec": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),

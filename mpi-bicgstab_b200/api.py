@@ -555,10 +555,10 @@ class DeviceMatrix:
         lib.bicg_spmv_time(self.h, reps, C.byref(ms), C.byref(by))
         return ms.value, by.value
 
-    def profile(self, method, iters):
+    def profile(self, method, iters, krr=0, nrr=0):
         ms = (C.c_double * 3)()
         cnt = (C.c_int * 3)()
-        rc = lib.bicg_profile_solve(self.h, METHODS[method], iters, ms, cnt)
+        rc = lib.bicg_profile_solve(self.h, METHODS[method], iters, int(krr), int(nrr), ms, cnt)
         if rc != 0:
             raise RuntimeError("bicg_profile_solve failed")
         return list(ms), list(cnt)

@@ -36,7 +36,7 @@ int run_shifted(int method, CSR_Matrix *D, CSR_Matrix *O, INFO_Matrix *info, dou
     Context &c = ctx();
     c.ensure();
     bicg_matrix *m = matrix_get_cached(D, O, info, nullptr);
-    const int k = shifted_solve(m, method, x_loc_set, r_loc, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    const int k = shifted_solve(m, method, x_loc_set, r_loc, sigma, sigma_len, seed, false);
     if (!c.cfg.cache) matrix_destroy(m);
     return k;
 }
@@ -224,7 +224,7 @@ int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();
-    const int k = shifted_solve(m, BICG_SHIFTED_SWITCHING, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    const int k = shifted_solve(m, BICG_SHIFTED_SWITCHING, x_set, r, sigma, sigma_len, seed, false);
     if (stats) *stats = c.last_stats;
     return k;
 }
@@ -232,7 +232,7 @@ int bicg_shifted_solve_ex(bicg_matrix *m, int method, double *x_set, double *r, 
                           bicg_stats *stats)
 {
     Context &c = ctx();
-    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter);
+    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, false);
     if (stats) *stats = c.last_stats;
     return k;
 }
@@ -251,7 +251,7 @@ int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r,
     for (const Args &a : all)
         if (a.bad || a.method != method || a.len != sigma_len || a.seed != seed) return -1;
     c.ensure();
-    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, c.cfg.shift_tol, c.cfg.shift_max_iter, true);
+    const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, true);
     if (stats) *stats = c.last_stats;
     return k;
 }

@@ -37,7 +37,6 @@ struct Config {
     int spmv_stages = 0;
     int spmv_ctas = 0;           // CTAs per SM (0 choose)
     int autotune = 1;
-    int graph = 1;
     int unroll = 10;
     int cache = 1;
     int mega = 1;                // 1: persistent cooperative kernel for the iteration loop where applicable
@@ -87,9 +86,6 @@ struct Context {
     // host-pointer keyed cache of uploaded matrices
     std::map<const void *, bicg_matrix *> cache;
     std::map<TuneKey, TuneVal> tuned;     // SpMV autotune winners by matrix shape
-    // pinned scratch
-    static constexpr int FLAG_RING = 64;
-    int *h_flags = nullptr;      // ring of FLAG_RING done flags, one per batch of iterations in flight (run_batches)
     // profiling of individual launches
     bool prof_on = false;
     std::vector<cudaEvent_t> prof_ev;
@@ -162,19 +158,22 @@ struct MegaPlan {
     std::vector<int> cta_row;    // grid + 1: first row of every CTA
 };
 
-// The loop of an asynchronous solve on the kernel-per-phase path (solve.cu): templates captured from the same sequence as
-// ensure_graph, and the executable graph of one WHILE node around them that an uncaptured call launches.
-struct AsyncLoopState { int count, batches, krr, nrr; };   // device memory: bodies run, their bound, PIPE_RR's schedule
+// The kernel-per-phase loop of a solve (solve.cu): the captured bodies, the kernels each launches, and the executable graph of
+// one WHILE node around them that an uncaptured call launches.
+// device memory: bodies run (PIPE_RR: iterations run), their bound, PIPE_RR's schedule, what the last body added to count
+struct AsyncLoopState { int count, batches, krr, nrr, step; };
 struct AsyncLoop {
-    cudaGraph_t iters = nullptr;      // `unroll` iterations (PIPE_RR: one pipe_iter)
+    cudaGraph_t iters = nullptr;      // `unroll` iterations (PIPE_RR: `unroll` pipe_iter)
+    cudaGraph_t one = nullptr;        // PIPE_RR: one pipe_iter
     cudaGraph_t rr = nullptr;         // PIPE_RR: one rr_replace_iter
     cudaGraphExec_t exec = nullptr;
     int unroll = 0;
+    int kernels = 0, kernels_one = 0, kernels_rr = 0;  // kernels of one run of iters / one / rr
 };
 
-// What an asynchronous shifted solve of one family (shifted.cu, shifted_lop.cu) keeps on a handle: every device buffer of
-// the solve for sigma_len = L and BICG_SHIFT_MAX_ITER up to cap, its state template, and per variant of the family the
-// captured batch of ShiftedSolve::U iterations and the executable graph of one WHILE node around it.
+// What a shifted solve of one family (shifted.cu, shifted_lop.cu) keeps on a handle: every device buffer of the solve for
+// sigma_len = L and BICG_SHIFT_MAX_ITER up to cap, its state template, and per variant of the family the captured body of
+// ShiftedSolve::U iterations, the kernels it launches and the executable graph of one WHILE node around it.
 struct ShiftWork {
     int L = 0, cap = 0;
     std::vector<void *> mem;             // every buffer below and the family's arrays (Context::dev_alloc)
@@ -183,8 +182,10 @@ struct ShiftWork {
     std::vector<unsigned char> tmpl;     // host copy of *d_tmpl (the buffers the enqueue stages sigma into and clears)
     double *d_x = nullptr;               // [L][stride] the caller's x_set, staged
     double *d_p = nullptr;               // [L][stride] p_j
+    double *d_b = nullptr;               // [n] b, kept by a synchronous solve for BICG_SHIFT_ERROR
     cudaGraph_t iters[2] = {};
     cudaGraphExec_t exec[2] = {};
+    int kernels[2] = {};
 };
 // where the last asynchronous shifted solve on a handle left its history (device memory, written by its result kernel)
 struct ShiftHistRef { const double *hist; int n, pad; };
@@ -239,9 +240,6 @@ struct bicg_matrix {
     int push_nruns[bicg::MAX_RANKS - 1] = {};
     // fused-vector launch shape
     int vgrid = 0, vchunk = 0;
-    // captured iteration batches, per method
-    cudaGraphExec_t graph[4] = {};
-    int graph_unroll[4] = {};
     // cache key
     const void *host_key = nullptr;
     uint64_t host_fp = 0;            // content fingerprint of the caller's arrays at upload time (matrix.cu)
@@ -280,15 +278,15 @@ int  matrix_history(bicg_matrix *m, double *out, int cap);
 // every synchronous entry point that touches a handle first makes the library's stream wait for the handle's last
 // asynchronous work (free when there is none)
 void wait_handle(bicg_matrix *m);
-void drop_async_loop(AsyncLoop &L);        // frees what bicg_solve_async_prepare built for one method
-// The device-side loop of the asynchronous solves, shared by solve.cu and the shifted solvers.  async_handle_init: the
-// handle's first asynchronous use (its last-work event, recorded on the library's stream, and the loop state).
+void drop_async_loop(AsyncLoop &L);        // frees the prepared kernel-per-phase loop of one method
+// The device-side loop of every kernel-per-phase solve, shared by solve.cu and the shifted solvers.  async_handle_init: the
+// handle's first asynchronous use (its last-work event, recorded on the library's stream).
 void async_handle_init(bicg_matrix *m);
 cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args);
 cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
                                      cudaGraphConditionalNodeType type, cudaGraph_t *body);
-// A WHILE node of g behind deps: `fill` adds the body's work to `body` and returns its last nodes (at most 2) in `tail`; then
-// loop_next_kernel runs the body again unless *done is set or m->d_loop's bound of bodies has run
+// A WHILE node of g behind deps: `fill` adds the body's work to `body` and returns its last nodes (at most 3) in `tail`; then
+// loop_next_kernel runs the body again unless *done is set or m->d_loop's bound of bodies has run (allocates m->d_loop)
 cudaGraphNode_t add_while_node(bicg_matrix *m, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const int *done,
                                const std::function<size_t(cudaGraph_t body, cudaGraphNode_t *tail)> &fill);
 // the loop on `st` without the host: loop_begin_kernel (`batches` bodies at most), then the node `add` builds into the caller's
@@ -307,15 +305,12 @@ void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist
 void print_times(double seconds, double iters);          // "Total time" / "Avg time/iter" (= seconds / iters), then flush
 void reset_scalars(bicg_matrix *m, double tol, int max_iter);   // Scalars of a new solve (enqueued on the stream)
 void reset_scalars(bicg_matrix *m, double tol, int max_iter, cudaStream_t st);
-// The host side of every kernel-per-phase loop: enqueues batch b = 0, 1, ... of U iterations (max_iter / U rounded up)
-// and reads the device's done flag *d_done after each; from batch `depth` on it first waits for batch b - depth and
-// stops once the flag was raised by its end.  The loop test runs on the device, which returns from every kernel after it.
-void run_batches(int max_iter, int U, int depth, const int *d_done, const std::function<void(int)> &enqueue_batch);
-// shifted.cu: method = BICG_SHIFTED_*; returns what that solver returns (shifted_lopbicg_switching: iterations + 1, the others:
-// the iterations performed), -1 for an unknown method, sigma_len <= 0 or seed outside [0, sigma_len).  dev: x_set (sigma_len
-// blocks of n_loc, any 8-byte alignment) and r are device pointers, updated in place; sigma is always a host array.
-int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed, double tol,
-                   int max_iter, bool dev = false);
+// shifted.cu: method = BICG_SHIFTED_*, with BICG_SHIFT_TOL and BICG_SHIFT_MAX_ITER; returns what that solver returns
+// (shifted_lopbicg_switching: iterations + 1, the others: the iterations performed), -1 for an unknown method, sigma_len <= 0
+// or seed outside [0, sigma_len).  device_vectors: x_set (sigma_len blocks of n_loc, any 8-byte alignment) and r are device
+// pointers, else host pointers; sigma is always a host array.
+int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
+                   bool device_vectors);
 // shift_check.cu, collective: x_j = d_x + j ldx (own rows, device), d_b (device), sigma (host) -> sum_i ((A + sigma_j I) x_j - b)_i^2
 // for j < L and sum_i b_i^2 last (L + 1 values, over every rank, added in rank order); enqueued on the stream, synchronises
 std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);

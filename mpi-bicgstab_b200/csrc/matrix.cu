@@ -54,7 +54,6 @@ const Option OPTIONS[] = {
     {"SPMV_STAGES", Parse::Int, &Config::spmv_stages},
     {"SPMV_CTAS", Parse::Int, &Config::spmv_ctas},
     {"AUTOTUNE", Parse::Int, &Config::autotune},
-    {"GRAPH", Parse::Int, &Config::graph},
     {"UNROLL", Parse::Int, &Config::unroll, nullptr, 1},
     {"CACHE", Parse::Int, &Config::cache},
     {"MEGA", Parse::Int, &Config::mega},
@@ -138,7 +137,6 @@ void Context::ensure()
     int rc = spmv_setup_attributes();
     if (rc == 0) rc = mega_setup_attributes();
     if (rc != 0) fatal("bicgstab_b200: cudaFuncSetAttribute failed: %s", cudaGetErrorString((cudaError_t)rc));
-    BICG_CUDA(cudaHostAlloc((void **)&h_flags, FLAG_RING * sizeof(int), cudaHostAllocDefault));
     ready = true;
 }
 
@@ -914,7 +912,6 @@ void matrix_destroy(bicg_matrix *m)
     for (auto it = c.cache.begin(); it != c.cache.end();) {
         if (it->second == m) it = c.cache.erase(it); else ++it;
     }
-    for (int g = 0; g < 4; ++g) if (m->graph[g]) cudaGraphExecDestroy(m->graph[g]);
     for (AsyncLoop &L : m->async) drop_async_loop(L);
     c.dev_free(m->d_loop);
     for (double *h : m->hist_retired) cudaFree(h);

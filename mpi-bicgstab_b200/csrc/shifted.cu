@@ -11,7 +11,7 @@
 //     length-n vectors) are ONE multi-vector kernel (sh_vec_shift): q, r_old and r are loaded once per row, then x_j and
 //     p_j of every active shift are read and written exactly once -- 32 B per row and shift, the HBM floor of the method.
 // Element-wise operation order = the reference's call order with gcc's FMA contraction (y += a x -> fma(a, x, y)).
-// The host only enqueues batches of iterations and polls a done flag (as solve.cu does).
+// The host only enqueues: the loop runs on the device as a CUDA graph WHILE node (as solve.cu's kernel-per-phase loop does).
 //
 // The same solve also runs shifted_lopbicg (shifted_switching_solver.c:20-257; prototype :11), the fixed-seed variant: until the
 // seed converges its arithmetic is the switching solver's line for line.  With ShiftDev::fixed set, sh_scalar_iter skips the
@@ -196,8 +196,7 @@ struct ShVec {
     const ShiftDev *sd;
     double *r, *rh, *p, *s, *y, *qc, *rold;      // arena vectors (own parts)
     double *x_set, *p_set;
-    long long xstride;                           // doubles between consecutive shifts in x_set (blocks may be misaligned)
-    long long stride;                            // ... in p_set (even: every block starts 16-byte aligned)
+    long long stride;                            // doubles between consecutive shifts in both (even: every block starts 16-byte aligned)
     int n, L;
     int chunk;                                   // shifts per pass of sh_vec_shift, the size of its coefficient table (<= L)
 };
@@ -233,7 +232,7 @@ __global__ void __launch_bounds__(256) sh_vec_xr(const __grid_constant__ ShVec a
     if (a.sd->done) return;
     __shared__ double scratch[32 * MAX_DOTS];
     const double al = a.kc.sc->alpha, om = a.kc.sc->omega;
-    double *x = a.x_set + (size_t)a.sd->seed * a.xstride;
+    double *x = a.x_set + (size_t)a.sd->seed * a.stride;
     double dot[2] = {0.0, 0.0};
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
         const double q = a.r[i];
@@ -272,16 +271,15 @@ __global__ void __launch_bounds__(256) sh_vec_shift(const __grid_constant__ ShVe
 #pragma unroll 2
             for (int t = 0; t < na; ++t) {
                 const double *c = s_coef + (size_t)t * SH_COEF;
-                double *xj = a.x_set + (size_t)s_idx[t] * a.xstride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
-                const bool xa = aligned16(xj);
+                double *xj = a.x_set + (size_t)s_idx[t] * a.stride + i, *pj = a.p_set + (size_t)s_idx[t] * a.stride + i;
                 double x[2], p[2];
-                ld2x(xj, 0, two, xa, x); ld2(pj, 0, two, p);
+                ld2(xj, 0, two, x); ld2(pj, 0, two, p);
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     x[e] = fma(c[0], q[e], x[e]); x[e] = fma(c[1], p[e], x[e]);
                     p[e] = fma(c[2], q[e], p[e]); p[e] = fma(c[3], o[e], p[e]); p[e] = c[4] * p[e]; p[e] = fma(c[5], r[e], p[e]);
                 }
-                st2x(xj, 0, two, xa, x); st2(pj, 0, two, p);
+                st2(xj, 0, two, x); st2(pj, 0, two, p);
             }
         }
     }
@@ -419,43 +417,44 @@ ShRun sh_run(ShiftedSolve &s, ShiftDev *d_sd, double *d_p)
     run.base.sd = d_sd;
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.qc = m->vec(V_W); run.base.rold = m->vec(V_V);
-    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
+    run.base.x_set = s.ws.d_x; run.base.p_set = d_p; run.base.stride = s.stride;
     run.base.n = s.n; run.base.L = s.L;
     run.ugrid = s.update_grid();
     run.base.chunk = std::min(s.L, table_chunk(sh_vec_shift, SH_ENTRY));
     return run;
 }
 
-// The enqueue half of every switching / fixed-seed solve on s.st, synchronous or asynchronous: the state from the template
-// d_tmpl (host copy h), the inputs, the reference's timed region (:364).  The outputs are s.finish / s.finish_async.
-void sh_enqueue(ShiftedSolve &s, ShiftDev *d_sd, const ShiftDev *d_tmpl, const ShiftDev &h, double *d_p, double *x_set, double *r,
-                const double *sigma, bool fixed, int seed, double tol, int max_iter)
+// The enqueue half of every switching / fixed-seed solve on s.st, synchronous or asynchronous: the state from the workspace's
+// template, the inputs (x_set and b moved by `in`, sigma by `sigma_in`), the reference's timed region (:364).  The outputs are
+// s.finish / s.outputs.
+void sh_enqueue(ShiftedSolve &s, const double *x_set, const double *r, const double *sigma, cudaMemcpyKind in, cudaMemcpyKind sigma_in,
+                bool fixed, int seed)
 {
+    const Config &cfg = s.c.cfg;
+    const int max_iter = cfg.shift_max_iter + 1;                                      // :293 (shifted_lopbicg: k from 0, :53-55)
+    ShiftDev h;
+    memcpy(&h, s.ws.tmpl.data(), sizeof(ShiftDev));
+    ShiftDev *d_sd = (ShiftDev *)s.ws.d_state;
     BICG_CUDA(cudaMemsetAsync(h.pi_arch, 0, (size_t)s.L * max_iter * sizeof(double), s.st));
     BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), s.st));
-    s.upload(x_set, r, sigma, h.sigma);
-    sh_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, d_tmpl, fixed ? 1 : 0, seed, tol, max_iter);
+    s.upload(x_set, r, sigma, h.sigma, in, sigma_in);
+    sh_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, (const ShiftDev *)s.ws.d_tmpl, fixed ? 1 : 0, seed, cfg.shift_tol, max_iter);
     check_launch("sh_begin_kernel");
-    ShRun run = sh_run(s, d_sd, d_p);
+    ShRun run = sh_run(s, d_sd, s.ws.d_p);
     s.run(run, max_iter, &d_sd->done, 0);
 }
 
 } // namespace
 
-int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const double *sigma, int L, int seed, double tol,
-                    int max_iter_opt, bool dev)
+int switching_solve(bicg_matrix *m, ShiftWork &ws, bool fixed, double *x_set, double *r, const double *sigma, int seed,
+                    cudaMemcpyKind in, cudaMemcpyKind back)
 {
-    ShiftedSolve s(m, L, dev);
+    ShiftedSolve s(m, ws, ctx().stream);
     Context &c = s.c;
-    const int max_iter = max_iter_opt + 1;                                            // :293 (shifted_lopbicg: k from 0, :53-55)
-
-    double *d_p = nullptr;
-    const ShiftDev h = sh_buffers(s, max_iter, &d_p);
-    ShiftDev *d_sd = s.alloc<ShiftDev>(2);                                            // the state, its template
-    BICG_CUDA(cudaMemcpyAsync(d_sd + 1, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
-    sh_enqueue(s, d_sd, d_sd + 1, h, d_p, x_set, r, sigma, fixed, seed, tol, max_iter);
-    const ShiftDev out = s.finish(x_set, r, d_sd);
-
+    const int L = s.L;
+    s.synchronous(r, in);
+    sh_enqueue(s, x_set, r, sigma, in, cudaMemcpyHostToDevice, fixed, seed);
+    const ShiftDev out = s.finish(x_set, r, back, (const ShiftDev *)ws.d_state);
     // ---- results ------------------------------------------------------------------------------------------------------
     const int k = out.k;
     c.last_hist.assign((size_t)std::max(k, 1), 0.0);
@@ -492,53 +491,33 @@ int switching_solve(bicg_matrix *m, bool fixed, double *x_set, double *r, const 
     return fixed ? k - 1 : k;                                                         // :255 / :600
 }
 
-// the one mapping from a BICG_SHIFTED_* method to its solver
-int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
-                  bool dev)
-{
-    ctx().ensure();
-    if (L <= 0 || seed < 0 || seed >= L) return -1;
-    wait_handle(m);
-    switch (method) {
-    case BICG_SHIFTED_SWITCHING: return switching_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter, dev);
-    case BICG_SHIFTED_LOPBICG:   return switching_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);
-    case BICG_SHIFTED_LOP:       return lop_solve(m, false, x_set, r, sigma, L, seed, tol, max_iter, dev);
-    case BICG_SHIFTED_PIPE_LOP:  return lop_solve(m, true, x_set, r, sigma, L, seed, tol, max_iter, dev);
-    default: return -1;
-    }
-}
-
-void switching_prepare(bicg_matrix *m, ShiftWork &ws, int L)
+void switching_prepare(bicg_matrix *m, ShiftWork &ws)
 {
     Context &c = ctx();
-    ShiftedSolve s(m, L, ws, c.stream);
-    ShiftDev *d_sd = nullptr;
+    ShiftedSolve s(m, ws, c.stream);
     if (ws.mem.empty()) {
-        ws.L = L; ws.cap = c.cfg.shift_max_iter;
-        ws.d_x = s.d_x = s.alloc<double>((size_t)L * s.stride);
+        ws.d_x = s.alloc<double>((size_t)s.L * s.stride);
+        ws.d_b = s.alloc<double>(s.n);
         const ShiftDev h = sh_buffers(s, ws.cap + 1, &ws.d_p);
-        d_sd = s.alloc<ShiftDev>(2);
+        ShiftDev *d_sd = s.alloc<ShiftDev>(2);
         ws.d_state = d_sd; ws.d_tmpl = d_sd + 1;
         ws.tmpl.assign((const unsigned char *)&h, (const unsigned char *)&h + sizeof(ShiftDev));
         BICG_CUDA(cudaMemcpyAsync(ws.d_tmpl, &h, sizeof(ShiftDev), cudaMemcpyHostToDevice, c.stream));
     }
-    d_sd = (ShiftDev *)ws.d_state;
     if (!ws.exec[0]) {                              // the body is the same for both methods: `fixed` is a device flag
+        ShiftDev *d_sd = (ShiftDev *)ws.d_state;
         ShRun run = sh_run(s, d_sd, ws.d_p);
         s.capture_loop(run, &d_sd->done, 0);
     }
 }
 
 void switching_solve_async(bicg_matrix *m, ShiftWork &ws, bool fixed, double *x_set, double *r, const double *sigma, int seed,
-                           double tol, int max_iter_opt, cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+                           cudaStream_t st, bicg_shift_result *result, int *stop_iter)
 {
-    ShiftedSolve s(m, ws.L, ws, st);
-    ShiftDev h;
-    memcpy(&h, ws.tmpl.data(), sizeof(ShiftDev));
-    ShiftDev *d_sd = (ShiftDev *)ws.d_state;
-    sh_enqueue(s, d_sd, (const ShiftDev *)ws.d_tmpl, h, ws.d_p, x_set, r, sigma, fixed, seed, tol, max_iter_opt + 1);
-    s.finish_async(x_set, r);
-    sh_result_kernel<<<1, 256, 0, st>>>(d_sd, m->d_sc, result, stop_iter, m->d_shift_last);
+    ShiftedSolve s(m, ws, st);
+    sh_enqueue(s, x_set, r, sigma, cudaMemcpyDeviceToDevice, cudaMemcpyDeviceToDevice, fixed, seed);
+    s.outputs(x_set, r, cudaMemcpyDeviceToDevice);
+    sh_result_kernel<<<1, 256, 0, st>>>((const ShiftDev *)ws.d_state, m->d_sc, result, stop_iter, m->d_shift_last);
     check_launch("sh_result_kernel");
 }
 
@@ -577,7 +556,41 @@ void drop_work(bicg_matrix *m, ShiftWork &ws, bool retire)
     ws = ShiftWork();
 }
 
+// The workspace of `method`'s family for L shifts and the current BICG_SHIFT_MAX_ITER with the method's loop captured, on the
+// library's stream behind the handle's last work.  One for another L or a smaller bound is replaced.  Not collective.
+ShiftWork &shift_work(bicg_matrix *m, int method, int L)
+{
+    Context &c = ctx();
+    ShiftWork &ws = m->shift_ws[shift_family(method)];
+    if (!ws.mem.empty() && (ws.L != L || ws.cap < c.cfg.shift_max_iter)) {
+        // outgrown: nothing may still run on the old buffers when they return to the pool
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+        if (m->ev_last) BICG_CUDA(cudaEventSynchronize(m->ev_last));
+        drop_work(m, ws, m->captured);
+    }
+    if (ws.mem.empty()) { ws.L = L; ws.cap = c.cfg.shift_max_iter; }
+    if (shift_family(method) == 0) switching_prepare(m, ws);
+    else lop_prepare(m, ws, method == BICG_SHIFTED_PIPE_LOP);
+    return ws;
+}
+
 } // namespace
+
+int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed, bool device_vectors)
+{
+    ctx().ensure();
+    if (!shift_method_known(method) || L <= 0 || seed < 0 || seed >= L) return -1;
+    wait_handle(m);
+    ShiftWork &ws = shift_work(m, method, L);
+    const cudaMemcpyKind in = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+    const cudaMemcpyKind back = device_vectors ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+    switch (method) {
+    case BICG_SHIFTED_SWITCHING: return switching_solve(m, ws, false, x_set, r, sigma, seed, in, back);
+    case BICG_SHIFTED_LOPBICG:   return switching_solve(m, ws, true, x_set, r, sigma, seed, in, back);
+    case BICG_SHIFTED_LOP:       return lop_solve(m, ws, false, x_set, r, sigma, seed, in, back);
+    default:                     return lop_solve(m, ws, true, x_set, r, sigma, seed, in, back);
+    }
+}
 
 int shifted_async_prepare(bicg_matrix *m, int method, int L)
 {
@@ -590,13 +603,6 @@ int shifted_async_prepare(bicg_matrix *m, int method, int L)
         if (a.bad || a.method != method || a.len != L) return -1;
     c.ensure();
     async_handle_init(m);
-    ShiftWork &ws = m->shift_ws[shift_family(method)];
-    if (!ws.mem.empty() && (ws.L != L || ws.cap < c.cfg.shift_max_iter)) {
-        // outgrown: nothing may still run on the old buffers when they return to the pool
-        BICG_CUDA(cudaStreamSynchronize(c.stream));
-        BICG_CUDA(cudaEventSynchronize(m->ev_last));
-        drop_work(m, ws, m->captured);
-    }
     // what this enqueues on the library's stream (the history record's and the template's initial values) goes behind the
     // handle's last work and ahead of the next call on it
     wait_handle(m);
@@ -604,12 +610,10 @@ int shifted_async_prepare(bicg_matrix *m, int method, int L)
         m->d_shift_last = (ShiftHistRef *)c.dev_alloc(sizeof(ShiftHistRef));
         BICG_CUDA(cudaMemsetAsync(m->d_shift_last, 0, sizeof(ShiftHistRef), c.stream));
     }
-    if (shift_family(method) == 0) switching_prepare(m, ws, L);
-    else lop_prepare(m, ws, L, method == BICG_SHIFTED_PIPE_LOP);
+    shift_work(m, method, L);
     BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
     return 0;
 }
-
 int shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed,
                         cudaStream_t st, bicg_shift_result *result, int *stop_iter)
 {
@@ -627,13 +631,11 @@ int shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, co
     BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
     if (captured) m->captured = true;
     ShiftWork &ws = m->shift_ws[shift_family(method)];
-    const double tol = c.cfg.shift_tol;
-    const int max_iter = c.cfg.shift_max_iter;
     switch (method) {
-    case BICG_SHIFTED_SWITCHING: switching_solve_async(m, ws, false, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
-    case BICG_SHIFTED_LOPBICG:   switching_solve_async(m, ws, true, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
-    case BICG_SHIFTED_LOP:       lop_solve_async(m, ws, false, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
-    default:                     lop_solve_async(m, ws, true, x_set, r, sigma, seed, tol, max_iter, st, result, stop_iter); break;
+    case BICG_SHIFTED_SWITCHING: switching_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
+    case BICG_SHIFTED_LOPBICG:   switching_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
+    case BICG_SHIFTED_LOP:       lop_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
+    default:                     lop_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
     }
     BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
     return 0;

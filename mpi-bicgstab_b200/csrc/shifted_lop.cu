@@ -128,8 +128,7 @@ struct LopVec {
     const LopDev *sd;
     double *r, *rh, *p, *s, *y, *z, *w, *v, *t, *rold;  // arena vectors (own parts); y, z, w, v, t as the algorithm uses them
     double *x_set, *p_set;
-    long long xstride;                                  // doubles between consecutive shifts in x_set (blocks may be misaligned)
-    long long stride;                                   // ... in p_set (even: every block starts 16-byte aligned)
+    long long stride;                                   // doubles between consecutive shifts in both (even: 16-byte aligned blocks)
     int n, L;
     int chunk;                                          // non-seed shifts per pass of lop_vec_update, the size of its table
 };
@@ -205,25 +204,21 @@ __device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, 
     const LopDev *sd = a.sd;
     const int seed = sd->seed;
     const double al = sd->alpha, om = sd->omega;
-    double *xs = a.x_set + (size_t)seed * a.xstride;
-    const bool xs_al = aligned16(xs);
+    double *xs = a.x_set + (size_t)seed * a.stride;
     for (int i = 2 * (blockIdx.x * blockDim.x + threadIdx.x); i < a.n; i += 2 * gridDim.x * blockDim.x) {
         const bool two = i + 1 < a.n;                   // stride and arena vectors are 16-byte aligned, i is even
         double q[2], o[2];
         ld2(a.r, i, two, q); ld2(a.rold, i, two, o);
         if constexpr (SEED) {
             const int ne = two ? 2 : 1;
-            double x[2], p[2], y[2], r[2], rh[2];
-            ld2x(xs, i, two, xs_al, x); ld2(a.p, i, two, p); ld2(a.rh, i, two, rh);
-            ld2(PIPE ? a.w : a.y, i, two, y);
+            double y[2], r[2], rh[2];
+            ld2(a.rh, i, two, rh); ld2(PIPE ? a.w : a.y, i, two, y);
             for (int e = 0; e < ne; ++e) {
-                x[e] = fma(al, p[e], x[e]);
-                x[e] = fma(om, q[e], x[e]);
                 r[e] = fma(-om, y[e], q[e]);
                 dot[0] = fma(r[e], r[e], dot[0]);
                 dot[1] = fma(rh[e], r[e], dot[1]);
             }
-            st2x(xs, i, two, xs_al, x); st2(a.r, i, two, r);
+            st2(a.r, i, two, r);
             if constexpr (PIPE) {
                 double t[2], v[2], w[2], s[2], z[2];
                 ld2(a.t, i, two, t); ld2(a.v, i, two, v); ld2(a.s, i, two, s); ld2(a.z, i, two, z);
@@ -236,23 +231,29 @@ __device__ __forceinline__ void lop_rows(const LopVec &a, const double *s_coef, 
                 }
                 st2(a.w, i, two, w);
             }
+            double x[2], p[2];                          // last: fewer values live at once (64 registers with PIPE)
+            ld2(xs, i, two, x); ld2(a.p, i, two, p);
+            for (int e = 0; e < ne; ++e) {
+                x[e] = fma(al, p[e], x[e]);
+                x[e] = fma(om, q[e], x[e]);
+            }
+            st2(xs, i, two, x);
         }
         if (!two) { q[1] = 0.0; o[1] = 0.0; }
 #pragma unroll 2
         for (int t = 0; t < na; ++t) {
             const double *c = s_coef + (size_t)t * LOP_COEF;
             const size_t j = (size_t)(t0 + t < seed ? t0 + t : t0 + t + 1);
-            double *xj = a.x_set + j * a.xstride + i, *pj = a.p_set + j * a.stride + i;
-            const bool xa = aligned16(xj);
+            double *xj = a.x_set + j * a.stride + i, *pj = a.p_set + j * a.stride + i;
             double xv[2], pv[2];
-            ld2x(xj, 0, two, xa, xv); ld2(pj, 0, two, pv);
+            ld2(xj, 0, two, xv); ld2(pj, 0, two, pv);
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
                 pv[e] = c[0] * pv[e]; pv[e] = fma(c[1], o[e], pv[e]);
                 xv[e] = fma(c[2], q[e], xv[e]); xv[e] = fma(c[3], pv[e], xv[e]);
                 pv[e] = fma(c[4], q[e], pv[e]); pv[e] = fma(c[5], o[e], pv[e]);
             }
-            st2x(xj, 0, two, xa, xv); st2(pj, 0, two, pv);
+            st2(xj, 0, two, xv); st2(pj, 0, two, pv);
         }
     }
 }
@@ -409,7 +410,7 @@ LopRun lop_run(ShiftedSolve &s, bool pipe, LopDev *d_sd, double *d_p)
     run.base.r = m->vec(V_R); run.base.rh = m->vec(V_RH); run.base.p = m->vec(V_P); run.base.s = m->vec(V_S);
     run.base.y = m->vec(V_Y); run.base.z = m->vec(V_Z); run.base.w = m->vec(V_W); run.base.v = m->vec(V_V); run.base.t = m->vec(V_T);
     run.base.rold = m->vec(pipe ? V_AX : V_V);
-    run.base.x_set = s.d_x; run.base.p_set = d_p; run.base.xstride = s.xstride; run.base.stride = s.stride;
+    run.base.x_set = s.ws.d_x; run.base.p_set = d_p; run.base.stride = s.stride;
     run.base.n = s.n; run.base.L = s.L;
     run.ugrid = s.update_grid();
     constexpr size_t entry = LOP_COEF * sizeof(double);
@@ -417,34 +418,37 @@ LopRun lop_run(ShiftedSolve &s, bool pipe, LopDev *d_sd, double *d_p)
     return run;
 }
 
-// The enqueue half of every LOP / PIPE-LOP solve on s.st, synchronous or asynchronous: the state from the template d_tmpl
-// (host copy h), the inputs, the reference's timed region (:237 / :759).  The outputs are s.finish / s.finish_async.
-void lop_enqueue(ShiftedSolve &s, bool pipe, LopDev *d_sd, const LopDev *d_tmpl, const LopDev &h, double *d_p, double *x_set,
-                 double *r, const double *sigma, int seed, double tol, int max_iter)
+// The enqueue half of every LOP / PIPE-LOP solve on s.st, synchronous or asynchronous: the state from the workspace's template,
+// the inputs (x_set and b moved by `in`, sigma by `sigma_in`), the reference's timed region (:237 / :759).  The outputs are
+// s.finish / s.outputs.
+void lop_enqueue(ShiftedSolve &s, bool pipe, const double *x_set, const double *r, const double *sigma, cudaMemcpyKind in,
+                 cudaMemcpyKind sigma_in, int seed)
 {
+    const Config &cfg = s.c.cfg;
+    const int max_iter = cfg.shift_max_iter;
+    LopDev h;
+    memcpy(&h, s.ws.tmpl.data(), sizeof(LopDev));
+    LopDev *d_sd = (LopDev *)s.ws.d_state;
     BICG_CUDA(cudaMemsetAsync(h.hist, 0, ((size_t)max_iter + 1) * sizeof(double), s.st));
-    BICG_CUDA(cudaMemsetAsync(d_p, 0, (size_t)s.L * s.stride * sizeof(double), s.st));        // p_loc_set = calloc(...)  :226
-    s.upload(x_set, r, sigma, h.sigma);
-    lop_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, d_tmpl, seed, tol, max_iter);
+    BICG_CUDA(cudaMemsetAsync(s.ws.d_p, 0, (size_t)s.L * s.stride * sizeof(double), s.st));   // p_loc_set = calloc(...)  :226
+    s.upload(x_set, r, sigma, h.sigma, in, sigma_in);
+    lop_begin_kernel<<<1, 1, 0, s.st>>>(d_sd, (const LopDev *)s.ws.d_tmpl, seed, cfg.shift_tol, max_iter);
     check_launch("lop_begin_kernel");
-    LopRun run = lop_run(s, pipe, d_sd, d_p);
+    LopRun run = lop_run(s, pipe, d_sd, s.ws.d_p);
     s.run(run, max_iter, &d_sd->done, pipe ? 1 : 0);
 }
 
 } // namespace
 
-int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double *sigma, int L, int seed, double tol, int max_iter,
-              bool dev)
+int lop_solve(bicg_matrix *m, ShiftWork &ws, bool pipe, double *x_set, double *r, const double *sigma, int seed, cudaMemcpyKind in,
+              cudaMemcpyKind back)
 {
-    ShiftedSolve s(m, L, dev);
+    ShiftedSolve s(m, ws, ctx().stream);
     Context &c = s.c;
-
-    double *d_p = nullptr;
-    const LopDev h = lop_buffers(s, max_iter, &d_p);
-    LopDev *d_sd = s.alloc<LopDev>(2);                                                // the state, its template
-    BICG_CUDA(cudaMemcpyAsync(d_sd + 1, &h, sizeof(LopDev), cudaMemcpyHostToDevice, c.stream));
-    lop_enqueue(s, pipe, d_sd, d_sd + 1, h, d_p, x_set, r, sigma, seed, tol, max_iter);
-    const LopDev out = s.finish(x_set, r, d_sd);
+    const int L = s.L;
+    s.synchronous(r, in);
+    lop_enqueue(s, pipe, x_set, r, sigma, in, cudaMemcpyHostToDevice, seed);
+    const LopDev out = s.finish(x_set, r, back, (const LopDev *)ws.d_state);
 
     // ---- results ------------------------------------------------------------------------------------------------------
     const int k = out.k;
@@ -468,13 +472,13 @@ int lop_solve(bicg_matrix *m, bool pipe, double *x_set, double *r, const double 
     return k;                                                                         // :352 / :894
 }
 
-void lop_prepare(bicg_matrix *m, ShiftWork &ws, int L, bool pipe)
+void lop_prepare(bicg_matrix *m, ShiftWork &ws, bool pipe)
 {
     Context &c = ctx();
-    ShiftedSolve s(m, L, ws, c.stream);
+    ShiftedSolve s(m, ws, c.stream);
     if (ws.mem.empty()) {
-        ws.L = L; ws.cap = c.cfg.shift_max_iter;
-        ws.d_x = s.d_x = s.alloc<double>((size_t)L * s.stride);
+        ws.d_x = s.alloc<double>((size_t)s.L * s.stride);
+        ws.d_b = s.alloc<double>(s.n);
         const LopDev h = lop_buffers(s, ws.cap, &ws.d_p);
         LopDev *d_sd = s.alloc<LopDev>(2);
         ws.d_state = d_sd; ws.d_tmpl = d_sd + 1;
@@ -489,16 +493,13 @@ void lop_prepare(bicg_matrix *m, ShiftWork &ws, int L, bool pipe)
     }
 }
 
-void lop_solve_async(bicg_matrix *m, ShiftWork &ws, bool pipe, double *x_set, double *r, const double *sigma, int seed, double tol,
-                     int max_iter, cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+void lop_solve_async(bicg_matrix *m, ShiftWork &ws, bool pipe, double *x_set, double *r, const double *sigma, int seed,
+                     cudaStream_t st, bicg_shift_result *result, int *stop_iter)
 {
-    ShiftedSolve s(m, ws.L, ws, st);
-    LopDev h;
-    memcpy(&h, ws.tmpl.data(), sizeof(LopDev));
-    LopDev *d_sd = (LopDev *)ws.d_state;
-    lop_enqueue(s, pipe, d_sd, (const LopDev *)ws.d_tmpl, h, ws.d_p, x_set, r, sigma, seed, tol, max_iter);
-    s.finish_async(x_set, r);
-    lop_result_kernel<<<1, 256, 0, st>>>(d_sd, m->d_sc, result, stop_iter, m->d_shift_last);
+    ShiftedSolve s(m, ws, st);
+    lop_enqueue(s, pipe, x_set, r, sigma, cudaMemcpyDeviceToDevice, cudaMemcpyDeviceToDevice, seed);
+    s.outputs(x_set, r, cudaMemcpyDeviceToDevice);
+    lop_result_kernel<<<1, 256, 0, st>>>((const LopDev *)ws.d_state, m->d_sc, result, stop_iter, m->d_shift_last);
     check_launch("lop_result_kernel");
 }
 

@@ -4,9 +4,9 @@
 // seven one-double MPI_Iallreduce/MPI_Wait pairs per iteration.  Here the host only *enqueues*: every
 // scalar (alpha, beta, omega, the dot products, k, the loop test) lives in HBM, is produced by the tail of
 // the kernel that reduces it and is read by the kernels that follow, so an iteration is a fixed list of 4-5
-// kernel launches with no host round trip.  BICG_UNROLL iterations are captured once into a CUDA graph and
-// replayed; when the device-side loop test fails it raises Scalars::done and all later kernels of a batch
-// return immediately, so the iteration count is exact although the host looks at the flag only once per batch.
+// kernel launches with no host round trip.  BICG_UNROLL iterations are captured once into a CUDA graph, the body
+// of a conditional WHILE node that runs until the device-side loop test fails; that test raises Scalars::done and
+// all later kernels of a body return immediately, so the iteration count is exact.
 //
 //   bicgstab       K1 SpMV s=Ap (+ (r#,s))  K2 q  K3 SpMV y=Aq (+ (q,y),(y,y))  K4 x,r (+ 2 dots)  K5 p
 //   ca_bicgstab    C1 p,s  C2 SpMV z=As  C3 q,y (+ 2 dots)  C4 x,r (+ local (r,r))  C5 SpMV w=Ar (+ 4 dots, 5-value reduction)
@@ -41,27 +41,40 @@ __global__ void fill_kernel(double *p, int n, double v)
 
 __global__ void set_coef_kernel(Scalars *s, double al, double be, double om) { s->alpha = al; s->beta = be; s->omega = om; }
 
+// solver.c:498, 522: PIPE_RR replaces iteration k (krr > 0)
+__host__ __device__ bool rr_replaces(int k, int krr, int nrr) { return k % krr == 0 && k > 0 && k <= krr * nrr; }
+// PIPE_RR's loop body after k iterations: 0 for the replacement iteration, else the plain iterations it runs, U when no
+// replacement falls among the next U, else 1
+__host__ __device__ int rr_body(int k, int krr, int nrr, int U)
+{
+    if (rr_replaces(k, krr, nrr)) return 0;
+    const int next = (k / krr + 1) * krr;                  // the first multiple of krr after k
+    return next > krr * nrr || next >= k + U ? U : 1;
+}
+
 // ---- the device-side loop of the asynchronous solves (one thread each) ------------------------------------------
 __global__ void loop_begin_kernel(AsyncLoopState *st, int batches, int krr, int nrr)
 {
-    st->count = 0; st->batches = batches; st->krr = krr; st->nrr = nrr;
+    st->count = 0; st->batches = batches; st->krr = krr; st->nrr = nrr; st->step = 1;
 }
 
-// end of a WHILE body: run the next batch unless the loop test has failed (*done: Scalars::done, or a shifted solver's own)
-// or max_iter / U batches have run (run_batches' bound)
+// end of a WHILE body: run the next one unless the loop test has failed (*done: Scalars::done, or a shifted solver's own)
+// or max_iter / U bodies have run
 __global__ void loop_next_kernel(cudaGraphConditionalHandle loop, const int *done, AsyncLoopState *st)
 {
-    const int b = ++st->count;
+    const int b = st->count += st->step;
     cudaGraphSetConditional(loop, (!*done && b < st->batches) ? 1u : 0u);
 }
 
-// PIPE_RR: iteration k = bodies run so far is a replacement iteration where solve() schedules one (solver.c:498, 522)
-__global__ void rr_choose_kernel(cudaGraphConditionalHandle replace, cudaGraphConditionalHandle plain, const AsyncLoopState *st)
+// PIPE_RR: which body follows the k = st->count iterations run so far (rr_body), and how far it advances count
+__global__ void rr_choose_kernel(cudaGraphConditionalHandle replace, cudaGraphConditionalHandle one, cudaGraphConditionalHandle many,
+                                 AsyncLoopState *st, int U)
 {
-    const int k = st->count;
-    const bool rep = (k % st->krr == 0) && k > 0 && k <= st->krr * st->nrr;
-    cudaGraphSetConditional(replace, rep ? 1u : 0u);
-    cudaGraphSetConditional(plain, rep ? 0u : 1u);
+    const int s = rr_body(st->count, st->krr, st->nrr, U);
+    cudaGraphSetConditional(replace, s == 0 ? 1u : 0u);
+    cudaGraphSetConditional(one, s == 1 ? 1u : 0u);
+    cudaGraphSetConditional(many, s > 1 ? 1u : 0u);
+    st->step = s > 1 ? s : 1;
 }
 
 // what bicg_solve reports in bicg_stats, with the same IEEE operations as the host (solve(): st.final_res)
@@ -87,6 +100,7 @@ void drop_async_loop(AsyncLoop &L)
     if (L.exec) cudaGraphExecDestroy(L.exec);
     if (L.iters) cudaGraphDestroy(L.iters);
     if (L.rr) cudaGraphDestroy(L.rr);
+    if (L.one) cudaGraphDestroy(L.one);
     L = AsyncLoop();
 }
 
@@ -105,7 +119,6 @@ void async_handle_init(bicg_matrix *m)
         BICG_CUDA(cudaEventCreateWithFlags(&m->ev_last, cudaEventDisableTiming));
         BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
     }
-    if (!m->d_loop) m->d_loop = (AsyncLoopState *)c.dev_alloc(sizeof(AsyncLoopState));
 }
 
 cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args)
@@ -132,11 +145,12 @@ cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps,
 cudaGraphNode_t add_while_node(bicg_matrix *m, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const int *done,
                                const std::function<size_t(cudaGraph_t body, cudaGraphNode_t *tail)> &fill)
 {
+    if (!m->d_loop) m->d_loop = (AsyncLoopState *)ctx().dev_alloc(sizeof(AsyncLoopState));
     cudaGraphConditionalHandle loop;
     BICG_CUDA(cudaGraphConditionalHandleCreate(&loop, g, 1, cudaGraphCondAssignDefault));
     cudaGraph_t body = nullptr;
     const cudaGraphNode_t node = add_conditional_node(g, deps, ndeps, loop, cudaGraphCondTypeWhile, &body);
-    cudaGraphNode_t tail[2] = {};
+    cudaGraphNode_t tail[3] = {};
     const size_t ntail = fill(body, tail);
     AsyncLoopState *st = m->d_loop;
     void *largs[3] = {&loop, (void *)&done, (void *)&st};
@@ -228,26 +242,6 @@ void PhaseLauncher::spmv(int x_id, int y_id, TailDesc tail, int ndot, const doub
     for (int k = 0; k < ndot; ++k) epi_add_dot(a.epi, as[k], bs[k]);
     launch_spmv_plan(m, m->plan, a, stream, 0);
     ++launches;
-}
-
-void run_batches(int max_iter, int U, int depth, const int *d_done, const std::function<void(int)> &enqueue_batch)
-{
-    Context &c = ctx();
-    std::vector<cudaEvent_t> ring((size_t)Context::FLAG_RING, nullptr);
-    const int batches = (max_iter + U - 1) / U;
-    for (int b = 0; b < batches; ++b) {
-        if (b >= depth) {
-            const int o = (b - depth) % Context::FLAG_RING;
-            BICG_CUDA(cudaEventSynchronize(ring[(size_t)o]));
-            if (c.h_flags[o]) break;                             // done was raised in batch b - depth
-        }
-        enqueue_batch(b);
-        const int o = b % Context::FLAG_RING;
-        BICG_CUDA(cudaMemcpyAsync(&c.h_flags[o], d_done, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        if (!ring[(size_t)o]) BICG_CUDA(cudaEventCreateWithFlags(&ring[(size_t)o], cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(ring[(size_t)o], c.stream));
-    }
-    for (cudaEvent_t e : ring) if (e) cudaEventDestroy(e);       // released by the driver once the stream has passed them
 }
 
 void print_times(double seconds, double iters)
@@ -388,42 +382,31 @@ struct Seq : PhaseLauncher {
     }
 };
 
-int kernels_per_iter(int method, int world)
+// iterations 0 .. count - 1 of `method`'s loop body on s's stream
+void enqueue_iters(Seq &s, int method, int count, int krr, int nrr)
 {
-    (void)world;
-    switch (method) {
-    case BICG_METHOD_BICGSTAB: return 5;
-    case BICG_METHOD_CA: return 5;
-    default: return 4;
+    for (int k = 0; k < count; ++k) {
+        if (method == BICG_METHOD_BICGSTAB) s.bicgstab_iter();
+        else if (method == BICG_METHOD_CA) s.ca_iter();
+        else if (method == BICG_METHOD_PIPE_RR && rr_replaces(k, krr, nrr)) s.rr_replace_iter();
+        else s.pipe_iter();
     }
 }
 
-// `count` iterations of `method`'s loop body (rr: PIPE_RR's replacement iteration instead), captured on the library's stream
-cudaGraph_t capture_iters(bicg_matrix *m, int method, int count, bool rr)
+// `count` iterations of `method`'s loop body (rr: PIPE_RR's replacement iteration instead), captured on the library's stream;
+// *kernels: the kernels one replay launches
+cudaGraph_t capture_iters(bicg_matrix *m, int method, int count, bool rr, int *kernels)
 {
     Context &c = ctx();
     cudaGraph_t g = nullptr;
     BICG_CUDA(cudaStreamBeginCapture(c.stream, cudaStreamCaptureModeThreadLocal));
     Seq s(m);
-    for (int u = 0; u < count; ++u) {
-        if (rr) s.rr_replace_iter();
-        else if (method == BICG_METHOD_BICGSTAB) s.bicgstab_iter();
-        else if (method == BICG_METHOD_CA) s.ca_iter();
-        else s.pipe_iter();
-    }
+    if (rr) s.rr_replace_iter();
+    else enqueue_iters(s, method == BICG_METHOD_PIPE_RR ? BICG_METHOD_PIPE : method, count, 0, 0);
     BICG_CUDA(cudaStreamEndCapture(c.stream, &g));
     c.launches -= s.launches;       // capture is not execution
+    *kernels = s.launches;
     return g;
-}
-
-void ensure_graph(bicg_matrix *m, int method, int unroll)
-{
-    if (m->graph[method] && m->graph_unroll[method] == unroll) return;
-    if (m->graph[method]) { cudaGraphExecDestroy(m->graph[method]); m->graph[method] = nullptr; }
-    cudaGraph_t g = capture_iters(m, method, unroll, false);
-    BICG_CUDA(cudaGraphInstantiate(&m->graph[method], g, 0));
-    BICG_CUDA(cudaGraphDestroy(g));
-    m->graph_unroll[method] = unroll;
 }
 
 // a history for max_iter iterations.  Growing it synchronises and allocates, and drops every graph that holds the old pointer
@@ -440,15 +423,15 @@ void ensure_hist(bicg_matrix *m, int max_iter)
     else if (m->hist_extra) cudaFree(m->hist_extra);
     BICG_CUDA(cudaMalloc((void **)&m->hist_extra, ((size_t)max_iter + 2) * sizeof(double)));
     m->d_hist = m->hist_extra; m->hist_cap = max_iter + 2;
-    for (int g = 0; g < 4; ++g) if (m->graph[g]) { cudaGraphExecDestroy(m->graph[g]); m->graph[g] = nullptr; }
     for (AsyncLoop &L : m->async) drop_async_loop(L);
 }
 
-// iterations per WHILE body: PIPE_RR chooses every iteration's kind on the device, the others run BICG_UNROLL per body
-int async_unroll(int method) { return method == BICG_METHOD_PIPE_RR ? 1 : std::max(1, ctx().cfg.unroll); }
+// iterations per WHILE body
+int async_unroll(int) { return std::max(1, ctx().cfg.unroll); }
 
-// The kernel-per-phase loop as one WHILE node of `g` behind `deps`: its body is the prepared batch of iterations (PIPE_RR:
-// one iteration, its kind chosen by two IF nodes), then loop_next_kernel, which decides on the device whether the body runs again
+// The kernel-per-phase loop as one WHILE node of `g` behind `deps`: its body is the prepared batch of iterations (PIPE_RR: the
+// replacement iteration, one plain iteration or the batch, chosen by three IF nodes), then loop_next_kernel, which decides on
+// the device whether the body runs again
 cudaGraphNode_t add_device_loop(bicg_matrix *m, int method, cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps)
 {
     const AsyncLoop &L = m->async[method];
@@ -457,19 +440,20 @@ cudaGraphNode_t add_device_loop(bicg_matrix *m, int method, cudaGraph_t g, const
             BICG_CUDA(cudaGraphAddChildGraphNode(&tail[0], body, nullptr, 0, L.iters));
             return 1;
         }
-        cudaGraphConditionalHandle rep, plain;
-        BICG_CUDA(cudaGraphConditionalHandleCreate(&rep, body, 0, 0));
-        BICG_CUDA(cudaGraphConditionalHandleCreate(&plain, body, 0, 0));
-        const AsyncLoopState *st = m->d_loop;
-        void *cargs[3] = {&rep, &plain, (void *)&st};
+        cudaGraphConditionalHandle h[3];
+        for (cudaGraphConditionalHandle &c : h) BICG_CUDA(cudaGraphConditionalHandleCreate(&c, body, 0, 0));
+        AsyncLoopState *st = m->d_loop;
+        int U = L.unroll;
+        void *cargs[5] = {&h[0], &h[1], &h[2], (void *)&st, &U};
         const cudaGraphNode_t choose = add_kernel_node(body, nullptr, 0, (const void *)rr_choose_kernel, cargs);
-        cudaGraph_t b_rep = nullptr, b_plain = nullptr;
-        tail[0] = add_conditional_node(body, &choose, 1, rep, cudaGraphCondTypeIf, &b_rep);
-        tail[1] = add_conditional_node(body, &choose, 1, plain, cudaGraphCondTypeIf, &b_plain);
-        cudaGraphNode_t n;
-        BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_rep, nullptr, 0, L.rr));
-        BICG_CUDA(cudaGraphAddChildGraphNode(&n, b_plain, nullptr, 0, L.iters));
-        return 2;
+        const cudaGraph_t run[3] = {L.rr, L.one, L.iters};
+        for (int i = 0; i < 3; ++i) {
+            cudaGraph_t b = nullptr;
+            tail[i] = add_conditional_node(body, &choose, 1, h[i], cudaGraphCondTypeIf, &b);
+            cudaGraphNode_t n;
+            BICG_CUDA(cudaGraphAddChildGraphNode(&n, b, nullptr, 0, run[i]));
+        }
+        return 3;
     });
 }
 
@@ -479,11 +463,47 @@ bool async_prepared(const bicg_matrix *m, int method)
     return m->ev_last && m->d_loop && L.exec && L.unroll == async_unroll(method) && ctx().cfg.max_iter + 2 <= m->hist_cap;
 }
 
+// the WHILE loop of `method` for the current BICG_UNROLL: its bodies captured and the executable graph around them instantiated,
+// once per handle and method.  Synchronous solves call it only when the kernel-per-phase loop runs, and then behind their
+// init phases on the library's stream; a captured asynchronous solve finds it prepared.
+void prepare_device_loop(bicg_matrix *m, int method)
+{
+    AsyncLoop &L = m->async[method];
+    const int U = async_unroll(method);
+    if (L.exec && L.unroll == U) return;
+    drop_async_loop(L);
+    L.iters = capture_iters(m, method, U, false, &L.kernels);
+    if (method == BICG_METHOD_PIPE_RR) {
+        L.one = capture_iters(m, method, 1, false, &L.kernels_one);
+        L.rr = capture_iters(m, method, 1, true, &L.kernels_rr);
+    }
+    L.unroll = U;
+    cudaGraph_t g = nullptr;
+    BICG_CUDA(cudaGraphCreate(&g, 0));
+    add_device_loop(m, method, g, nullptr, 0);
+    BICG_CUDA(cudaGraphInstantiate(&L.exec, g, 0));
+    BICG_CUDA(cudaGraphDestroy(g));
+}
+
+// the kernels the prepared loop launched, from the loop state's count after a solve (PIPE_RR: the bodies rr_body chose)
+int loop_kernels(const bicg_matrix *m, int method, int count, int krr, int nrr)
+{
+    const AsyncLoop &L = m->async[method];
+    if (method != BICG_METHOD_PIPE_RR) return count * L.kernels;
+    int n = 0;
+    for (int k = 0; k < count;) {
+        const int s = rr_body(k, krr, nrr, L.unroll);
+        n += s == 0 ? L.kernels_rr : s == 1 ? L.kernels_one : L.kernels;
+        k += s > 1 ? s : 1;
+    }
+    return n;
+}
+
 // the kernel-per-phase loop on `st` without the host: into the caller's capture as a WHILE node, else the prepared graph
 void enqueue_device_loop(bicg_matrix *m, int method, int krr, int nrr, cudaStream_t st)
 {
-    const int U = m->async[method].unroll;
-    enqueue_while(m, st, (ctx().cfg.max_iter + U - 1) / U, krr, nrr, m->async[method].exec,
+    const int U = m->async[method].unroll, max_iter = ctx().cfg.max_iter;
+    enqueue_while(m, st, method == BICG_METHOD_PIPE_RR ? max_iter : (max_iter + U - 1) / U, krr, nrr, m->async[method].exec,
                   [&](cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps) { return add_device_loop(m, method, g, deps, ndeps); });
 }
 
@@ -511,11 +531,11 @@ namespace {
 }
 
 // The enqueue half of a solve on stream `st`: inputs, scalars, the init phases, the loop, the outputs.  marks: four events
-// recorded before and after the inputs, after the loop and after the outputs (bicg_solve's timing), or null.  device_loop:
-// the kernel-per-phase loop runs as a WHILE node (asynchronous solves); otherwise the host polls it as it always has.
-// Returns whether the persistent kernel ran the loop.
+// recorded before and after the inputs, after the loop and after the outputs (bicg_solve's timing), or null.  The loop is the
+// persistent kernel where it runs, else the WHILE node of the kernel-per-phase loop; bicg_profile_solve (Context::prof_on)
+// launches every iteration from the host instead.  Returns whether the persistent kernel ran the loop.
 bool enqueue_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, bool device_vectors, cudaStream_t st,
-                   const cudaEvent_t *marks, bool device_loop)
+                   const cudaEvent_t *marks)
 {
     Context &c = ctx();
     const Config &cfg = c.cfg;
@@ -547,30 +567,11 @@ bool enqueue_solve(bicg_matrix *m, int method, double *x, double *r, int krr, in
 
     bool use_mega = cfg.mega && m->mega.ok && !c.prof_on;
     if (use_mega) use_mega = seq.mega(method, krr, nrr);
-    if (!use_mega && device_loop) {
-        enqueue_device_loop(m, method, krr, nrr, st);
+    if (!use_mega && c.prof_on) {
+        enqueue_iters(seq, method, max_iter, krr, nrr);       // tol = 0: every iteration runs
     } else if (!use_mega) {
-        const bool use_graph = cfg.graph && !c.prof_on && method != BICG_METHOD_PIPE_RR;   // replacement iterations are host-scheduled
-        const int U = std::max(1, cfg.unroll);
-        if (use_graph) ensure_graph(m, method, U);
-        run_batches(max_iter, U, 3, &m->d_sc->done, [&](int b) {
-            if (use_graph) {
-                BICG_CUDA(cudaGraphLaunch(m->graph[method], c.stream));
-                c.launches += U * kernels_per_iter(method, m->world);
-                return;
-            }
-            for (int u = 0; u < U; ++u) {
-                const int k = b * U + u;
-                if (k >= max_iter) break;
-                if (method == BICG_METHOD_BICGSTAB) seq.bicgstab_iter();
-                else if (method == BICG_METHOD_CA) seq.ca_iter();
-                else if (method == BICG_METHOD_PIPE) seq.pipe_iter();
-                else {
-                    const bool replace = (k % krr == 0) && k > 0 && k <= krr * nrr;       // solver.c:498, 522
-                    if (replace) seq.rr_replace_iter(); else seq.pipe_iter();
-                }
-            }
-        });
+        prepare_device_loop(m, method);
+        enqueue_device_loop(m, method, krr, nrr, st);
     }
     if (marks) BICG_CUDA(cudaEventRecord(marks[2], st));
 
@@ -597,11 +598,14 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     cudaEvent_t ev[4];     // before / after the inputs, after the loop, after the outputs
     for (cudaEvent_t &e : ev) BICG_CUDA(cudaEventCreate(&e));
     const int launches0 = c.launches;
-    const bool use_mega = enqueue_solve(m, method, x, r, krr, nrr, device_vectors != 0, c.stream, ev, false);
+    const bool use_mega = enqueue_solve(m, method, x, r, krr, nrr, device_vectors != 0, c.stream, ev);
+    const bool device_loop = !use_mega && !c.prof_on;
 
     // ---- finish: statistics, trace, history --------------------------------------------------------------
     Scalars hs;
+    AsyncLoopState ls{};
     BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
+    if (device_loop) BICG_CUDA(cudaMemcpyAsync(&ls, m->d_loop, sizeof(AsyncLoopState), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
 
     if (hs.error) timeout_fatal(m);
@@ -667,7 +671,7 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     BICG_CUDA(cudaEventElapsedTime(&ms, ev[2], ev[3])); st.d2h_ms = ms;
     st.h2d_bytes = device_vectors ? 0 : 2 * vbytes;
     st.d2h_bytes = device_vectors ? 0 : 2 * vbytes;
-    st.kernel_launches = c.launches - launches0;
+    st.kernel_launches = c.launches - launches0 + (device_loop ? loop_kernels(m, method, ls.count, krr, nrr) : 0);
     st.spmv_lanes = m->plan.lanes; st.spmv_kind = m->plan.kind;
     for (cudaEvent_t e : ev) cudaEventDestroy(e);
 
@@ -685,19 +689,8 @@ int solve_async_prepare(bicg_matrix *m, int method)
     if (!m || method < 0 || method > 3) return -1;
     ensure_hist(m, c.cfg.max_iter);
     async_handle_init(m);
-    if (method == BICG_METHOD_PIPE_RR) solve_async_prepare(m, BICG_METHOD_PIPE);   // what PIPE_RR with krr <= 0 runs
-    AsyncLoop &L = m->async[method];
-    const int U = async_unroll(method);
-    if (L.exec && L.unroll == U) return 0;
-    drop_async_loop(L);
-    L.iters = capture_iters(m, method, U, false);
-    if (method == BICG_METHOD_PIPE_RR) L.rr = capture_iters(m, method, 1, true);
-    L.unroll = U;
-    cudaGraph_t g = nullptr;
-    BICG_CUDA(cudaGraphCreate(&g, 0));
-    add_device_loop(m, method, g, nullptr, 0);
-    BICG_CUDA(cudaGraphInstantiate(&L.exec, g, 0));
-    BICG_CUDA(cudaGraphDestroy(g));
+    if (method == BICG_METHOD_PIPE_RR) prepare_device_loop(m, BICG_METHOD_PIPE);    // what PIPE_RR with krr <= 0 runs
+    prepare_device_loop(m, method);
     return 0;
 }
 
@@ -716,7 +709,7 @@ int solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int n
     // order the replays behind the handle's last work at replay time
     BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
     if (captured) m->captured = true;
-    enqueue_solve(m, method, x, r, krr, nrr, true, st, nullptr, true);
+    enqueue_solve(m, method, x, r, krr, nrr, true, st, nullptr);
     if (result) result_kernel<<<1, 1, 0, st>>>(m->d_sc, result);
     BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
     return 0;
@@ -944,9 +937,9 @@ extern "C" int bicg_debug_stream_values(bicg_matrix *m, int on)
 }
 
 // ------------------------------------------------------------------------------------------------
-// profile: one solve with plain stream launches, every launch bracketed by events
+// profile: one solve of `iters` iterations launched from the host, every launch bracketed by events
 // ------------------------------------------------------------------------------------------------
-extern "C" int bicg_profile_solve(bicg_matrix *m, int method, int iters, double class_ms[3], int class_launches[3])
+extern "C" int bicg_profile_solve(bicg_matrix *m, int method, int iters, int krr, int nrr, double class_ms[3], int class_launches[3])
 {
     using namespace bicg;
     Context &c = ctx();
@@ -956,7 +949,7 @@ extern "C" int bicg_profile_solve(bicg_matrix *m, int method, int iters, double 
     if (iters + 2 > m->hist_cap) { c.cfg = saved; return -1; }
     std::vector<double> x((size_t)m->n_loc, 0.0), b((size_t)m->n_loc, 1.0);
     c.prof_on = true; c.prof_ev.clear(); c.prof_class.clear();
-    solve(m, method, x.data(), b.data(), 0, 0, 0, nullptr);
+    solve(m, method, x.data(), b.data(), krr, nrr, 0, nullptr);
     c.prof_on = false;
     for (int k = 0; k < 3; ++k) { class_ms[k] = 0.0; class_launches[k] = 0; }
     for (size_t i = 0; i < c.prof_class.size(); ++i) {

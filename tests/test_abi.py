@@ -322,11 +322,13 @@ def test_halo_runs_gap_merging(B):
             assert k <= 3                          # one run per owner
 
 
-def test_options_and_unknown_keys(B):
-    B.set_options(tol=1e-9, max_iter=77, out_iter=5, unroll=4, graph=0, cache=1, mega=1)
+def test_options_retired_and_unknown_keys(B):
+    B.set_options(tol=1e-9, max_iter=77, out_iter=5, unroll=4, cache=1, mega=1)
     with pytest.raises(KeyError):
         B.set_option("NO_SUCH_OPTION", 1)
-    B.set_options(tol=1e-15, max_iter=1000, out_iter=100, unroll=10, graph=1)
+    with pytest.raises(KeyError):                  # retired: the kernel-per-phase loop always runs as a CUDA-graph WHILE node
+        B.set_options(graph=0)
+    B.set_options(tol=1e-15, max_iter=1000, out_iter=100, unroll=10)
     assert B.lib.bicg_comm_rank() == 0 and B.lib.bicg_comm_world() == 1 and B.lib.bicg_comm_selftest() == 0
 
 

@@ -7,6 +7,7 @@ Tolerances (SURVEY.md 8(c), north_star: residual history within 1e-10 relative):
 The summation order of the dots and of each row differs from the reference's scalar loops (parallel
 reduction), so bit-exactness is not expected beyond the element-wise updates.
 """
+import ctypes as C
 import os
 
 import numpy as np
@@ -85,21 +86,36 @@ def test_history_and_convergence(B, O, name, kind, g, p0, method):
     assert abs(np.dot(b, b) / np.dot(b0, b0) - hist[iters]) <= 1e-9 * hist[iters]
 
 
-@pytest.mark.parametrize("method", METHODS[:3])
-def test_graph_and_stream_paths_agree(B, method):
+@pytest.mark.parametrize("method", METHODS)
+def test_while_loop_and_host_launches_agree(B, method):
+    """The kernel-per-phase loop as a CUDA-graph WHILE node (bicg_solve, BICG_MEGA=0) and the same iterations launched one by
+    one from the host (bicg_profile_solve) run the same kernels in the same order: x, r and the scalars are bitwise equal.
+    pipe_bicgstab_rr replaces iterations 4, 8 and 12 of 14 (krr nrr = 12)."""
     blk = B.gen_block("stencil15", 12, 14.0)
-    n = blk.n
-    out = {}
-    for graph in (1, 0):
-        B.set_options(tol=1e-9, max_iter=400, graph=graph, mega=0)
-        b = B.spmv_ovlap(blk, np.ones(n))
-        x = np.zeros(n)
-        it = B.solve(method, blk, x, b)
-        out[graph] = (it, x.copy(), B.last_history().copy())
-    B.set_options(graph=1)
-    assert out[0][0] == out[1][0]
-    assert np.array_equal(out[0][1], out[1][1])          # same kernels, same order -> bitwise equal
-    assert np.array_equal(out[0][2], out[1][2])
+    n, k = blk.n, 14
+    kw = dict(krr=4, nrr=3) if method.endswith("rr") else {}
+    dm = B.DeviceMatrix(blk)
+
+    def state():
+        v = [np.empty(n) for _ in range(2)]
+        for vec, vid in zip(v, (0, 1)):                   # x, r
+            assert B.lib.bicg_debug_get_vec(dm.h, vid, vec.ctypes.data_as(C.c_void_p)) == 0
+        s13 = (C.c_double * 13)()
+        B.lib.bicg_debug_get_scalars(dm.h, s13)
+        return v + [np.array(s13[:])]
+
+    try:
+        B.set_options(tol=0.0, max_iter=k, mega=0)
+        x, r = np.zeros(n), np.ones(n)                    # bicg_profile_solve's inputs
+        it, _ = dm.solve(method, x, r, **kw)
+        assert it == k
+        graph = state()
+        dm.profile(method, k, **kw)
+        stream = state()
+    finally:
+        dm.destroy()
+    for name, g, s_ in zip(("x", "r", "scalars"), graph, stream):
+        assert np.array_equal(g, s_), name               # same kernels, same order -> bitwise equal
 
 
 def test_max_iter_stops_exactly(B):

@@ -6,12 +6,12 @@ import pytest
 DEFAULTS = {
     "TOL": "1e-15", "MAX_ITER": "1000", "OUT_ITER": "100", "QUIET": "0",
     "SPMV": "auto", "SPMV_LANES": "0", "SPMV_THREADS": "0", "SPMV_STAGES": "0", "SPMV_CTAS": "0",
-    "AUTOTUNE": "1", "GRAPH": "1", "UNROLL": "10", "CACHE": "1",
+    "AUTOTUNE": "1", "UNROLL": "10", "CACHE": "1",
     "MEGA": "1", "MEGA_THREADS": "0", "MEGA_TRACE": "0", "MEGA_LANES": "0", "RESIDENT": "1",
     "BOUNDARY_WEIGHT": "300", "ROW_WEIGHT": "1200", "DEVICE": "-1", "HALO_GAP": "64", "VERBOSE": "0",
     "PEER_TIMEOUT_S": "20", "SHIFT_TOL": "1e-12", "SHIFT_MAX_ITER": "1000", "SHIFT_ERROR": "0",
 }
-RETIRED = ["GATHER_CG", "L2_HINT", "FENCE_WRITERS", "STAGE_UPLOAD"]
+RETIRED = ["GATHER_CG", "L2_HINT", "FENCE_WRITERS", "STAGE_UPLOAD", "GRAPH"]
 
 
 @pytest.mark.parametrize("prefix", ["", "BICG_"])

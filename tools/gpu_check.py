@@ -32,8 +32,8 @@ for w in which:
     print(f"spmv+dot: {ms * 1e3:.1f} us, {by / ms / 1e6:.0f} GB/s algorithmic = {by / ms / 1e6 / PEAK:.3f} of measured HBM peak", flush=True)
     n = blk.n
     for method in ("bicgstab", "ca_bicgstab", "pipe_bicgstab"):
-        for graph in (2, 1, 0):
-            B.set_options(tol=0.0, max_iter=200, graph=min(graph, 1), mega=1 if graph == 2 else 0)
+        for mega in (1, 0):
+            B.set_options(tol=0.0, max_iter=200, mega=mega)
             b = dm.spmv(np.ones(n))
             x = np.zeros(n)
             it, st = dm.solve(method, x, b)
@@ -41,9 +41,9 @@ for w in which:
             per = st["loop_ms"] / max(it, 1) * 1e3
             nb = {"bicgstab": 160, "ca_bicgstab": 216, "pipe_bicgstab": 232}[method]
             byt = 24 * blk.nnz_loc + nb * n
-            print(f"{method:14s} mode={['stream', 'graph', 'mega'][graph]}: {it} it, {per:.1f} us/it, {1e6 / per:.0f} it/s, "
+            print(f"{method:14s} mode={['graph', 'mega'][mega]}: {it} it, {per:.1f} us/it, {1e6 / per:.0f} it/s, "
                   f"{byt / per / 1e3:.0f} GB/s = {byt / per / 1e3 / PEAK:.3f} of peak, launches {st['kernel_launches']}", flush=True)
-    B.set_options(graph=1, mega=1)
+    B.set_options(mega=1)
     ms3, cnt3 = dm.profile("bicgstab", 100)
     print("profile bicgstab 100 it: class ms", [round(v, 3) for v in ms3], "launches", cnt3,
           "avg us", [round(1e3 * a / max(b_, 1), 1) for a, b_ in zip(ms3, cnt3)], flush=True)

@@ -1,5 +1,5 @@
 """Short, deterministic run for ncu: one matrix, a few iterations of one method.
-usage: prof_run.py <workload> <method> <iters> <mode: mega|graph|stream>"""
+usage: prof_run.py <workload> <method> <iters> <mode: mega|graph>"""
 import os
 import sys
 
@@ -12,8 +12,8 @@ import mpi_bicgstab_b200 as B
 workload = sys.argv[1] if len(sys.argv) > 1 else "transport"
 method = sys.argv[2] if len(sys.argv) > 2 else "bicgstab"
 iters = int(sys.argv[3]) if len(sys.argv) > 3 else 30
-mode = sys.argv[4] if len(sys.argv) > 4 else "stream"
-B.set_options(quiet=1, tol=0.0, max_iter=iters, mega=1 if mode == "mega" else 0, graph=1 if mode == "graph" else 0)
+mode = sys.argv[4] if len(sys.argv) > 4 else "graph"
+B.set_options(quiet=1, tol=0.0, max_iter=iters, mega=1 if mode == "mega" else 0)
 blk = {"transport": lambda: B.gen_block("stencil15", 117, 14.0), "laplace": lambda: B.gen_block("laplace5", 2000),
        "random": lambda: B.gen_block("random", 2_000_000, 32)}[workload]()
 dm = B.DeviceMatrix(blk)

@@ -25,7 +25,7 @@ nl = blk.n_loc
 resident = [int(v) for v in os.environ.get("QP_RESIDENT", "").split(",") if v != ""]       # e.g. "1,0": persistent kernel with / without resident slices
 for method in (sys.argv[1:] or ["bicgstab", "ca_bicgstab", "pipe_bicgstab"]):
     for mode in (modes if not resident else [f"mega/r{r}" for r in resident]):
-        kw = dict(mega=1) if mode.startswith("mega") else dict(mega=0, graph=1)
+        kw = dict(mega=1) if mode.startswith("mega") else dict(mega=0)
         if "/r" in mode:
             kw["resident"] = int(mode[-1])
         B.set_options(tol=0.0, max_iter=iters, **kw)
