@@ -7,8 +7,8 @@
  * compiles UNCHANGED against include/compat/mpi.h + the reference's own solver.h and links against
  * this library instead of solver.c / matrix.c / vector.c.
  * Part 2 is the small extension surface (prefix bicg_) that tests, bench.py and multi-process
- * launchers use: rank/communicator bootstrap, device-resident matrices, solve statistics,
- * synthetic-matrix generators.  No torch / CUDA types appear anywhere in this header.
+ * launchers use: rank/communicator bootstrap, device-resident matrices (whose values can be
+ * replaced in place, pattern kept), solve statistics, synthetic-matrix generators.  No torch / CUDA types appear anywhere in this header.
  *
  * Every entry point drives hand-written sm_90a CUDA kernels; there is no CPU fallback -- if no
  * CUDA device is usable the compute entry points print an error and exit(1) (the reference's own
@@ -161,6 +161,38 @@ void         bicg_matrix_destroy(bicg_matrix *m);
 /* drop the cached upload of a host matrix whose values were changed in place (csr_shift_diagonal,
  * matrix.c:536-551, does that) */
 void         bicg_matrix_invalidate(const CSR_Matrix *diag);
+
+/* New values on a resident matrix, same pattern: for a sequence of systems that share one sparsity pattern (implicit time
+ * steps, Newton-Krylov, continuation, a diagonal shift).  The halo plan, the merged layout, the arena, the SpMV and
+ * persistent-kernel plans and the column codes are kept; the merged values are rewritten and the persistent kernel's per-CTA
+ * value tables and packed values rebuilt by the pass bicg_matrix_create runs, so every result on the handle afterwards is
+ * bit-identical to that of a handle freshly created from blocks holding the same values.  Pointers on the handle do not
+ * change: a captured solve keeps working and reads the new values when it is replayed.
+ *
+ * Values: diag_val holds diag.nz doubles and offd_val offd.nz doubles, in the order of the CSR_Matrix blocks the handle was
+ * created from (their ptr and col are the creation's by contract and are not passed again).  diag_val must not be null;
+ * offd_val may be null only when the handle has no offd entries (always with one rank, where the offd block is ignored).
+ * Returns 0, or -1 for a null handle or diag_val (checked before the device is touched) or a null offd_val on a handle with
+ * offd entries.
+ *
+ * Rank-local: neither call communicates, so neither is collective.  Each rank sets the values of its own rows; the next solve
+ * is collective as before and multiplies with whatever values every rank has set.  No bootstrap exchange runs again, which is
+ * what makes an update cheap on several GPUs.
+ *
+ * bicg_matrix_set_values: host pointers, or device pointers when device_vectors != 0.  Waits for the handle's earlier
+ * asynchronous work and returns once the new values are in place.
+ * bicg_matrix_set_values_async: device pointers only, enqueued on the caller's CUDA stream `stream` behind the handle's
+ * previous work, with the ordering of bicg_solve_async: no host synchronisation, allocation or pageable copy, and the values
+ * are read in stream order, so a replay of a captured update reads the buffers as they are at that point.  It needs no prepare
+ * step and works inside a stream capture as it is (there is no -2).
+ *
+ * bicg_matrix_shift_diagonal: A_diag += sigma I on the handle, like csr_shift_diagonal (matrix.c:536-551) on the host arrays:
+ * sigma is added to the first entry of every own row whose column is that row; repeated calls accumulate.  Synchronous and
+ * rank-local.  Returns 0, or -1 for a null handle or when a row of this rank has no diagonal entry (the reference exits
+ * there), and then no value has changed.  An asynchronous shift is bicg_matrix_set_values_async with shifted values. */
+int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, int device_vectors);
+int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream);
+int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma);
 
 enum { BICG_METHOD_BICGSTAB = 0, BICG_METHOD_CA = 1, BICG_METHOD_PIPE = 2, BICG_METHOD_PIPE_RR = 3 };
 

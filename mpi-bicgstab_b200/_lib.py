@@ -80,6 +80,9 @@ SYMBOLS = {
     "bicg_matrix_create": (C.c_void_p, [_P(CSR_Matrix), _P(CSR_Matrix), _P(INFO_Matrix)]),
     "bicg_matrix_destroy": (None, [C.c_void_p]),
     "bicg_matrix_invalidate": (None, [_P(CSR_Matrix)]),
+    "bicg_matrix_set_values": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
+    "bicg_matrix_set_values_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bicg_matrix_shift_diagonal": (C.c_int, [C.c_void_p, C.c_double]),
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "bicg_solve_async_prepare": (C.c_int, [C.c_void_p, C.c_int]),

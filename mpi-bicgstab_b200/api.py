@@ -296,6 +296,29 @@ def _checked_cuda_vectors(*args):
     return [C.c_void_p(t.data_ptr()) for _, t, _ in args]
 
 
+def _value_args(blk, diag_val, offd_val):
+    """(name, array, expected shape) of new values for blk's blocks; offd_val may be None only where the handle has no offd
+    entries (one rank, or an empty offd block)."""
+    args = [("diag_val", diag_val, (int(blk.diag.nz),))]
+    if offd_val is not None:
+        args.append(("offd_val", offd_val, (int(blk.offd.nz),)))
+    elif int(blk.offd.nz) and lib.bicg_comm_world() > 1:
+        raise ValueError(f"offd_val: the offd block has {int(blk.offd.nz)} entries, got None")
+    return args
+
+
+def _checked_host_vectors(*args):
+    """Pointers of numpy float64 arrays, given as (name, array, expected shape) triples: contiguous, of the expected shape."""
+    for name, a, shape in args:
+        if a.dtype != np.float64:
+            raise TypeError(f"{name}: need a float64 array, got {a.dtype}")
+        if not a.flags["C_CONTIGUOUS"]:
+            raise ValueError(f"{name}: need a contiguous array")
+        if a.shape != tuple(shape):
+            raise ValueError(f"{name}: shape {a.shape}, expected {tuple(shape)}")
+    return [_dptr(a) for _, a, _ in args]
+
+
 def _host_sigma(sigma):
     """sigma as a contiguous float64 numpy array; a torch tensor (on any device) is copied to the host."""
     if not isinstance(sigma, np.ndarray) and hasattr(sigma, "detach"):
@@ -388,6 +411,46 @@ class DeviceMatrix:
         self.h = lib.bicg_matrix_create(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info))
         if not self.h:
             raise RuntimeError("bicg_matrix_create failed")
+
+    def set_values(self, diag_val, offd_val=None):
+        """bicg_matrix_set_values: new values for the pattern the handle was created with, in the order of blk's diag and offd
+        blocks (blk.diag.nz and blk.offd.nz of them; offd_val may be None where the handle has no offd entries).  Both numpy
+        float64 arrays, or both contiguous CUDA float64 tensors (read after torch's current stream has been synchronised).
+        Returns once the values are in place; every later result equals that of a handle freshly created from the new values.
+        Rank-local: each rank sets its own rows.  blk's host arrays keep the old values: they no longer describe the device
+        matrix."""
+        args = _value_args(self.blk, diag_val, offd_val)
+        if all(isinstance(a, np.ndarray) for _, a, _ in args):
+            ptrs, dev = _checked_host_vectors(*args), 0
+        else:
+            ptrs, dev = _cuda_vectors(*args), 1
+        rc = lib.bicg_matrix_set_values(self.h, ptrs[0], ptrs[1] if len(ptrs) > 1 else None, dev)
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_set_values failed with {rc}")
+
+    def set_values_async(self, diag_val, offd_val=None, stream=None):
+        """bicg_matrix_set_values_async: set_values on contiguous CUDA float64 tensors only, enqueued on `stream` (default: torch's
+        current stream) behind the handle's earlier work, with no host synchronisation.  The tensors are read in stream order,
+        so a replay of a captured update reads them as they are then; works inside torch.cuda.graph with no prepare step.  blk's
+        host arrays no longer describe the device matrix afterwards."""
+        import torch
+        args = _value_args(self.blk, diag_val, offd_val)
+        for name, a, _ in args:
+            if not isinstance(a, torch.Tensor):
+                raise TypeError(f"{name}: set_values_async takes CUDA tensors only, got {type(a).__name__}")
+        ptrs = _checked_cuda_vectors(*args)
+        if stream is None:
+            stream = torch.cuda.current_stream(diag_val.device)
+        rc = lib.bicg_matrix_set_values_async(self.h, ptrs[0], ptrs[1] if len(ptrs) > 1 else None, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_set_values_async failed with {rc}")
+
+    def shift_diagonal(self, sigma):
+        """bicg_matrix_shift_diagonal: A_diag += sigma I on the device, like csr_shift_diagonal on the host blocks (the first
+        entry of every own row whose column is that row; calls accumulate).  Raises ValueError, with no value changed, when a
+        row of this rank has no diagonal entry.  blk's host arrays no longer describe the device matrix afterwards."""
+        if lib.bicg_matrix_shift_diagonal(self.h, float(sigma)) != 0:
+            raise ValueError("bicg_matrix_shift_diagonal failed: a row of this rank has no diagonal entry (no value was changed)")
 
     def solve(self, method, x, r, krr=0, nrr=0):
         """bicg_solve: x (initial guess in, solution out) and r (b in, final residual out) are both numpy float64 arrays, or both

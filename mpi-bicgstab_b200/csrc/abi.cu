@@ -210,6 +210,16 @@ void bicg_matrix_invalidate(const CSR_Matrix *diag)
     else c.cache[(const void *)m] = m;
 }
 
+int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, int device_vectors)
+{
+    return matrix_set_values(m, diag_val, offd_val, device_vectors != 0, false, nullptr);
+}
+int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream)
+{
+    return matrix_set_values(m, diag_val, offd_val, true, true, (cudaStream_t)stream);
+}
+int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma) { return matrix_shift_diagonal(m, sigma); }
+
 int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *stats)
 {
     return solve(m, method, x, r, krr, nrr, device_vectors, stats);

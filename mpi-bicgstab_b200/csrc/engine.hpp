@@ -197,12 +197,19 @@ struct bicg_matrix {
     int rank = 0, world = 1;
     int n_loc = 0, n_glob = 0;
     size_t nnz = 0;              // entries of this rank's rows (diag + offd)
+    size_t nnz_offd = 0;         // ... of them from the offd block (0 on one rank)
     unsigned max_row = 0;
     double mean_row = 0.0;
     // device CSR over the extended local column space
     double *d_val = nullptr;
     unsigned *d_col = nullptr;
     unsigned *d_ptr = nullptr;
+    // value updates (bicg_matrix_set_values*, bicg_matrix_shift_diagonal): with offd entries, the diag and offd row pointers of
+    // the creation, [2][n_loc + 1], which place the caller's values in d_val; the position in d_val of every own row's
+    // diagonal entry (-1: none), computed at the first shift, and whether some row has none
+    unsigned *d_blk_ptr = nullptr;
+    int *d_diag_pos = nullptr;
+    bool diag_missing = false;
     bicg::SpmvPlan plan;
     bicg::MegaPlan mega;             // persistent-kernel plan (mega.cu)
     bicg::MegaSync *d_msync = nullptr;
@@ -269,6 +276,9 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
 void matrix_destroy(bicg_matrix *m);
 double matrix_upload_ms(bicg_matrix *m);
 bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, bool *fresh);
+// bicg_matrix_set_values (async = false: on the library's stream, returns once done) and bicg_matrix_set_values_async (on st)
+int  matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st);
+int  matrix_shift_diagonal(bicg_matrix *m, double sigma);     // bicg_matrix_shift_diagonal
 // solve.cu
 int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *st);
 // bicg_solve_async / bicg_solve_async_prepare / bicg_matrix_history (include/bicgstab_b200.h)

@@ -491,6 +491,17 @@ static int mega_lanes_for(double mean_row)
     return 32;
 }
 
+// The value tables and packed values of the persistent kernel's plan (mega.cu: mega_value_kernel) from d_val, on `st`.  The
+// plan's creation and every value update run this same pass, so an updated handle holds what a fresh one would.
+static void launch_value_tables(const bicg_matrix *m, cudaStream_t st)
+{
+    const MegaPlan &mp = m->mega;
+    if (!mp.d_vtab) return;
+    launch_mega_values(m->d_val, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, mp.grid, m->ghost_off, mp.d_cta_dep, mp.d_vtab, mp.d_vhi,
+                       mp.d_vmid, mp.d_vlo, st);
+    BICG_CUDA(cudaGetLastError());
+}
+
 // Plan of the persistent solver kernel (mega.cu): one CTA per SM, every CTA owns a contiguous, work-balanced range of rows
 // (plan.cpp: plan_cta_tiles), cut into tiles of <= threads / lanes rows.  row_extra[i] = number of peers row i is pushed to.
 static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::vector<unsigned char> &row_extra)
@@ -576,9 +587,7 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
             BICG_CUDA(cudaMemsetAsync(mp.d_vhi + m->nnz, 0, pad, c.stream));
             BICG_CUDA(cudaMemsetAsync(mp.d_vmid + m->nnz, 0, pad * sizeof(unsigned short), c.stream));
             BICG_CUDA(cudaMemsetAsync(mp.d_vlo + m->nnz, 0, pad * sizeof(unsigned), c.stream));
-            launch_mega_values(m->d_val, m->d_ptr, mp.d_tile_row, mp.d_cta_tile, G, m->ghost_off, mp.d_cta_dep, mp.d_vtab, mp.d_vhi,
-                               mp.d_vmid, mp.d_vlo, c.stream);
-            BICG_CUDA(cudaGetLastError());
+            launch_value_tables(m, c.stream);
         }
         mp.ok = true;
         if (c.cfg.verbose)
@@ -591,27 +600,66 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
 // ------------------------------------------------------------------------------------------------
 // device-side merge of the reference's diag / offd blocks (matrix.c:380-392) into one CSR over [own | ghost] columns
 // ------------------------------------------------------------------------------------------------
-// One thread per row: diag entries first, then offd entries (the reference's accumulation order, matrix.c:437-440);
-// an offd entry's global column becomes ghost_off + ghost slot of the receive run that contains it.
+// Where row i's entries land in the merged CSR: its diag entries first, then its offd entries (the reference's accumulation
+// order, matrix.c:437-440).  diag(k, j): diag entry j goes to merged entry k; offd(k, j) likewise.  The merge of
+// matrix_create and every value update place entries through this one function.
+template <class Diag, class Offd>
+__device__ __forceinline__ void merge_row(int i, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr, Diag diag,
+                                          Offd offd)
+{
+    const unsigned d0 = dptr[i], d1 = dptr[i + 1], o0 = optr[i], o1 = optr[i + 1];
+    unsigned k = d0 + o0;
+    for (unsigned j = d0; j < d1; ++j, ++k) diag(k, j);
+    for (unsigned j = o0; j < o1; ++j, ++k) offd(k, j);
+}
+
+// One thread per row; an offd entry's global column becomes ghost_off + ghost slot of the receive run that contains it.
 __global__ void __launch_bounds__(256) merge_rows_kernel(int n_loc, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr,
                                                          const double *__restrict__ dval, const unsigned *__restrict__ dcol,
                                                          const double *__restrict__ oval, const unsigned *__restrict__ ocol,
                                                          const int *__restrict__ runs /* quadruples */, int nruns, int ghost_off,
                                                          double *__restrict__ mval, unsigned *__restrict__ mcol)
 {
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x)
+        merge_row(i, dptr, optr, [&](unsigned k, unsigned j) { mval[k] = dval[j]; mcol[k] = dcol[j]; },
+                  [&](unsigned k, unsigned j) {
+                      const int gc = (int)ocol[j];
+                      int a = 0, b = nruns;                          // last run whose first column is <= gc
+                      while (b - a > 1) { const int mid = (a + b) >> 1; if (runs[4 * mid] <= gc) a = mid; else b = mid; }
+                      mval[k] = oval[j];
+                      mcol[k] = (unsigned)(ghost_off + runs[4 * a + 3] + (gc - runs[4 * a]));
+                  });
+}
+
+// the values alone, for a value update: the columns are the creation's
+__global__ void __launch_bounds__(256) merge_values_kernel(int n_loc, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr,
+                                                           const double *__restrict__ dval, const double *__restrict__ oval,
+                                                           double *__restrict__ mval)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x)
+        merge_row(i, dptr, optr, [&](unsigned k, unsigned j) { mval[k] = dval[j]; }, [&](unsigned k, unsigned j) { mval[k] = oval[j]; });
+}
+
+// bicg_matrix_shift_diagonal: the first entry of every own row whose column is that row (matrix.c:540-545).  Own columns are
+// local (< n_loc) and ghost columns >= ghost_off >= n_loc, so the search can only end among the row's diag entries.
+__global__ void __launch_bounds__(256) diag_pos_kernel(int n_loc, const unsigned *__restrict__ ptr, const unsigned *__restrict__ col,
+                                                       int *__restrict__ pos, int *__restrict__ missing)
+{
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x) {
-        const unsigned d0 = dptr[i], d1 = dptr[i + 1], o0 = optr[i], o1 = optr[i + 1];
-        unsigned k = d0 + o0;
-        for (unsigned j = d0; j < d1; ++j, ++k) { mval[k] = dval[j]; mcol[k] = dcol[j]; }
-        for (unsigned j = o0; j < o1; ++j, ++k) {
-            const int gc = (int)ocol[j];
-            int a = 0, b = nruns;                          // last run whose first column is <= gc
-            while (b - a > 1) { const int mid = (a + b) >> 1; if (runs[4 * mid] <= gc) a = mid; else b = mid; }
-            mval[k] = oval[j];
-            mcol[k] = (unsigned)(ghost_off + runs[4 * a + 3] + (gc - runs[4 * a]));
-        }
+        int p = -1;
+        for (unsigned j = ptr[i]; j < ptr[i + 1]; ++j)
+            if (col[j] == (unsigned)i) { p = (int)j; break; }
+        pos[i] = p;
+        if (p < 0) atomicAdd(missing, 1);
     }
 }
+
+__global__ void __launch_bounds__(256) shift_diag_kernel(int n_loc, const int *__restrict__ pos, double sigma, double *__restrict__ val)
+{
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x) val[pos[i]] += sigma;
+}
+
+static int row_blocks(int n_loc) { return std::max(1, std::min((n_loc + 255) / 256, ctx().sm_count * 8)); }
 
 void Context::release_arenas()
 {
@@ -671,6 +719,7 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
     m->n_loc = (int)diag->rows; m->n_glob = (int)info->rows;
     const size_t nd = diag->nz, no = (offd && m->world > 1) ? offd->nz : 0;
     m->nnz = nd + no;
+    m->nnz_offd = no;
     m->host_key = diag->val ? (const void *)diag->val : (const void *)diag;
     m->ghost_off = round_up(m->n_loc, 16);
 
@@ -767,16 +816,17 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
         }
         c.h2d(t_oval, offd->val, no * sizeof(double));
         c.h2d(t_ocol, offd->col, no * sizeof(unsigned));
-        const int blocks = std::max(1, std::min((m->n_loc + 255) / 256, c.sm_count * 8));
-        merge_rows_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, t_ptr, t_ptr + np1, t_dval, t_dcol, t_oval, t_ocol, t_runs,
-                                                        (int)(m->recv_runs.size() / 4), m->ghost_off, m->d_val, m->d_col);
+        merge_rows_kernel<<<row_blocks(m->n_loc), 256, 0, c.stream>>>(m->n_loc, t_ptr, t_ptr + np1, t_dval, t_dcol, t_oval, t_ocol,
+                                                                      t_runs, (int)(m->recv_runs.size() / 4), m->ghost_off, m->d_val,
+                                                                      m->d_col);
         BICG_CUDA(cudaGetLastError());
+        m->d_blk_ptr = t_ptr;                               // kept: value updates place entries with it (merge_values_kernel)
         // back to the pool -- but only once the merge has run: planning below fills freshly allocated blocks with SYNCHRONOUS
         // copies that are not ordered behind this stream
         cudaEvent_t merged;
         BICG_CUDA(cudaEventCreateWithFlags(&merged, cudaEventDisableTiming));
         BICG_CUDA(cudaEventRecord(merged, c.stream));
-        c.dev_free_after({t_dval, t_oval, t_dcol, t_ocol, t_ptr, t_runs}, merged);
+        c.dev_free_after({t_dval, t_oval, t_dcol, t_ocol, t_runs}, merged);
     }
     m->upload_bytes = m->nnz * 12 + ((size_t)m->n_loc + 1) * 4 * (no ? 2 : 1);
 
@@ -927,9 +977,82 @@ void matrix_destroy(bicg_matrix *m)
     c.dev_free(m->mega.d_vtab); c.dev_free(m->mega.d_vhi); c.dev_free(m->mega.d_vmid); c.dev_free(m->mega.d_vlo);
     if (m->hist_extra) cudaFree(m->hist_extra);
     c.dev_free(m->d_val); c.dev_free(m->d_col); c.dev_free(m->d_ptr);
+    c.dev_free(m->d_blk_ptr); c.dev_free(m->d_diag_pos);
     if (m->world > 1) c.arena_pool.emplace(m->arena_bytes, Context::ArenaRec{m->arena, m->arena_bytes, m->arena_id, m->arena_handle});
     else c.dev_free(m->arena);
     delete m;
+}
+
+// ------------------------------------------------------------------------------------------------
+// value updates: everything but d_val and what matrix_create derived from it (the value tables and packed values of the
+// persistent kernel's plan) depends on the pattern alone and stays
+// ------------------------------------------------------------------------------------------------
+int matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st)
+{
+    if (!m || !diag_val) return -1;
+    Context &c = ctx();
+    c.ensure();
+    const size_t no = m->nnz_offd, nd = m->nnz - no;
+    if (no && !offd_val) return -1;
+    bool captured = false;
+    if (async) {
+        cudaStreamCaptureStatus cs;
+        BICG_CUDA(cudaStreamIsCapturing(st, &cs));
+        captured = cs != cudaStreamCaptureStatusNone;
+        async_handle_init(m);
+        BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    } else {
+        wait_handle(m);
+        st = c.stream;
+    }
+    double *stage = nullptr;                  // host values with offd entries: staged through a pool block, as at creation
+    if (!device_ptrs && no) {
+        stage = (double *)c.dev_alloc((nd + no) * sizeof(double));
+        if (nd) c.h2d(stage, diag_val, nd * sizeof(double));
+        c.h2d(stage + nd, offd_val, no * sizeof(double));
+        diag_val = stage; offd_val = stage + nd;
+    }
+    if (!no) {
+        if (nd && device_ptrs) BICG_CUDA(cudaMemcpyAsync(m->d_val, diag_val, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        else if (nd) c.h2d(m->d_val, diag_val, nd * sizeof(double));
+    } else {
+        const size_t np1 = (size_t)m->n_loc + 1;
+        merge_values_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_blk_ptr, m->d_blk_ptr + np1, diag_val, offd_val, m->d_val);
+        BICG_CUDA(cudaGetLastError());
+    }
+    launch_value_tables(m, st);
+    if (async) {
+        BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    } else {
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+        c.dev_free(stage);
+    }
+    return 0;
+}
+
+int matrix_shift_diagonal(bicg_matrix *m, double sigma)
+{
+    if (!m) return -1;
+    Context &c = ctx();
+    c.ensure();
+    wait_handle(m);
+    const int blocks = row_blocks(m->n_loc);
+    if (!m->d_diag_pos) {
+        m->d_diag_pos = (int *)c.dev_alloc(((size_t)m->n_loc + 1) * sizeof(int));      // + the count of rows without one
+        int missing = 0;
+        BICG_CUDA(cudaMemsetAsync(m->d_diag_pos + m->n_loc, 0, sizeof(int), c.stream));
+        diag_pos_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_ptr, m->d_col, m->d_diag_pos, m->d_diag_pos + m->n_loc);
+        BICG_CUDA(cudaGetLastError());
+        BICG_CUDA(cudaMemcpyAsync(&missing, m->d_diag_pos + m->n_loc, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+        m->diag_missing = missing > 0;
+    }
+    if (m->diag_missing) return -1;           // the reference exits here (matrix.c:547-550); nothing has been changed
+    shift_diag_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
+    BICG_CUDA(cudaGetLastError());
+    launch_value_tables(m, c.stream);
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    return 0;
 }
 
 // Content fingerprint of the caller's blocks: sizes + up to 8192 evenly spaced samples of val / col / ptr of both blocks
