@@ -343,6 +343,37 @@ int bicg_last_shift_error(double *out, int cap);
 /* y_loc = A x_loc on a resident matrix (host pointers) -- the kernel behind MPI_csr_spmv_ovlap. */
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc);
 
+/* y_j = alpha (A + sigma_j I) x_j + beta y_j on this rank's rows, j < nvec: forming a right-hand side from the current matrix,
+ * a true residual b - A x (alpha = -1, beta = 1, y = b), (A + sigma_j I) x_j for the x_set of a shifted solve.  x and y are
+ * nvec contiguous blocks of n_loc doubles (the x_set layout: any 8-byte alignment, no padding).  sigma is null (no shift term)
+ * or nvec doubles.  One pass over the matrix serves up to 8 vectors (csrc/multiply.cu).
+ *
+ * Arithmetic, per component i of vector j:
+ *   t = the row sum exactly as bicg_spmv computes it on this handle (same plan, lanes and order over the merged layout), so
+ *       with sigma null and alpha = 1, beta = 0, y_j is bit-identical to bicg_spmv(x_j), whatever nvec is;
+ *   sigma given: t = fma(sigma_j, x_j[i], t), for every j including sigma_j = 0 (so a null sigma and a zero sigma can differ
+ *       in the sign of a zero);
+ *   beta == 0: y = alpha * t, and y is not read (a NaN in y does not propagate); else y = fma(alpha, t, beta * y_in).
+ * Returns 0, or -1 for a null handle, x or y, nvec <= 0, or x's range overlapping y's (a gather SpMV cannot run in place);
+ * these are checked before the device is touched.  bicg_last_stats, bicg_last_history and bicg_last_shift_* are not updated.
+ *
+ * bicg_matrix_multiply: x and y are host pointers, or device pointers when device_vectors != 0; sigma is a host array.
+ * Waits for the handle's earlier asynchronous work and returns once y is in the caller's buffer.
+ * bicg_matrix_multiply_async: x, y and sigma are device pointers, read and written in stream order on the caller's CUDA stream
+ * `stream` behind the handle's previous work, with the ordering of bicg_solve_async: no host synchronisation, allocation,
+ * pageable copy or output.  It needs no prepare step and works inside a stream capture as it is (there is no -2); a replay
+ * reads x, y and sigma as they are at that point.
+ *
+ * Collective, like bicg_spmv: the ghost columns of every x_j come from the neighbours, and the call ends in an empty
+ * cross-GPU reduction.  The synchronous call checks its arguments on every rank first: every rank returns -1 if any rank's
+ * arguments are bad or the ranks disagree on nvec or on whether sigma is null; a peer timeout is fatal, as in bicg_spmv.  The
+ * asynchronous call checks its arguments locally, so the ranks must agree on nvec and on whether sigma is null; a peer timeout
+ * there is reported by the next synchronous call on the handle. */
+int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
+                         const double *sigma, int device_vectors);
+int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
+                               const double *sigma, void *stream);
+
 /* Time `reps` launches of the fused SpMV + (r_hat, s) dot kernel (the dominant kernel of every
  * variant) with CUDA events on the library's stream; returns average ms per launch in *ms and the
  * algorithmic bytes of one launch (12 nnz + 28 n_loc, SURVEY.md 8(d) phase P1) in *bytes. */

@@ -82,6 +82,10 @@ SYMBOLS = {
     "bicg_matrix_invalidate": (None, [_P(CSR_Matrix)]),
     "bicg_matrix_set_values": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]),
     "bicg_matrix_set_values_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bicg_matrix_multiply": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
+                                       C.c_int]),
+    "bicg_matrix_multiply_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
+                                             C.c_void_p]),
     "bicg_matrix_shift_diagonal": (C.c_int, [C.c_void_p, C.c_double]),
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

@@ -586,6 +586,64 @@ class DeviceMatrix:
             raise ValueError(f"bicg_shift_residuals failed with {rc}")
         return out[:L]
 
+    def _multiply_shape(self, x):
+        """(n_loc,) or (nvec, n_loc) as x has it; a shape that is neither is then rejected by the vector checks"""
+        n = self.blk.n_loc
+        shape = tuple(getattr(x, "shape", ()))
+        return shape if len(shape) in (1, 2) and shape[-1] == n else (n,)
+
+    def multiply(self, x, y=None, alpha=1.0, beta=0.0, sigma=None):
+        """bicg_matrix_multiply: y_j = alpha (A + sigma_j I) x_j + beta y_j for every row x_j of x, on the GPU.  x is a numpy float64
+        array or a contiguous CUDA float64 tensor of shape (n_loc,) or (nvec, n_loc); y has the same kind and shape and is
+        allocated when None (then beta must be 0).  sigma: None (no shift term) or nvec values (numpy or tensor, copied to the
+        host).  With sigma None, alpha = 1 and beta = 0 every y_j is bit-identical to spmv(x_j).  Tensors are read after torch's
+        current stream has been synchronised.  Collective over the ranks.  Returns y."""
+        shape = self._multiply_shape(x)
+        nvec = shape[0] if len(shape) == 2 else 1
+        if y is None:
+            if beta != 0.0:
+                raise ValueError("y: needed when beta != 0")
+            if isinstance(x, np.ndarray):
+                y = np.empty(shape)
+            elif hasattr(x, "new_empty"):
+                y = x.new_empty(shape, dtype=x.dtype)
+        args = [("x", x, shape), ("y", y, shape)]
+        if isinstance(x, np.ndarray) and isinstance(y, np.ndarray):
+            (xp, yp), dev = _checked_host_vectors(*args), 0
+        else:
+            (xp, yp), dev = _cuda_vectors(*args), 1
+        sp_ = None
+        if sigma is not None:
+            sigma = _host_sigma(sigma)
+            if sigma.shape != (nvec,):
+                raise ValueError(f"sigma: shape {sigma.shape}, expected ({nvec},)")
+            sp_ = _dptr(sigma)
+        rc = lib.bicg_matrix_multiply(self.h, nvec, xp, yp, float(alpha), float(beta), sp_, dev)
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_multiply failed with {rc}")
+        return y
+
+    def multiply_async(self, x, y, alpha=1.0, beta=0.0, sigma=None, stream=None):
+        """bicg_matrix_multiply_async: multiply on contiguous CUDA float64 tensors only, enqueued on `stream` (default: torch's
+        current stream) behind the handle's earlier work, with no host synchronisation.  x and y as in multiply (y is required);
+        sigma: None or a CUDA float64 tensor of shape (nvec,).  All are read and written in stream order, so a replay of a
+        captured multiply reads them as they are then; works inside torch.cuda.graph with no prepare step.  Returns y."""
+        import torch
+        for name, t in (("x", x), ("y", y)) + ((("sigma", sigma),) if sigma is not None else ()):
+            if not isinstance(t, torch.Tensor):
+                raise TypeError(f"{name}: multiply_async takes CUDA tensors only, got {type(t).__name__}")
+        shape = self._multiply_shape(x)
+        nvec = shape[0] if len(shape) == 2 else 1
+        args = [("x", x, shape), ("y", y, shape)] + ([("sigma", sigma, (nvec,))] if sigma is not None else [])
+        ptrs = _checked_cuda_vectors(*args)
+        if stream is None:
+            stream = torch.cuda.current_stream(x.device)
+        rc = lib.bicg_matrix_multiply_async(self.h, nvec, ptrs[0], ptrs[1], float(alpha), float(beta),
+                                            ptrs[2] if sigma is not None else None, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_multiply_async failed with {rc}")
+        return y
+
     def spmv(self, x_loc):
         y = np.empty(self.blk.n_loc)
         lib.bicg_spmv(self.h, _vec(x_loc, self.blk.n_loc), _dptr(y))

@@ -231,6 +231,16 @@ int bicg_solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, 
 int bicg_solve_async_prepare(bicg_matrix *m, int method) { return solve_async_prepare(m, method); }
 int bicg_matrix_history(bicg_matrix *m, double *out, int cap) { return matrix_history(m, out, cap); }
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_host(m, x_loc, y_loc, nullptr); }
+int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                         int device_vectors)
+{
+    return matrix_multiply(m, nvec, x, y, alpha, beta, sigma, device_vectors != 0);
+}
+int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                               void *stream)
+{
+    return matrix_multiply_async(m, nvec, x, y, alpha, beta, sigma, (cudaStream_t)stream);
+}
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();

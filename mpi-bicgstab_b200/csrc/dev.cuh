@@ -280,6 +280,41 @@ __device__ __forceinline__ double row_product(Value value, Column column, const 
     return lanes_sum<LANES>(acc);
 }
 
+// row_product for NV vectors at once (the batched multiply, spmv.cu): entry idx is read once and multiplied with x[v][col]
+// for every v, so UNR * NV gathers are in flight per thread.  Per vector the order is row_product's -- entries in storage
+// order, one fma each, then lanes_sum -- and UNR only decides how many entries one pass loads, so acc[v] is bit-identical to
+// row_product(value, column, x[v], j, e) whatever UNR and NV are.
+template <int LANES, int UNR, int NV, class Value, class Column>
+__device__ __forceinline__ void row_products(Value value, Column column, const double *const (&x)[NV], int j, int e,
+                                             double (&acc)[NV])
+{
+#pragma unroll
+    for (int v = 0; v < NV; ++v) acc[v] = 0.0;
+    while (j < e) {
+        unsigned c[UNR];
+        double a[UNR];
+        double xv[NV][UNR];
+#pragma unroll
+        for (int u = 0; u < UNR; ++u) {
+            const int idx = min(j + u * LANES, e - 1);
+            c[u] = column(idx);
+            a[u] = value(idx);
+        }
+#pragma unroll
+        for (int v = 0; v < NV; ++v)
+#pragma unroll
+            for (int u = 0; u < UNR; ++u) xv[v][u] = ld_coherent(x[v] + c[u]);
+#pragma unroll
+        for (int v = 0; v < NV; ++v)
+#pragma unroll
+            for (int u = 0; u < UNR; ++u)
+                if (j + u * LANES < e) acc[v] = fma(a[u], xv[v][u], acc[v]);
+        j += UNR * LANES;
+    }
+#pragma unroll
+    for (int v = 0; v < NV; ++v) acc[v] = lanes_sum<LANES>(acc[v]);
+}
+
 // Sum N per-thread values over the CTA.  Result is valid in every lane of warp 0.  `scratch` holds
 // 32 * N doubles.  Fixed combination order -> deterministic.
 template <int N>

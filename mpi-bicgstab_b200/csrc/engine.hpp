@@ -326,6 +326,14 @@ int  shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const d
 std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
 // ... as ||(A + sigma_j I) x_j - b|| / ||b||
 std::vector<double> shift_relative_errors(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
+// an empty cross-GPU reduction on st: every rank has finished what it enqueued on the handle before (with peers only)
+void peer_barrier(bicg_matrix *m, cudaStream_t st);
+// multiply.cu: bicg_matrix_multiply (device_vectors: x, y are device pointers; sigma is a host array) and
+// bicg_matrix_multiply_async (x, y and sigma device pointers, on st)
+int  matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                     bool device_vectors);
+int  matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                           cudaStream_t st);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class = 0);

@@ -1,0 +1,130 @@
+// multiply.cu -- y_j = alpha (A + sigma_j I) x_j + beta y_j, j < nvec, on a resident matrix: bicg_matrix_multiply (synchronous,
+// host or device vectors) and bicg_matrix_multiply_async (device vectors, on the caller's stream, capturable).
+//
+// The work is the batched SpMV of spmv.cu on the handle's SpMV plan: a launch takes up to MUL_NV_MAX vectors and streams
+// the matrix once for all of them, so every row sum is the one bicg_spmv computes for that vector alone.  At one rank the
+// kernels gather straight from the caller's x_j and write straight into y_j.  With peers the ghost columns of x_j come from
+// the ghost tail of an arena vector (MUL_SLOT[k], the slots of shift_check.cu): the owner copies x_j's own rows into that
+// vector, so the kernel reads one extended vector, and pushes the boundary runs into the same slot on its neighbours.  Each
+// launch then ends in an empty cross-GPU reduction, so no rank pushes the next batch into a slot a peer is still reading.
+#include "engine.hpp"
+
+#include <algorithm>
+#include <cstdint>
+
+namespace bicg {
+
+namespace {
+
+// arena vectors whose ghost tails carry a batch's halo with peers (never V_R: a shifted solve returns its seed residual there)
+constexpr int MUL_SLOT[MUL_NV_MAX] = {V_X, V_RH, V_P, V_S, V_Y, V_W, V_V, V_T};
+
+// the checks both calls make before the device is touched: -1 cases of include/bicgstab_b200.h
+bool bad_args(const bicg_matrix *m, int nvec, const double *x, const double *y)
+{
+    if (!m || !x || !y || nvec <= 0) return true;
+    // a gather SpMV cannot run in place; x == y counts as overlapping even without rows
+    const uintptr_t bytes = std::max<uintptr_t>((uintptr_t)nvec * (uintptr_t)m->n_loc * sizeof(double), sizeof(double));
+    const uintptr_t x0 = (uintptr_t)x, y0 = (uintptr_t)y;
+    return x0 < y0 + bytes && y0 < x0 + bytes;
+}
+
+// every batch of one multiply on st: x, y device pointers, sigma nvec device values or null
+void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                      cudaStream_t st)
+{
+    const SpmvPlan &p = m->plan;
+    const bool peers = m->world > 1;
+    const long long n = m->n_loc;
+    PhaseLauncher pl(m, st);
+    MultiplyArgs a{};
+    a.kc = pl.common(peers ? tail_allreduce(FIN_NONE, 0) : tail_none());
+    a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
+    a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
+    a.alpha = alpha; a.beta = beta;
+    a.wait_halo = (peers && m->comm.recv_mask != 0) ? 1 : 0;
+    const size_t smem = p.kind == 0 ? multiply_tma_smem_bytes(p.cap, p.stages, p.threads, p.lanes) : 0;
+    if (peers) {
+        // the halo push returns at once while `done` is set (as a finished solve leaves it); then wait until the peers are
+        // done with the slots' ghost tails
+        BICG_CUDA(cudaMemsetAsync(&m->d_sc->done, 0, sizeof(int), st));
+        peer_barrier(m, st);
+    }
+    for (int j0 = 0; j0 < nvec; j0 += MUL_NV_MAX) {
+        const int nv = std::min(MUL_NV_MAX, nvec - j0);
+        a.nv = nv;
+        a.sigma = sigma ? sigma + j0 : nullptr;
+        for (int v = 0; v < MUL_NV_MAX; ++v) {
+            const int k = std::min(v, nv - 1);
+            a.x[v] = peers ? m->vec(MUL_SLOT[k]) : x + (j0 + k) * n;
+            a.y[v] = y + (j0 + k) * n;
+        }
+        if (peers) {
+            for (int k = 0; k < nv; ++k) {
+                const double *xk = x + (j0 + k) * n;
+                BICG_CUDA(cudaMemcpyAsync(m->vec(MUL_SLOT[k]), xk, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+                pl.vec(PH_PUSH, tail_none(), MUL_SLOT[k], xk);
+            }
+        }
+        const int rc = launch_multiply(p.kind, p.lanes, p.threads, p.grid, smem, multiply_nv(nv), a, st);
+        if (rc) fatal("bicgstab_b200: multiply launch failed (kind %d lanes %d threads %d grid %d vectors %d): %s", p.kind, p.lanes,
+                      p.threads, p.grid, nv, cudaGetErrorString((cudaError_t)rc));
+        ++ctx().launches;
+    }
+}
+
+} // namespace
+
+int matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                    bool device_vectors)
+{
+    Context &c = ctx();
+    // collective: a rank with bad arguments must not leave the others waiting for it in the halo exchange and the barrier, so
+    // every rank learns every rank's verdict, nvec and whether it passed sigma before any of them starts
+    struct Args { int bad, nvec, shifted; } mine{bad_args(m, nvec, x, y) ? 1 : 0, nvec, sigma ? 1 : 0};
+    std::vector<Args> all((size_t)c.world);
+    c.host_allgather(&mine, all.data(), sizeof(Args));
+    for (const Args &o : all)
+        if (o.bad || o.nvec != nvec || o.shifted != mine.shifted) return -1;
+    c.ensure();
+    wait_handle(m);
+    const size_t bytes = (size_t)nvec * (size_t)m->n_loc * sizeof(double);
+    const double *dx = x;
+    double *dy = y, *tmp = nullptr, *d_sigma = nullptr;
+    if (!device_vectors) {
+        tmp = (double *)c.dev_alloc(2 * bytes);
+        dx = tmp; dy = tmp + bytes / sizeof(double);
+        c.h2d(tmp, x, bytes);
+        if (beta != 0.0) c.h2d(dy, y, bytes);
+    }
+    if (sigma) {
+        d_sigma = (double *)c.dev_alloc((size_t)nvec * sizeof(double));
+        BICG_CUDA(cudaMemcpyAsync(d_sigma, sigma, (size_t)nvec * sizeof(double), cudaMemcpyHostToDevice, c.stream));
+    }
+    enqueue_multiply(m, nvec, dx, dy, alpha, beta, d_sigma, c.stream);
+    if (!device_vectors) BICG_CUDA(cudaMemcpyAsync(y, dy, bytes, cudaMemcpyDeviceToHost, c.stream));
+    int error = 0;
+    BICG_CUDA(cudaMemcpyAsync(&error, &m->d_sc->error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    if (error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU during a multiply", m->rank);
+    c.dev_free(tmp); c.dev_free(d_sigma);
+    return 0;
+}
+
+int matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                          cudaStream_t st)
+{
+    if (bad_args(m, nvec, x, y)) return -1;
+    Context &c = ctx();
+    c.ensure();
+    cudaStreamCaptureStatus cs;
+    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
+    const bool captured = cs != cudaStreamCaptureStatusNone;
+    async_handle_init(m);
+    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    enqueue_multiply(m, nvec, x, y, alpha, beta, sigma, st);
+    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    return 0;
+}
+
+} // namespace bicg

@@ -141,6 +141,13 @@ __global__ void shift_barrier_kernel(const __grid_constant__ KernelCommon kc)
 
 } // namespace
 
+void peer_barrier(bicg_matrix *m, cudaStream_t st)
+{
+    PhaseLauncher pl(m, st);
+    shift_barrier_kernel<<<1, 32, 0, st>>>(pl.common(tail_allreduce(FIN_NONE, 0)));
+    BICG_CUDA(cudaGetLastError());
+}
+
 std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L)
 {
     Context &c = ctx();
@@ -169,8 +176,7 @@ std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long 
     for (int k = 0; k < SC_B; ++k) a.ghost[k] = m->vec(SC_SLOT[k]);
     if (peers) {
         reset_scalars(m, c.cfg.tol, c.cfg.max_iter);          // clears `done`, which every launcher kernel tests first
-        shift_barrier_kernel<<<1, 32, 0, c.stream>>>(a.kc);    // the peers are done with the slots' ghost tails
-        BICG_CUDA(cudaGetLastError());
+        peer_barrier(m, c.stream);                            // the peers are done with the slots' ghost tails
     }
     for (int j0 = 0; j0 < L; j0 += nj_max) {
         a.j0 = j0; a.nj = std::min(nj_max, L - j0); a.with_b = j0 == 0;
