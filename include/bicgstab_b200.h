@@ -194,6 +194,37 @@ int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double 
 int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream);
 int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma);
 
+/* A^T of a resident matrix as a handle of its own: for adjoint systems A^T lambda = g (the gradient of an objective of the
+ * solution of A x = b, the backward of a differentiable solve), two-sided Krylov methods and the normal equations.
+ *
+ * bicg_matrix_create_transpose: same global size and row partition as m (its recvcounts / displs, under BICG_PARTITION=nnz
+ * too), with its own plans, arena and halo.  Pattern: row j of A^T holds the entries (i, j) of A by ascending i; entries with
+ * equal (i, j) keep their order in row i of A; duplicates and explicit zeros are kept; within a row, as for any handle, diag
+ * columns come first, then offd columns.  So every result on it (spmv, multiply, every solve and shifted solve, histories and
+ * stats apart from timings) is bit-identical to that of bicg_matrix_create on the blocks of the global CSR of A^T built by a
+ * stable sort of A's global triplets by (column, row).  Once created it is independent of m: destroying m leaves it working,
+ * and bicg_matrix_set_values on it takes its own block order.  Setup work, collective over the ranks like bicg_matrix_create
+ * (the entries whose column another rank owns travel through the host allgather once).  Returns null for a null m, on every
+ * rank if any rank passed one.
+ *
+ * bicg_matrix_transpose_values: mt's values become those of bicg_matrix_create_transpose(src) for src as it is at that point,
+ * where src must be the handle mt was created from; the pattern is not rebuilt, only the values are copied on the device and
+ * the persistent kernel's value tables rebuilt, as bicg_matrix_set_values does.  Returns 0, or -1 for a null mt or src or an
+ * src that is not mt's source (then nothing is touched).  The synchronous call waits for both handles' earlier asynchronous
+ * work, checks its arguments on every rank (every rank returns -1 if any rank's are bad) and returns once done; a peer timeout
+ * is fatal.  bicg_matrix_transpose_values_async runs on the caller's CUDA stream behind both handles' earlier work, and both
+ * handles' next work waits for it: no host synchronisation, allocation, pageable copy or output, no prepare step (there is no
+ * -2), and it works inside a stream capture, where a replay reads src's values as they are then.  It checks its arguments
+ * locally; a peer timeout is reported by the next synchronous call on mt.  Both are collective: with peers, each rank first
+ * stores the values other ranks' rows of A^T need into their receive regions, between two empty cross-GPU reductions.
+ *
+ * bicg_matrix_block_nz: the entries of the diag and offd blocks of this rank's rows of a handle (offd is 0 with one rank),
+ * which bicg_matrix_set_values takes; for a transpose these are not otherwise known to the caller.  -1 for a null argument. */
+bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m);
+int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src);
+int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream);
+int bicg_matrix_block_nz(const bicg_matrix *m, unsigned *diag_nz, unsigned *offd_nz);
+
 enum { BICG_METHOD_BICGSTAB = 0, BICG_METHOD_CA = 1, BICG_METHOD_PIPE = 2, BICG_METHOD_PIPE_RR = 3 };
 
 typedef struct {

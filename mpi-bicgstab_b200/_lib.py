@@ -87,6 +87,10 @@ SYMBOLS = {
     "bicg_matrix_multiply_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                              C.c_void_p]),
     "bicg_matrix_shift_diagonal": (C.c_int, [C.c_void_p, C.c_double]),
+    "bicg_matrix_create_transpose": (C.c_void_p, [C.c_void_p]),
+    "bicg_matrix_transpose_values": (C.c_int, [C.c_void_p, C.c_void_p]),
+    "bicg_matrix_transpose_values_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bicg_matrix_block_nz": (C.c_int, [C.c_void_p, _P(C.c_uint), _P(C.c_uint)]),
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "bicg_solve_async_prepare": (C.c_int, [C.c_void_p, C.c_int]),

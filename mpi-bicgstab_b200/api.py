@@ -403,14 +403,65 @@ def last_stats():
     return _stats_dict(lib.bicg_last_stats().contents)
 
 
+class _CountBlock:
+    def __init__(self, nz):
+        self.nz = nz
+
+
+class _HandleShape:
+    """What a DeviceMatrix needs of its MatrixBlock, for a handle the library built (a transpose): no host arrays."""
+
+    def __init__(self, n_loc, n, diag_nz, offd_nz):
+        self.n_loc, self.n = n_loc, n
+        self.diag, self.offd = _CountBlock(diag_nz), _CountBlock(offd_nz)
+
+
 class DeviceMatrix:
     """A device-resident matrix handle (bicg_matrix): upload once, solve / multiply many times."""
 
-    def __init__(self, blk):
+    def __init__(self, blk, handle=None):
+        """blk: the MatrixBlock to upload; or, with `handle`, an existing bicg_matrix that this object takes over (then blk only
+        describes its shape: n_loc, n and the diag.nz / offd.nz that set_values takes)."""
         self.blk = blk
-        self.h = lib.bicg_matrix_create(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info))
+        self.h = handle if handle is not None else lib.bicg_matrix_create(C.byref(blk.diag), C.byref(blk.offd), C.byref(blk.info))
         if not self.h:
             raise RuntimeError("bicg_matrix_create failed")
+
+    def transpose(self):
+        """bicg_matrix_create_transpose: a new DeviceMatrix holding A^T with this handle's row partition, its own plans and
+        arena, independent of this one once created.  Row j holds the entries (i, j) of A by ascending i (equal (i, j) in
+        their order in row i of A), diag columns first: results are bit-identical to a DeviceMatrix on
+        blocks_from_csr of that global CSR.  Collective over the ranks."""
+        h = lib.bicg_matrix_create_transpose(self.h)
+        if not h:
+            raise RuntimeError("bicg_matrix_create_transpose failed")
+        dnz, onz = C.c_uint(), C.c_uint()
+        lib.bicg_matrix_block_nz(h, C.byref(dnz), C.byref(onz))
+        return DeviceMatrix(_HandleShape(self.blk.n_loc, self.blk.n, dnz.value, onz.value), handle=h)
+
+    def transpose_values(self, src):
+        """bicg_matrix_transpose_values: this transpose's values become src^T for src's current values, where src is the
+        DeviceMatrix it was made from.  Returns once done.  Collective over the ranks."""
+        if not isinstance(src, DeviceMatrix):
+            raise TypeError(f"src: need a DeviceMatrix, got {type(src).__name__}")
+        rc = lib.bicg_matrix_transpose_values(self.h, src.h)
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_transpose_values failed with {rc} (src is not the matrix this one was transposed from)")
+
+    def transpose_values_async(self, src, stream=None):
+        """bicg_matrix_transpose_values_async: transpose_values enqueued on `stream` (default: torch's current stream) behind both
+        handles' earlier work, and both handles' next work waits for it; no host synchronisation.  src's values are read in
+        stream order, so a replay of a captured refresh reads them as they are then; works inside torch.cuda.graph with no
+        prepare step.  Collective over the ranks."""
+        import torch
+        if not isinstance(src, DeviceMatrix):
+            raise TypeError(f"src: need a DeviceMatrix, got {type(src).__name__}")
+        if stream is None:
+            stream = torch.cuda.current_stream(torch.device("cuda", lib.bicg_device()))
+        rc = lib.bicg_matrix_transpose_values_async(self.h, src.h, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_transpose_values_async failed with {rc} (src is not the matrix this one was transposed "
+                             f"from)")
 
     def set_values(self, diag_val, offd_val=None):
         """bicg_matrix_set_values: new values for the pattern the handle was created with, in the order of blk's diag and offd

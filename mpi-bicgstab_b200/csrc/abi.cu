@@ -219,6 +219,19 @@ int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const d
     return matrix_set_values(m, diag_val, offd_val, true, true, (cudaStream_t)stream);
 }
 int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma) { return matrix_shift_diagonal(m, sigma); }
+bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m) { return matrix_create_transpose(m); }
+int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src) { return matrix_transpose_values(mt, src, false, nullptr); }
+int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream)
+{
+    return matrix_transpose_values(mt, src, true, (cudaStream_t)stream);
+}
+int bicg_matrix_block_nz(const bicg_matrix *m, unsigned *diag_nz, unsigned *offd_nz)
+{
+    if (!m || !diag_nz || !offd_nz) return -1;
+    *diag_nz = (unsigned)(m->nnz - m->nnz_offd);
+    *offd_nz = (unsigned)m->nnz_offd;
+    return 0;
+}
 
 int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *stats)
 {

@@ -189,6 +189,8 @@ struct ShiftWork {
 };
 // where the last asynchronous shifted solve on a handle left its history (device memory, written by its result kernel)
 struct ShiftHistRef { const double *hist; int n, pad; };
+// one value a transpose refresh pushes to a peer: the source's d_val[src] into slot `slot` of rank `rank`'s receive region
+struct TransposePush { int src, rank, slot; };
 
 } // namespace bicg
 
@@ -265,20 +267,40 @@ struct bicg_matrix {
     bicg::ShiftWork shift_ws[2];
     std::vector<void *> shift_retired;
     bicg::ShiftHistRef *d_shift_last = nullptr;
+    // identity of the handle (never reused in a process): what a transpose records as its source
+    unsigned long long uid = 0;
+    // a handle made by bicg_matrix_create_transpose (transpose.cu): the source's uid; for every entry of d_val the position
+    // in the source's d_val it is copied from (>= 0) or ~slot of the receive region (< 0); the source's entries that other
+    // ranks hold in their transposes, pushed by a refresh into those ranks' receive regions; and this rank's receive region
+    // in the arena (t_nrecv doubles) with every peer's, as mapped here
+    unsigned long long t_src_uid = 0;
+    int *d_tperm = nullptr;
+    bicg::TransposePush *d_tpush = nullptr;
+    int t_npush = 0;
+    double *d_trecv = nullptr;
+    size_t t_nrecv = 0;
+    double *peer_trecv[bicg::MAX_RANKS] = {};
 
     double *vec(int id) const { return vec_base + (long long)id * vstride; }
 };
 
 namespace bicg {
 
-// matrix.cu
-bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info);
+// matrix.cu.  recv_doubles > 0: the arena also holds a region of that many doubles that the peers can store into (the receive
+// region of a transpose, transpose.cu), at m->d_trecv, and m->peer_trecv[p] is rank p's
+bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, size_t recv_doubles = 0);
 void matrix_destroy(bicg_matrix *m);
 double matrix_upload_ms(bicg_matrix *m);
 bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, bool *fresh);
 // bicg_matrix_set_values (async = false: on the library's stream, returns once done) and bicg_matrix_set_values_async (on st)
 int  matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st);
 int  matrix_shift_diagonal(bicg_matrix *m, double sigma);     // bicg_matrix_shift_diagonal
+// the persistent kernel's value tables and packed values from d_val, on st: what creation and every value update run last
+void launch_value_tables(const bicg_matrix *m, cudaStream_t st);
+// transpose.cu: bicg_matrix_create_transpose, bicg_matrix_transpose_values (async = false: on the library's stream, returns
+// once done) and bicg_matrix_transpose_values_async (on st)
+bicg_matrix *matrix_create_transpose(bicg_matrix *m);
+int  matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src, bool async, cudaStream_t st);
 // solve.cu
 int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *st);
 // bicg_solve_async / bicg_solve_async_prepare / bicg_matrix_history (include/bicgstab_b200.h)

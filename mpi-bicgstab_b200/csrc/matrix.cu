@@ -493,7 +493,7 @@ static int mega_lanes_for(double mean_row)
 
 // The value tables and packed values of the persistent kernel's plan (mega.cu: mega_value_kernel) from d_val, on `st`.  The
 // plan's creation and every value update run this same pass, so an updated handle holds what a fresh one would.
-static void launch_value_tables(const bicg_matrix *m, cudaStream_t st)
+void launch_value_tables(const bicg_matrix *m, cudaStream_t st)
 {
     const MegaPlan &mp = m->mega;
     if (!mp.d_vtab) return;
@@ -682,7 +682,7 @@ constexpr int INLINE_RUNS = 48;      // receive runs that travel inside the boot
 struct ArenaHdr {
     cudaIpcMemHandle_t handle;
     unsigned long long arena_id;
-    long long vec_off, vstride, ghost_off, mail_off, hflag_off, msync_off, ll_off, ll_stride;
+    long long vec_off, vstride, ghost_off, mail_off, hflag_off, msync_off, ll_off, ll_stride, trecv_off;
     int n_loc, n_ghost, n_runs, pad_;
     int runs[4 * INLINE_RUNS];
 };
@@ -693,8 +693,9 @@ static double now_ms()
     return 1e3 * (double)ts.tv_sec + 1e-6 * (double)ts.tv_nsec;
 }
 
-bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info)
+bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, size_t recv_doubles)
 {
+    static unsigned long long next_uid = 0;
     Context &c = ctx();
     c.ensure();
     const double t_begin = now_ms();
@@ -716,6 +717,7 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
 
     bicg_matrix *m = new bicg_matrix();
     m->rank = c.rank; m->world = c.world;
+    m->uid = ++next_uid;
     m->n_loc = (int)diag->rows; m->n_glob = (int)info->rows;
     const size_t nd = diag->nz, no = (offd && m->world > 1) ? offd->nz : 0;
     m->nnz = nd + no;
@@ -755,6 +757,7 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
     const size_t ll_stride = (size_t)round_up(std::max(m->n_ghost, 1), 16);
     const bool want_ll = m->world > 1 && (c.cfg.mega == 2 || c.cfg.mega_lanes > 0 || mega_lanes_for(m->mean_row) == 1);
     const size_t ll_off = off;    off = align(off + (want_ll ? (size_t)LL_REGIONS * ll_stride * 16 : 0));
+    const size_t trecv_off = off; off = align(off + recv_doubles * sizeof(double));
     m->arena_bytes = std::max<size_t>(off, (size_t)4 << 20);     // its own allocation granule: the IPC handle maps exactly this
     if (m->world > 1) {
         // exported through CUDA IPC: an allocation of its own (peers map exactly this one), parked and re-used by size
@@ -780,6 +783,8 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
     m->d_msync = (MegaSync *)(m->arena + msync_off);
     m->d_ll = want_ll ? (unsigned long long *)(m->arena + ll_off) : nullptr;
     m->ll_stride = (long long)ll_stride;
+    m->t_nrecv = recv_doubles;
+    m->d_trecv = recv_doubles ? (double *)(m->arena + trecv_off) : nullptr;
     BICG_CUDA(cudaStreamSynchronize(c.stream));            // arena zeroed before any peer may write into it
 
     lap("arena alloc + zero");
@@ -842,6 +847,7 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
         mine.vec_off = (long long)vec_off; mine.vstride = m->vstride; mine.ghost_off = m->ghost_off;
         mine.mail_off = (long long)mail_off; mine.hflag_off = (long long)hflag_off; mine.msync_off = (long long)msync_off;
         mine.ll_off = want_ll ? (long long)ll_off : -1; mine.ll_stride = (long long)ll_stride;
+        mine.trecv_off = recv_doubles ? (long long)trecv_off : -1;
         mine.n_loc = m->n_loc; mine.n_ghost = m->n_ghost;
         const int my_cnt = (int)(m->recv_runs.size() / 4);
         mine.n_runs = my_cnt;
@@ -867,6 +873,7 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
             m->peer_msync[p] = (MegaSync *)((char *)m->peer_base[p] + all[(size_t)p].msync_off);
             m->peer_ll[p] = all[(size_t)p].ll_off >= 0 ? (unsigned long long *)((char *)m->peer_base[p] + all[(size_t)p].ll_off) : nullptr;
             m->peer_ll_stride[p] = all[(size_t)p].ll_stride;
+            m->peer_trecv[p] = all[(size_t)p].trecv_off >= 0 ? (double *)((char *)m->peer_base[p] + all[(size_t)p].trecv_off) : nullptr;
         }
         // receive lists of every rank: inline in the header, or (irregular matrices with many runs) a second round
         std::vector<int> cnts((size_t)m->world);
@@ -978,6 +985,7 @@ void matrix_destroy(bicg_matrix *m)
     if (m->hist_extra) cudaFree(m->hist_extra);
     c.dev_free(m->d_val); c.dev_free(m->d_col); c.dev_free(m->d_ptr);
     c.dev_free(m->d_blk_ptr); c.dev_free(m->d_diag_pos);
+    c.dev_free(m->d_tperm); c.dev_free(m->d_tpush);
     if (m->world > 1) c.arena_pool.emplace(m->arena_bytes, Context::ArenaRec{m->arena, m->arena_bytes, m->arena_id, m->arena_handle});
     else c.dev_free(m->arena);
     delete m;
