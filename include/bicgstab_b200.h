@@ -405,6 +405,40 @@ int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, d
 int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
                                const double *sigma, void *stream);
 
+/* The gradient with respect to the stored values of a resident matrix: for x_j = A^-1 b_j and a loss L, with
+ * lambda_j = A^-T dL/dx_j (a solve on the handle of bicg_matrix_create_transpose), dL/da_e = -sum_j lambda_j[i] x_j[c] for every
+ * stored entry e = (i, c); for y_j = A x_j, dL/da_e = sum_j (dL/dy_j)[i] x_j[c].  Both are this sampled outer product over the
+ * pattern.  u (row factors) and v (column factors) are nvec contiguous blocks of n_loc doubles each (the x_set layout of
+ * bicg_matrix_multiply); one pass over the pattern serves up to 8 vectors (csrc/value_grad.cu).
+ *
+ * Arithmetic, per stored entry e of this rank's rows at local row i and column c (own or ghost), for one batch of vectors
+ * j0 .. j0 + nb - 1 (batches of up to 8, in order):
+ *   t = u_j0[i] * v_j0[c];  t = fma(u_j[i], v_j[c], t) for j = j0 + 1 .. j0 + nb - 1, in that order;
+ *   beta == 0: out_e = alpha * t, and out_e is not read (a NaN in it does not propagate); else out_e = fma(alpha, t, beta * out_e).
+ * Every batch after the first applies with beta = 1 onto the previous batch's output.  Each output element depends only on its
+ * own inputs, so the result does not depend on the launch shape, the SpMV plan or its lanes per row.
+ *
+ * Order: diag_out[j] belongs to diag entry j of the blocks the handle was created from, and offd_out[j] to offd entry j: the
+ * order bicg_matrix_set_values takes, so set_values(diag - eta g_diag, offd - eta g_offd) is a gradient step.  A transpose's
+ * order is its own (bicg_matrix_block_nz gives its counts).  offd_out may be null when the handle has no offd entries (always
+ * with one rank).  Returns 0, or -1 for a null handle, u, v or diag_out, nvec <= 0, a null offd_out on a handle with offd
+ * entries, or an output range overlapping u's or v's; these are checked before the device is touched.
+ *
+ * bicg_matrix_value_grad: u, v, diag_out and offd_out are host pointers, or device pointers when device_vectors != 0.  Waits
+ * for the handle's earlier asynchronous work and returns once the outputs are in the caller's buffers.
+ * bicg_matrix_value_grad_async: device pointers, read and written in stream order on the caller's CUDA stream `stream` behind
+ * the handle's previous work, with the ordering of bicg_solve_async: no host synchronisation, allocation, pageable copy or
+ * output.  It needs no prepare step and works inside a stream capture as it is (there is no -2).
+ *
+ * Collective when there are peers: the ghost columns of every v_j come from the neighbours, and every batch ends in an empty
+ * cross-GPU reduction.  The synchronous call checks its arguments on every rank first: every rank returns -1 if any rank's
+ * arguments are bad or the ranks disagree on nvec; a peer timeout is fatal.  The asynchronous call checks its arguments
+ * locally, so the ranks must agree on nvec; a peer timeout there is reported by the next synchronous call on the handle. */
+int bicg_matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                           double *diag_out, double *offd_out, int device_vectors);
+int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                                 double *diag_out, double *offd_out, void *stream);
+
 /* Time `reps` launches of the fused SpMV + (r_hat, s) dot kernel (the dominant kernel of every
  * variant) with CUDA events on the library's stream; returns average ms per launch in *ms and the
  * algorithmic bytes of one launch (12 nnz + 28 n_loc, SURVEY.md 8(d) phase P1) in *bytes. */
@@ -433,7 +467,15 @@ int bicg_profile_solve(bicg_matrix *m, int method, int iters, int krr, int nrr, 
  *                         (a per-CTA sign / exponent table index + the 52 mantissa bits) instead of 8-byte values (csrc/mega.cu).
  *   bicg_debug_stream_values: on = 0 makes every streaming CTA of later launches on this handle stream 8-byte values (the
  *                         column codes stay), on = 1 restores the default; returns the previous setting.  Both formats give
- *                         bit-identical results. */
+ *                         bit-identical results.
+ *   bicg_debug_value_grad_layout: later value gradients on this handle use `lanes` threads per row (1, 2, 4, ..., 32; 0: the
+ *                         library's choice), and, when blk_ptr is not null, take the merged rows as split into diag and offd
+ *                         parts by the device array blk_ptr = [diag row pointers | offd row pointers] (2 (n_loc + 1)
+ *                         unsigned, diag_ptr[i] + offd_ptr[i] = the merged row start), writing diag_out and offd_out in
+ *                         that order, as a handle with offd entries does (null: the handle's own order; device-pointer calls
+ *                         only).  blk_ptr must stay
+ *                         valid while it is set, and is refused (-1) on a handle with offd entries; -1 also for a null handle
+ *                         or a bad lanes. */
 int bicg_debug_vec_phase(bicg_matrix *m, int phase, const double coef[3], double *vecs, double dots[8]);
 int bicg_debug_spmv_epi(bicg_matrix *m, int epi, double *vecs, double dots[8]);
 int bicg_debug_get_vec(bicg_matrix *m, int id, double *out);
@@ -443,6 +485,7 @@ int bicg_debug_coded_ctas(bicg_matrix *m);
 int bicg_debug_stream_codes(bicg_matrix *m, int on);
 int bicg_debug_packed_ctas(bicg_matrix *m);
 int bicg_debug_stream_values(bicg_matrix *m, int on);
+int bicg_debug_value_grad_layout(bicg_matrix *m, int lanes, const unsigned *blk_ptr);
 
 /* full-precision history of the last solve on this rank: out[k] = dot_r/dot_zero after iteration k
  * (out[0] = 1).  Returns the number of entries available (iters + 1). */

@@ -13,3 +13,13 @@ from .api import (METHODS, GEN_KINDS, MatrixBlock, DeviceMatrix, blocks_from_csr
                   shifted_lopbicgstab, shifted_pipe_lopbicgstab, last_shift_info, last_shift_error, set_option, set_options, last_history, last_stats, comm_init,
                   comm_init_torch, comm_finalize)
 from ._lib import lib, CSR_Matrix, INFO_Matrix, bicg_stats, SYMBOLS, LIB_PATH
+
+# the differentiable entry points need torch, which importing the package does not: autograd.py is loaded on first use
+_AUTOGRAD = ("solve_autograd", "multiply_autograd", "SolveFunction", "MultiplyFunction")
+
+
+def __getattr__(name):
+    if name in _AUTOGRAD:
+        from . import autograd
+        return getattr(autograd, name)
+    raise AttributeError(f"module {__name__!r} has no attribute {name!r}")

@@ -86,6 +86,10 @@ SYMBOLS = {
                                        C.c_int]),
     "bicg_matrix_multiply_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                              C.c_void_p]),
+    "bicg_matrix_value_grad": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
+                                         C.c_void_p, C.c_int]),
+    "bicg_matrix_value_grad_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
+                                               C.c_void_p, C.c_void_p]),
     "bicg_matrix_shift_diagonal": (C.c_int, [C.c_void_p, C.c_double]),
     "bicg_matrix_create_transpose": (C.c_void_p, [C.c_void_p]),
     "bicg_matrix_transpose_values": (C.c_int, [C.c_void_p, C.c_void_p]),
@@ -117,6 +121,7 @@ SYMBOLS = {
     "bicg_debug_stream_codes": (C.c_int, [C.c_void_p, C.c_int]),
     "bicg_debug_packed_ctas": (C.c_int, [C.c_void_p]),
     "bicg_debug_stream_values": (C.c_int, [C.c_void_p, C.c_int]),
+    "bicg_debug_value_grad_layout": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p]),
     "bicg_last_history": (C.c_int, [_P(C.c_double), C.c_int]),
     "bicg_last_stats": (_P(bicg_stats), []),
     "bicg_stream": (C.c_void_p, []),

@@ -419,6 +419,8 @@ class _HandleShape:
 class DeviceMatrix:
     """A device-resident matrix handle (bicg_matrix): upload once, solve / multiply many times."""
 
+    _t = None                  # the transpose prepare_autograd made (or the first backward that needed one)
+
     def __init__(self, blk, handle=None):
         """blk: the MatrixBlock to upload; or, with `handle`, an existing bicg_matrix that this object takes over (then blk only
         describes its shape: n_loc, n and the diag.nz / offd.nz that set_values takes)."""
@@ -695,6 +697,94 @@ class DeviceMatrix:
             raise ValueError(f"bicg_matrix_multiply_async failed with {rc}")
         return y
 
+    def _has_offd(self):
+        """whether the handle holds offd entries (with one rank the offd block is ignored)"""
+        return int(self.blk.offd.nz) > 0 and lib.bicg_comm_world() > 1
+
+    def _grad_outputs(self, u, beta, diag_out, offd_out):
+        """(name, array, expected shape) of value_grad's outputs: diag_out, and offd_out where the handle has offd entries or
+        one is given; allocated like u when None (then beta must be 0)"""
+        outs = [("diag_out", diag_out, (int(self.blk.diag.nz),))]
+        if offd_out is not None or self._has_offd():
+            outs.append(("offd_out", offd_out, (int(self.blk.offd.nz),)))
+        for k, (name, a, shape) in enumerate(outs):
+            if a is None:
+                if beta != 0.0:
+                    raise ValueError(f"{name}: needed when beta != 0")
+                if isinstance(u, np.ndarray):
+                    a = np.empty(shape)
+                elif hasattr(u, "new_empty"):
+                    a = u.new_empty(shape, dtype=u.dtype)
+                outs[k] = (name, a, shape)
+        return outs
+
+    def value_grad(self, u, v, alpha=1.0, beta=0.0, diag_out=None, offd_out=None):
+        """bicg_matrix_value_grad: for every stored entry e = (i, c) of this rank's rows, out_e = alpha sum_j u_j[i] v_j[c]
+        (+ beta out_e), in the block order set_values takes, so set_values(diag - eta g_diag, offd - eta g_offd) is a gradient
+        step (a transpose's own order for a transpose).  u and v are numpy float64 arrays or contiguous CUDA float64 tensors of
+        shape (n_loc,) or (nvec, n_loc); the outputs have the same kind, diag.nz and offd.nz elements, and are allocated when None
+        (then beta must be 0).  With u = lambda = A^-T dL/dx, v = x and alpha = -1 this is dL/dA of a solve; with u = dL/dy,
+        v = x and alpha = 1 the one of y = A x.  Tensors are read after torch's current stream has been synchronised.
+        Collective over the ranks.  Returns (diag_out, offd_out); offd_out is None where the handle has no offd entries."""
+        shape = self._multiply_shape(u)
+        nvec = shape[0] if len(shape) == 2 else 1
+        outs = self._grad_outputs(u, beta, diag_out, offd_out)
+        args = [("u", u, shape), ("v", v, shape)] + outs
+        if all(isinstance(a, np.ndarray) for _, a, _ in args):
+            ptrs, dev = _checked_host_vectors(*args), 0
+        else:
+            ptrs, dev = _cuda_vectors(*args), 1
+        rc = lib.bicg_matrix_value_grad(self.h, nvec, ptrs[0], ptrs[1], float(alpha), float(beta), ptrs[2],
+                                        ptrs[3] if len(ptrs) > 3 else None, dev)
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_value_grad failed with {rc}")
+        return outs[0][1], (outs[1][1] if len(outs) > 1 else None)
+
+    def value_grad_async(self, u, v, alpha=1.0, beta=0.0, diag_out=None, offd_out=None, stream=None):
+        """bicg_matrix_value_grad_async: value_grad on contiguous CUDA float64 tensors only, enqueued on `stream` (default:
+        torch's current stream) behind the handle's earlier work, with no host synchronisation.  All are read and written in
+        stream order, so a replay of a captured call reads them as they are then; works inside torch.cuda.graph with no prepare
+        step.  Returns (diag_out, offd_out) as value_grad does."""
+        import torch
+        for name, t in (("u", u), ("v", v), ("diag_out", diag_out), ("offd_out", offd_out)):
+            if t is not None and not isinstance(t, torch.Tensor):
+                raise TypeError(f"{name}: value_grad_async takes CUDA tensors only, got {type(t).__name__}")
+        shape = self._multiply_shape(u)
+        nvec = shape[0] if len(shape) == 2 else 1
+        outs = self._grad_outputs(u, beta, diag_out, offd_out)
+        ptrs = _checked_cuda_vectors(("u", u, shape), ("v", v, shape), *outs)
+        if stream is None:
+            stream = torch.cuda.current_stream(u.device)
+        if stream != torch.cuda.current_stream(u.device):
+            for (name, t, _), given in zip(outs, (diag_out, offd_out)):
+                if given is None:
+                    t.record_stream(stream)       # written on `stream`, not on the one it was allocated on
+        rc = lib.bicg_matrix_value_grad_async(self.h, nvec, ptrs[0], ptrs[1], float(alpha), float(beta), ptrs[2],
+                                              ptrs[3] if len(ptrs) > 3 else None, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_value_grad_async failed with {rc}")
+        return outs[0][1], (outs[1][1] if len(outs) > 1 else None)
+
+    def prepare_autograd(self, method):
+        """What solve_autograd and multiply_autograd on this handle need inside torch.cuda.graph: creates and keeps this
+        handle's transpose (transpose(): host work, collective over the ranks) and runs prepare_async(method) on both handles.
+        Call it outside any capture.  destroy() destroys the transpose too."""
+        if self._t is None:
+            self._t = self.transpose()
+        self.prepare_async(method)
+        self._t.prepare_async(method)
+
+    def _adjoint(self):
+        """The transpose the backward of a differentiable solve or multiply runs on: the one prepare_autograd made, else created
+        here, which a stream capture cannot hold."""
+        if self._t is None:
+            import torch
+            if torch.cuda.is_current_stream_capturing():
+                raise RuntimeError("a backward through this DeviceMatrix inside a CUDA graph capture needs "
+                                   "dm.prepare_autograd(method) before the capture: creating the transpose is host work")
+            self._t = self.transpose()
+        return self._t
+
     def spmv(self, x_loc):
         y = np.empty(self.blk.n_loc)
         lib.bicg_spmv(self.h, _vec(x_loc, self.blk.n_loc), _dptr(y))
@@ -736,6 +826,9 @@ class DeviceMatrix:
         return list(ms), list(cnt)
 
     def destroy(self):
+        if self._t is not None:
+            self._t.destroy()
+            self._t = None
         if self.h:
             lib.bicg_matrix_destroy(self.h)
             self.h = None

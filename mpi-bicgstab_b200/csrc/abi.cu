@@ -254,6 +254,16 @@ int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double
 {
     return matrix_multiply_async(m, nvec, x, y, alpha, beta, sigma, (cudaStream_t)stream);
 }
+int bicg_matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                           double *diag_out, double *offd_out, int device_vectors)
+{
+    return matrix_value_grad(m, nvec, u, v, alpha, beta, diag_out, offd_out, device_vectors != 0);
+}
+int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                                 double *diag_out, double *offd_out, void *stream)
+{
+    return matrix_value_grad_async(m, nvec, u, v, alpha, beta, diag_out, offd_out, (cudaStream_t)stream);
+}
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();

@@ -232,6 +232,23 @@ __device__ __forceinline__ double lanes_sum(double v)
 }
 
 // ------------------------------------------------------------------------------------------------
+// the merged layout of a handle's rows (matrix.cu) against the diag / offd blocks it was created from
+// ------------------------------------------------------------------------------------------------
+// Where row i's entries land in the merged CSR: its diag entries first, then its offd entries (the reference's accumulation
+// order, matrix.c:437-440), so diag entry j is merged entry optr[i] + j and offd entry j is merged entry dptr[i + 1] + j.
+// diag(k, j): diag entry j is merged entry k; offd(k, j) likewise.  The merge of matrix_create, every value update and the
+// value gradient (value_grad.cu) place entries through this one function.  first / step: visit only the entries first,
+// first + step, ... of each block of the row (a group of step lanes sharing the row).
+template <class Diag, class Offd>
+__device__ __forceinline__ void merge_row(int i, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr, Diag diag,
+                                          Offd offd, unsigned first = 0, unsigned step = 1)
+{
+    const unsigned d0 = dptr[i], d1 = dptr[i + 1], o0 = optr[i], o1 = optr[i + 1];
+    for (unsigned j = d0 + first; j < d1; j += step) diag(o0 + j, j);
+    for (unsigned j = o0 + first; j < o1; j += step) offd(d1 + j, j);
+}
+
+// ------------------------------------------------------------------------------------------------
 // TMA-fed CSR SpMV: what the stand-alone spmv_ws_kernel (spmv.cu) and the persistent kernel (mega.cu) share
 // ------------------------------------------------------------------------------------------------
 constexpr int PROW_PAD = 8;       // extra ptr / epilogue slots per stage for the 16-byte alignment window

@@ -212,6 +212,10 @@ struct bicg_matrix {
     unsigned *d_blk_ptr = nullptr;
     int *d_diag_pos = nullptr;
     bool diag_missing = false;
+    // test hooks of the value gradient (bicg_debug_value_grad_layout): a forced group width per row (0: chosen) and, at one
+    // rank, caller-supplied diag / offd row pointers [2][n_loc + 1] that split every merged row (null: the handle's own order)
+    int vg_lanes = 0;
+    const unsigned *vg_blk_ptr = nullptr;
     bicg::SpmvPlan plan;
     bicg::MegaPlan mega;             // persistent-kernel plan (mega.cu)
     bicg::MegaSync *d_msync = nullptr;
@@ -356,6 +360,12 @@ int  matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, doubl
                      bool device_vectors);
 int  matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
                            cudaStream_t st);
+// value_grad.cu: bicg_matrix_value_grad (device_vectors: u, v, diag_out and offd_out are device pointers) and
+// bicg_matrix_value_grad_async (device pointers, on st)
+int  matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta, double *diag_out,
+                       double *offd_out, bool device_vectors);
+int  matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                             double *diag_out, double *offd_out, cudaStream_t st);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class = 0);
@@ -389,6 +399,23 @@ struct PhaseLauncher {
     void spmv(int x_id, int y_id, TailDesc tail, int ndot = 0, const double *a0 = nullptr, const double *b0 = nullptr,
               const double *a1 = nullptr, const double *b1 = nullptr, const double *a2 = nullptr, const double *b2 = nullptr,
               const double *a3 = nullptr, const double *b3 = nullptr);
+};
+
+// The halo staging of the batched kernels that gather vectors over the extended column space, up to MUL_NV_MAX per launch:
+// the multiply (multiply.cu) and the value gradient (value_grad.cu).  The constructor enqueues on st what precedes the first
+// batch: with peers, an empty cross-GPU reduction, after which no peer still reads the slots' ghost tails.  stage(x, j0, nv,
+// xs) sets xs[v] to x_{j0+v} (x: blocks of n_loc doubles; slots v >= nv repeat the last): the caller's vector at one rank;
+// with peers the arena vector MUL_SLOT[v], into which x_{j0+v}'s own rows are copied and whose boundary runs are pushed to the
+// neighbours.  Each batch's kernel then waits for the halo flags when wait_halo is set and ends with the tail of kc: with
+// peers an empty cross-GPU reduction, so no rank pushes the next batch into a slot a peer is still reading.
+struct HaloBatches {
+    bicg_matrix *m;
+    PhaseLauncher pl;
+    bool peers;
+    KernelCommon kc;
+    int wait_halo;
+    HaloBatches(bicg_matrix *m, cudaStream_t st);
+    void stage(const double *x, int j0, int nv, const double *(&xs)[MUL_NV_MAX]);
 };
 
 } // namespace bicg

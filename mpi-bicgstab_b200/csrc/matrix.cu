@@ -600,20 +600,7 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
 // ------------------------------------------------------------------------------------------------
 // device-side merge of the reference's diag / offd blocks (matrix.c:380-392) into one CSR over [own | ghost] columns
 // ------------------------------------------------------------------------------------------------
-// Where row i's entries land in the merged CSR: its diag entries first, then its offd entries (the reference's accumulation
-// order, matrix.c:437-440).  diag(k, j): diag entry j goes to merged entry k; offd(k, j) likewise.  The merge of
-// matrix_create and every value update place entries through this one function.
-template <class Diag, class Offd>
-__device__ __forceinline__ void merge_row(int i, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr, Diag diag,
-                                          Offd offd)
-{
-    const unsigned d0 = dptr[i], d1 = dptr[i + 1], o0 = optr[i], o1 = optr[i + 1];
-    unsigned k = d0 + o0;
-    for (unsigned j = d0; j < d1; ++j, ++k) diag(k, j);
-    for (unsigned j = o0; j < o1; ++j, ++k) offd(k, j);
-}
-
-// One thread per row; an offd entry's global column becomes ghost_off + ghost slot of the receive run that contains it.
+// merge_row (dev.cuh) places every entry.  One thread per row; an offd entry's global column becomes ghost_off + ghost slot of the receive run that contains it.
 __global__ void __launch_bounds__(256) merge_rows_kernel(int n_loc, const unsigned *__restrict__ dptr, const unsigned *__restrict__ optr,
                                                          const double *__restrict__ dval, const unsigned *__restrict__ dcol,
                                                          const double *__restrict__ oval, const unsigned *__restrict__ ocol,

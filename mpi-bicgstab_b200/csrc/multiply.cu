@@ -7,6 +7,7 @@
 // the ghost tail of an arena vector (MUL_SLOT[k], the slots of shift_check.cu): the owner copies x_j's own rows into that
 // vector, so the kernel reads one extended vector, and pushes the boundary runs into the same slot on its neighbours.  Each
 // launch then ends in an empty cross-GPU reduction, so no rank pushes the next batch into a slot a peer is still reading.
+// HaloBatches does this staging for the value gradient (value_grad.cu) too.
 #include "engine.hpp"
 
 #include <algorithm>
@@ -29,43 +30,57 @@ bool bad_args(const bicg_matrix *m, int nvec, const double *x, const double *y)
     return x0 < y0 + bytes && y0 < x0 + bytes;
 }
 
-// every batch of one multiply on st: x, y device pointers, sigma nvec device values or null
-void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                      cudaStream_t st)
+} // namespace
+
+HaloBatches::HaloBatches(bicg_matrix *mm, cudaStream_t st) : m(mm), pl(mm, st), peers(mm->world > 1)
 {
-    const SpmvPlan &p = m->plan;
-    const bool peers = m->world > 1;
-    const long long n = m->n_loc;
-    PhaseLauncher pl(m, st);
-    MultiplyArgs a{};
-    a.kc = pl.common(peers ? tail_allreduce(FIN_NONE, 0) : tail_none());
-    a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
-    a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
-    a.alpha = alpha; a.beta = beta;
-    a.wait_halo = (peers && m->comm.recv_mask != 0) ? 1 : 0;
-    const size_t smem = p.kind == 0 ? multiply_tma_smem_bytes(p.cap, p.stages, p.threads, p.lanes) : 0;
+    kc = pl.common(peers ? tail_allreduce(FIN_NONE, 0) : tail_none());
+    wait_halo = (peers && m->comm.recv_mask != 0) ? 1 : 0;
     if (peers) {
         // the halo push returns at once while `done` is set (as a finished solve leaves it); then wait until the peers are
         // done with the slots' ghost tails
         BICG_CUDA(cudaMemsetAsync(&m->d_sc->done, 0, sizeof(int), st));
         peer_barrier(m, st);
     }
+}
+
+void HaloBatches::stage(const double *x, int j0, int nv, const double *(&xs)[MUL_NV_MAX])
+{
+    const long long n = m->n_loc;
+    for (int v = 0; v < MUL_NV_MAX; ++v) {
+        const int k = std::min(v, nv - 1);
+        xs[v] = peers ? m->vec(MUL_SLOT[k]) : x + (j0 + k) * n;
+    }
+    if (!peers) return;
+    for (int k = 0; k < nv; ++k) {
+        const double *xk = x + (j0 + k) * n;
+        BICG_CUDA(cudaMemcpyAsync(m->vec(MUL_SLOT[k]), xk, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, pl.stream));
+        pl.vec(PH_PUSH, tail_none(), MUL_SLOT[k], xk);
+    }
+}
+
+namespace {
+
+// every batch of one multiply on st: x, y device pointers, sigma nvec device values or null
+void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
+                      cudaStream_t st)
+{
+    const SpmvPlan &p = m->plan;
+    const long long n = m->n_loc;
+    HaloBatches hb(m, st);
+    MultiplyArgs a{};
+    a.kc = hb.kc;
+    a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
+    a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
+    a.alpha = alpha; a.beta = beta;
+    a.wait_halo = hb.wait_halo;
+    const size_t smem = p.kind == 0 ? multiply_tma_smem_bytes(p.cap, p.stages, p.threads, p.lanes) : 0;
     for (int j0 = 0; j0 < nvec; j0 += MUL_NV_MAX) {
         const int nv = std::min(MUL_NV_MAX, nvec - j0);
         a.nv = nv;
         a.sigma = sigma ? sigma + j0 : nullptr;
-        for (int v = 0; v < MUL_NV_MAX; ++v) {
-            const int k = std::min(v, nv - 1);
-            a.x[v] = peers ? m->vec(MUL_SLOT[k]) : x + (j0 + k) * n;
-            a.y[v] = y + (j0 + k) * n;
-        }
-        if (peers) {
-            for (int k = 0; k < nv; ++k) {
-                const double *xk = x + (j0 + k) * n;
-                BICG_CUDA(cudaMemcpyAsync(m->vec(MUL_SLOT[k]), xk, (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
-                pl.vec(PH_PUSH, tail_none(), MUL_SLOT[k], xk);
-            }
-        }
+        for (int v = 0; v < MUL_NV_MAX; ++v) a.y[v] = y + (j0 + std::min(v, nv - 1)) * n;
+        hb.stage(x, j0, nv, a.x);
         const int rc = launch_multiply(p.kind, p.lanes, p.threads, p.grid, smem, multiply_nv(nv), a, st);
         if (rc) fatal("bicgstab_b200: multiply launch failed (kind %d lanes %d threads %d grid %d vectors %d): %s", p.kind, p.lanes,
                       p.threads, p.grid, nv, cudaGetErrorString((cudaError_t)rc));
