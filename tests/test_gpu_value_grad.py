@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from test_gpu_multiply import _fma
+from rowsum_model import value_grad as replica      # the header's arithmetic, correctly rounded, entry by entry
 from test_gpu_set_values import _chunked_matrix
 from test_gpu_transpose import _case_csr, transposed_csr
 
@@ -53,27 +53,6 @@ def csr_of(B, case):
     return _case_csr(B, case)
 
 
-def sample(nnz, seed=0):
-    """the entries the replica checks: the first and last 150 and 400 random ones (the Fraction replica is slow)"""
-    idx = np.concatenate([np.arange(min(150, nnz)), np.arange(max(0, nnz - 150), nnz),
-                          np.random.default_rng(seed).integers(0, nnz, size=min(400, nnz))])
-    return np.unique(idx)
-
-
-def replica(rows, cols, u, v, alpha, beta, out0):
-    """The header's arithmetic, correctly rounded, for entries at (rows, cols): batches of NV_MAX vectors, t = u_0 v_0, then
-    fma(u_k, v_k, t) in order; out = alpha t, or fma(alpha, t, beta out) (beta = 1 after the first batch)."""
-    out = None
-    for j0 in range(0, u.shape[0], NV_MAX):
-        t = u[j0, rows] * v[j0, cols]
-        for k in range(j0 + 1, min(j0 + NV_MAX, u.shape[0])):
-            t = _fma(u[k, rows], v[k, cols], t)
-        b = beta if j0 == 0 else 1.0
-        prev = out0 if j0 == 0 else out
-        out = alpha * t if b == 0.0 else _fma(alpha, t, b * prev)
-    return out
-
-
 def _uv(nvec, n, seed):
     rng = np.random.default_rng(seed + 97 * nvec)
     return rng.standard_normal((nvec, n)), rng.standard_normal((nvec, n))
@@ -89,13 +68,13 @@ def case(request, B):
 
 
 def test_matches_replica(B, case):
-    """host, device and stream-ordered calls agree bit for bit with each other and with the replica on sampled entries, for
+    """host, device and stream-ordered calls agree bit for bit with each other and with the replica on every entry, for
     vector counts 1, 3, 8, 9, 17, negative alpha, beta != 0 and a NaN-filled output at beta = 0"""
     torch = _torch()
     name, n, ptr, col, val, dm = case
     nnz = int(ptr[-1])
     rows = np.repeat(np.arange(n), np.diff(ptr))
-    idx = sample(nnz)
+    idx = np.arange(nnz)                             # every entry
     for i, nvec in enumerate(NVECS):
         alpha, beta = COMBOS[i % len(COMBOS)]
         u, v = _uv(nvec, n, 1)
@@ -189,7 +168,7 @@ def test_transpose_handle_in_its_own_order(B, case):
         u, v = _uv(3, n, 4)
         got, _ = mt.value_grad(u, v, alpha=-1.0)
         assert _bits(got) == _bits(fresh.value_grad(u, v, alpha=-1.0)[0]), name
-        idx = sample(int(tp[-1]), 1)
+        idx = np.arange(int(tp[-1]))
         trows = np.repeat(np.arange(n), np.diff(tp))
         assert _bits(got[idx]) == _bits(replica(trows[idx], tc[idx], u, v, -1.0, 0.0, None)), name
     finally:
