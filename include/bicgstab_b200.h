@@ -189,10 +189,24 @@ void         bicg_matrix_invalidate(const CSR_Matrix *diag);
  * bicg_matrix_shift_diagonal: A_diag += sigma I on the handle, like csr_shift_diagonal (matrix.c:536-551) on the host arrays:
  * sigma is added to the first entry of every own row whose column is that row; repeated calls accumulate.  Synchronous and
  * rank-local.  Returns 0, or -1 for a null handle or when a row of this rank has no diagonal entry (the reference exits
- * there), and then no value has changed.  An asynchronous shift is bicg_matrix_set_values_async with shifted values. */
+ * there), and then no value has changed.
+ *
+ * bicg_matrix_shift_diagonal_async: the same shift by *sigma, one double in DEVICE memory read in stream order, enqueued on the
+ * caller's CUDA stream `stream` with the ordering of bicg_matrix_set_values_async (no host synchronisation, allocation or
+ * pageable copy), so a replay of a captured shift adds the value the buffer holds then; the persistent kernel's value tables
+ * are rebuilt as by every value update, and the result is bit-identical to bicg_matrix_shift_diagonal by that value.
+ * Rank-local.  Returns 0; -1 for a null m or sigma (checked before the device is touched), or when a row of this rank, or of
+ * any rank at the last prepare, has no diagonal entry (then no value has changed); -2 inside a stream capture when
+ * bicg_matrix_shift_diagonal_async_prepare has not run on the handle (the capture stays valid).
+ * bicg_matrix_shift_diagonal_async_prepare finds the diagonal positions (once per handle; it may synchronise) outside any
+ * capture; an uncaptured shift calls it itself at the handle's first asynchronous shift.  Collective: every rank returns -1
+ * if any rank passed a null handle or has a row without a diagonal entry, so a refusal leaves no rank waiting in collective
+ * work that would follow the shift (a transpose refresh, a solve); else 0. */
 int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, int device_vectors);
 int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream);
 int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma);
+int bicg_matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, void *stream);
+int bicg_matrix_shift_diagonal_async_prepare(bicg_matrix *m);
 
 /* A^T of a resident matrix as a handle of its own: for adjoint systems A^T lambda = g (the gradient of an objective of the
  * solution of A x = b, the backward of a differentiable solve), two-sided Krylov methods and the normal equations.
@@ -438,6 +452,26 @@ int bicg_matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const doub
                            double *diag_out, double *offd_out, int device_vectors);
 int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
                                  double *diag_out, double *offd_out, void *stream);
+
+/* Global dot products of vectors in the x_set layout: out[j] = sum over ranks of sum_i u_j[i] v_j[i] for j < nvec, where u and v
+ * are nvec contiguous blocks of n_loc doubles each and out is nvec doubles, all DEVICE memory, read and written in stream order
+ * on the caller's CUDA stream `stream` behind the handle's previous work, with the ordering of bicg_matrix_multiply_async: no
+ * host synchronisation, allocation, pageable copy or output, no prepare step (there is no -2), and it works inside a stream
+ * capture.  The handle lends its ranks and scratch: u and v need not have anything to do with its matrix.  Every rank gets the
+ * same bits of every out[j].
+ *
+ * Arithmetic, for one vector j (csrc/dots.cu), fixed by the element index, n_loc and the rank count alone, not by the grid, the
+ * SM count or the SpMV plan:
+ *   chunks of 4096 elements: chunk c, thread t (t < 256) runs p_t = fma(u[e], v[e], p_t) from p_t = +0.0 over the elements
+ *       e = 4096 c + t + 256 s, s = 0 .. 15, those < n_loc, in s order;
+ *   the chunk's sum is the tree p_t = p_t + p_(t + h) for h = 128, 64, .., 1, t < h: p_0;
+ *   the rank's sum adds the chunk sums in chunk order onto +0.0 (n_loc = 0: +0.0);
+ *   out[j] adds the ranks' sums in rank order: S_0 + S_1 + ... + S_(P-1).
+ * No result is -0.  Vectors go in batches of up to 8, one cross-GPU reduction each (the shifted solvers' reduction).
+ *
+ * Returns 0, or -1 for a null handle, u, v or out, or nvec <= 0; these are checked before the device is touched.  Collective
+ * when there are peers: the ranks must agree on nvec; a peer timeout is reported by the next synchronous call on the handle. */
+int bicg_matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, void *stream);
 
 /* Time `reps` launches of the fused SpMV + (r_hat, s) dot kernel (the dominant kernel of every
  * variant) with CUDA events on the library's stream; returns average ms per launch in *ms and the

@@ -15,7 +15,8 @@ from .api import (METHODS, GEN_KINDS, MatrixBlock, DeviceMatrix, blocks_from_csr
 from ._lib import lib, CSR_Matrix, INFO_Matrix, bicg_stats, SYMBOLS, LIB_PATH
 
 # the differentiable entry points need torch, which importing the package does not: autograd.py is loaded on first use
-_AUTOGRAD = ("solve_autograd", "multiply_autograd", "SolveFunction", "MultiplyFunction")
+_AUTOGRAD = ("solve_autograd", "multiply_autograd", "shifted_solve_autograd", "SolveFunction", "MultiplyFunction",
+             "ShiftedSolveFunction")
 
 
 def __getattr__(name):

@@ -91,6 +91,9 @@ SYMBOLS = {
     "bicg_matrix_value_grad_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                                C.c_void_p, C.c_void_p]),
     "bicg_matrix_shift_diagonal": (C.c_int, [C.c_void_p, C.c_double]),
+    "bicg_matrix_shift_diagonal_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bicg_matrix_shift_diagonal_async_prepare": (C.c_int, [C.c_void_p]),
+    "bicg_matrix_dots_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "bicg_matrix_create_transpose": (C.c_void_p, [C.c_void_p]),
     "bicg_matrix_transpose_values": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bicg_matrix_transpose_values_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),

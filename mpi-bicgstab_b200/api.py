@@ -505,6 +505,56 @@ class DeviceMatrix:
         if lib.bicg_matrix_shift_diagonal(self.h, float(sigma)) != 0:
             raise ValueError("bicg_matrix_shift_diagonal failed: a row of this rank has no diagonal entry (no value was changed)")
 
+    def shift_diagonal_async(self, sigma, stream=None):
+        """bicg_matrix_shift_diagonal_async: shift_diagonal by the value a CUDA float64 tensor of one element holds (a view
+        sigma[j:j+1] works), enqueued on `stream` (default: torch's current stream) behind the handle's earlier work, with no host
+        synchronisation; the value is read in stream order, so a replay of a captured shift adds what the tensor holds then.
+        Bit-identical to shift_diagonal by that value.  Inside torch.cuda.graph, call prepare_shift_diagonal_async first; an
+        uncaptured call runs it itself the first time, which makes that call collective.  Raises ValueError, with no value
+        changed, when a row has no diagonal entry."""
+        import torch
+        if not isinstance(sigma, torch.Tensor):
+            raise TypeError(f"sigma: shift_diagonal_async takes a CUDA tensor, got {type(sigma).__name__}")
+        (sp_,) = _checked_cuda_vectors(("sigma", sigma, (1,)))
+        if stream is None:
+            stream = torch.cuda.current_stream(sigma.device)
+        rc = lib.bicg_matrix_shift_diagonal_async(self.h, sp_, C.c_void_p(stream.cuda_stream))
+        if rc == -2:
+            raise RuntimeError("shift_diagonal_async inside a stream capture needs prepare_shift_diagonal_async() first")
+        if rc != 0:
+            raise ValueError("bicg_matrix_shift_diagonal_async failed: a row has no diagonal entry (no value was changed)")
+
+    def prepare_shift_diagonal_async(self):
+        """bicg_matrix_shift_diagonal_async_prepare: find the diagonal positions shift_diagonal_async needs, outside any capture.
+        Collective over the ranks; raises ValueError on every rank when a row of any rank has no diagonal entry."""
+        if lib.bicg_matrix_shift_diagonal_async_prepare(self.h) != 0:
+            raise ValueError("bicg_matrix_shift_diagonal_async_prepare failed: a row has no diagonal entry (on this or another rank)")
+
+    def dots_async(self, u, v, out=None, stream=None):
+        """bicg_matrix_dots_async: out[j] = <u_j, v_j> summed over every rank's rows, for u and v contiguous CUDA float64 tensors
+        of shape (n_loc,) or (nvec, n_loc) (the rows of the x_set layout), in the fixed order the header gives; every rank gets
+        the same bits.  out: a contiguous CUDA float64 tensor of shape (nvec,), allocated when None.  Enqueued on `stream`
+        (default: torch's current stream) behind the handle's earlier work with no host synchronisation; works inside
+        torch.cuda.graph with no prepare step.  Collective over the ranks.  Returns out."""
+        import torch
+        for name, t in (("u", u), ("v", v), ("out", out)):
+            if t is not None and not isinstance(t, torch.Tensor):
+                raise TypeError(f"{name}: dots_async takes CUDA tensors only, got {type(t).__name__}")
+        shape = self._multiply_shape(u)
+        nvec = shape[0] if len(shape) == 2 else 1
+        given = out is not None
+        if not given:
+            out = u.new_empty((nvec,), dtype=u.dtype)
+        up, vp, op_ = _checked_cuda_vectors(("u", u, shape), ("v", v, shape), ("out", out, (nvec,)))
+        if stream is None:
+            stream = torch.cuda.current_stream(u.device)
+        if not given and stream != torch.cuda.current_stream(u.device):
+            out.record_stream(stream)             # written on `stream`, not on the one it was allocated on
+        rc = lib.bicg_matrix_dots_async(self.h, nvec, up, vp, op_, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_dots_async failed with {rc}")
+        return out
+
     def solve(self, method, x, r, krr=0, nrr=0):
         """bicg_solve: x (initial guess in, solution out) and r (b in, final residual out) are both numpy float64 arrays, or both
         contiguous CUDA float64 torch tensors of shape (n_loc,), which are updated in place.  Returns (iterations, stats)."""
@@ -773,6 +823,19 @@ class DeviceMatrix:
             self._t = self.transpose()
         self.prepare_async(method)
         self._t.prepare_async(method)
+
+    def prepare_shifted_autograd(self, method, sigma_len, adjoint_method="bicgstab"):
+        """What shifted_solve_autograd on this handle needs inside torch.cuda.graph: creates and keeps the transpose as
+        prepare_autograd does, runs prepare_shifted_async(method, sigma_len) here and prepare_async(adjoint_method) on the
+        transpose, and finds the transpose's diagonal positions for shift_diagonal_async.  Call it outside any capture.
+        Collective over the ranks; raises ValueError on every rank when a row of A^T on any rank has no diagonal entry."""
+        if self._t is None:
+            self._t = self.transpose()
+        self.prepare_shifted_async(method, sigma_len)
+        self._t.prepare_async(adjoint_method)
+        if lib.bicg_matrix_shift_diagonal_async_prepare(self._t.h) != 0:
+            raise ValueError("prepare_shifted_autograd: a row of A^T has no diagonal entry (a column of A without one, on this or "
+                             "another rank), so A^T + sigma I cannot be formed by shifting stored entries")
 
     def _adjoint(self):
         """The transpose the backward of a differentiable solve or multiply runs on: the one prepare_autograd made, else created

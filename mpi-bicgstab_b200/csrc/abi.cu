@@ -219,6 +219,11 @@ int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const d
     return matrix_set_values(m, diag_val, offd_val, true, true, (cudaStream_t)stream);
 }
 int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma) { return matrix_shift_diagonal(m, sigma); }
+int bicg_matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, void *stream)
+{
+    return matrix_shift_diagonal_async(m, sigma, (cudaStream_t)stream);
+}
+int bicg_matrix_shift_diagonal_async_prepare(bicg_matrix *m) { return matrix_shift_diagonal_async_prepare(m); }
 bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m) { return matrix_create_transpose(m); }
 int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src) { return matrix_transpose_values(mt, src, false, nullptr); }
 int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream)
@@ -263,6 +268,10 @@ int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, cons
                                  double *diag_out, double *offd_out, void *stream)
 {
     return matrix_value_grad_async(m, nvec, u, v, alpha, beta, diag_out, offd_out, (cudaStream_t)stream);
+}
+int bicg_matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, void *stream)
+{
+    return matrix_dots_async(m, nvec, u, v, out, (cudaStream_t)stream);
 }
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {

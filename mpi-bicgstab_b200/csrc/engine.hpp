@@ -212,6 +212,8 @@ struct bicg_matrix {
     unsigned *d_blk_ptr = nullptr;
     int *d_diag_pos = nullptr;
     bool diag_missing = false;
+    // bicg_matrix_shift_diagonal_async_prepare has run, and whether it found a row without a diagonal entry on some rank
+    bool diag_prepared = false, diag_refused = false;
     // test hooks of the value gradient (bicg_debug_value_grad_layout): a forced group width per row (0: chosen) and, at one
     // rank, caller-supplied diag / offd row pointers [2][n_loc + 1] that split every merged row (null: the handle's own order)
     int vg_lanes = 0;
@@ -299,6 +301,9 @@ bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, c
 // bicg_matrix_set_values (async = false: on the library's stream, returns once done) and bicg_matrix_set_values_async (on st)
 int  matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st);
 int  matrix_shift_diagonal(bicg_matrix *m, double sigma);     // bicg_matrix_shift_diagonal
+// bicg_matrix_shift_diagonal_async (on st) and its prepare step
+int  matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, cudaStream_t st);
+int  matrix_shift_diagonal_async_prepare(bicg_matrix *m);
 // the persistent kernel's value tables and packed values from d_val, on st: what creation and every value update run last
 void launch_value_tables(const bicg_matrix *m, cudaStream_t st);
 // transpose.cu: bicg_matrix_create_transpose, bicg_matrix_transpose_values (async = false: on the library's stream, returns
@@ -366,6 +371,8 @@ int  matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *
                        double *offd_out, bool device_vectors);
 int  matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
                              double *diag_out, double *offd_out, cudaStream_t st);
+// dots.cu: bicg_matrix_dots_async (device pointers, on st)
+int  matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, cudaStream_t st);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class = 0);

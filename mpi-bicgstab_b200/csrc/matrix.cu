@@ -646,6 +646,14 @@ __global__ void __launch_bounds__(256) shift_diag_kernel(int n_loc, const int *_
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x) val[pos[i]] += sigma;
 }
 
+// the same with sigma read from device memory in stream order (bicg_matrix_shift_diagonal_async)
+__global__ void __launch_bounds__(256) shift_diag_dev_kernel(int n_loc, const int *__restrict__ pos, const double *sigma,
+                                                             double *__restrict__ val)
+{
+    const double s = *sigma;
+    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_loc; i += gridDim.x * blockDim.x) val[pos[i]] += s;
+}
+
 static int row_blocks(int n_loc) { return std::max(1, std::min((n_loc + 255) / 256, ctx().sm_count * 8)); }
 
 void Context::release_arenas()
@@ -1025,6 +1033,21 @@ int matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd
     return 0;
 }
 
+// d_diag_pos and diag_missing, found at the first call (on the library's stream, synchronising); the pattern never changes
+static void find_diag_pos(bicg_matrix *m)
+{
+    if (m->d_diag_pos) return;
+    Context &c = ctx();
+    m->d_diag_pos = (int *)c.dev_alloc(((size_t)m->n_loc + 1) * sizeof(int));      // + the count of rows without one
+    int missing = 0;
+    BICG_CUDA(cudaMemsetAsync(m->d_diag_pos + m->n_loc, 0, sizeof(int), c.stream));
+    diag_pos_kernel<<<row_blocks(m->n_loc), 256, 0, c.stream>>>(m->n_loc, m->d_ptr, m->d_col, m->d_diag_pos, m->d_diag_pos + m->n_loc);
+    BICG_CUDA(cudaGetLastError());
+    BICG_CUDA(cudaMemcpyAsync(&missing, m->d_diag_pos + m->n_loc, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    m->diag_missing = missing > 0;
+}
+
 int matrix_shift_diagonal(bicg_matrix *m, double sigma)
 {
     if (!m) return -1;
@@ -1032,21 +1055,55 @@ int matrix_shift_diagonal(bicg_matrix *m, double sigma)
     c.ensure();
     wait_handle(m);
     const int blocks = row_blocks(m->n_loc);
-    if (!m->d_diag_pos) {
-        m->d_diag_pos = (int *)c.dev_alloc(((size_t)m->n_loc + 1) * sizeof(int));      // + the count of rows without one
-        int missing = 0;
-        BICG_CUDA(cudaMemsetAsync(m->d_diag_pos + m->n_loc, 0, sizeof(int), c.stream));
-        diag_pos_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_ptr, m->d_col, m->d_diag_pos, m->d_diag_pos + m->n_loc);
-        BICG_CUDA(cudaGetLastError());
-        BICG_CUDA(cudaMemcpyAsync(&missing, m->d_diag_pos + m->n_loc, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-        BICG_CUDA(cudaStreamSynchronize(c.stream));
-        m->diag_missing = missing > 0;
-    }
+    find_diag_pos(m);
     if (m->diag_missing) return -1;           // the reference exits here (matrix.c:547-550); nothing has been changed
     shift_diag_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
     BICG_CUDA(cudaGetLastError());
     launch_value_tables(m, c.stream);
     BICG_CUDA(cudaStreamSynchronize(c.stream));
+    return 0;
+}
+
+int matrix_shift_diagonal_async_prepare(bicg_matrix *m)
+{
+    Context &c = ctx();
+    // collective: a rank that refuses must not leave the others waiting in the collective work that follows a shift
+    int bad = 1;
+    if (m) {
+        c.ensure();
+        wait_handle(m);
+        find_diag_pos(m);
+        bad = m->diag_missing ? 1 : 0;
+    }
+    std::vector<int> all((size_t)c.world);
+    c.host_allgather(&bad, all.data(), sizeof(int));
+    bool any = false;
+    for (int b : all) any = any || b != 0;
+    if (!m) return -1;
+    m->diag_prepared = true;
+    m->diag_refused = any;
+    return any ? -1 : 0;
+}
+
+int matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, cudaStream_t st)
+{
+    if (!m || !sigma) return -1;
+    Context &c = ctx();
+    c.ensure();
+    cudaStreamCaptureStatus cs;
+    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
+    const bool captured = cs != cudaStreamCaptureStatusNone;
+    if (!m->diag_prepared) {
+        if (captured) return -2;
+        if (matrix_shift_diagonal_async_prepare(m) != 0) return -1;
+    }
+    if (m->diag_missing || m->diag_refused) return -1;        // nothing has been changed
+    async_handle_init(m);
+    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    shift_diag_dev_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
+    BICG_CUDA(cudaGetLastError());
+    launch_value_tables(m, st);
+    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
     return 0;
 }
 
