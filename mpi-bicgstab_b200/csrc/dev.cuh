@@ -267,52 +267,26 @@ __device__ __forceinline__ TileWindow tile_window(int row0, int row1, unsigned p
     return w;
 }
 
-// One row's product with x over the staged entries [j, e) (j already includes the thread's offset in its group of
-// LANES), summed over the group.  This loop decides the bits of y: entries in storage order, one fma each, then
-// lanes_sum.  UNR gathers are in flight per thread; `column(idx)` and `value(idx)` return the column and the value of
-// staged entry idx (a value may come as an object that converts to double: it is converted where it is multiplied).
-template <int LANES, int UNR, class Value, class Column>
-__device__ __forceinline__ double row_product(Value value, Column column, const double *x, int j, int e)
-{
-    double acc = 0.0;
-    while (j < e) {
-        unsigned c[UNR];
-        decltype(value(0)) v[UNR];
-        double xv[UNR];
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) {
-            // clamp instead of predicating: unconditional loads batch freely (a predicated load per slot runs out
-            // of predicate registers after 7); the FMA below is what is predicated
-            const int idx = min(j + u * LANES, e - 1);
-            c[u] = column(idx);
-            v[u] = value(idx);
-        }
-#pragma unroll
-        for (int u = 0; u < UNR; ++u) xv[u] = ld_coherent(x + c[u]);
-#pragma unroll
-        for (int u = 0; u < UNR; ++u)
-            if (j + u * LANES < e) acc = fma((double)v[u], xv[u], acc);
-        j += UNR * LANES;
-    }
-    return lanes_sum<LANES>(acc);
-}
-
-// row_product for NV vectors at once (the batched multiply, spmv.cu): entry idx is read once and multiplied with x[v][col]
-// for every v, so UNR * NV gathers are in flight per thread.  Per vector the order is row_product's -- entries in storage
-// order, one fma each, then lanes_sum -- and UNR only decides how many entries one pass loads, so acc[v] is bit-identical to
-// row_product(value, column, x[v], j, e) whatever UNR and NV are.
+// One row's product with NV vectors x[v] over the staged entries [j, e) (j already includes the thread's offset in its
+// group of LANES), summed over the group into acc[v].  This loop decides the bits of y: per vector, entries in storage
+// order, one fma each, then lanes_sum.  Entry idx is read once for all NV gathers x[v][col], so UNR * NV gathers are in
+// flight per thread; UNR only decides how many entries one pass loads, so acc[v] does not depend on UNR or NV.
+// `column(idx)` and `value(idx)` return the column and the value of staged entry idx (a value may come as an object that
+// converts to double: it is converted where it is multiplied).
 template <int LANES, int UNR, int NV, class Value, class Column>
-__device__ __forceinline__ void row_products(Value value, Column column, const double *const (&x)[NV], int j, int e,
-                                             double (&acc)[NV])
+__device__ __forceinline__ void row_product(Value value, Column column, const double *const (&x)[NV], int j, int e,
+                                            double (&acc)[NV])
 {
 #pragma unroll
     for (int v = 0; v < NV; ++v) acc[v] = 0.0;
     while (j < e) {
         unsigned c[UNR];
-        double a[UNR];
+        decltype(value(0)) a[UNR];
         double xv[NV][UNR];
 #pragma unroll
         for (int u = 0; u < UNR; ++u) {
+            // clamp instead of predicating: unconditional loads batch freely (a predicated load per slot runs out
+            // of predicate registers after 7); the FMA below is what is predicated
             const int idx = min(j + u * LANES, e - 1);
             c[u] = column(idx);
             a[u] = value(idx);
@@ -325,7 +299,7 @@ __device__ __forceinline__ void row_products(Value value, Column column, const d
         for (int v = 0; v < NV; ++v)
 #pragma unroll
             for (int u = 0; u < UNR; ++u)
-                if (j + u * LANES < e) acc[v] = fma(a[u], xv[v][u], acc[v]);
+                if (j + u * LANES < e) acc[v] = fma((double)a[u], xv[v][u], acc[v]);
         j += UNR * LANES;
     }
 #pragma unroll

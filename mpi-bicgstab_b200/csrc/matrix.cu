@@ -288,7 +288,7 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
     Context &c = ctx();
     const int rpt = threads / lanes;
     const long long SMEM_MAX = 224 * 1024;
-    const long long fixed = (long long)(rpt + 8) * 36;        // ptr slice + 4 epilogue slices per stage (spmv.cu)
+    const long long fixed = (long long)spmv_stage_bytes(0, rpt, SPMV_EPI_SLICES);   // a stage's bytes beside the entries
     // stage capacity: a full tile of average rows with 25 % head-room, never less than the longest row
     long long cap = (long long)std::ceil(rpt * m->mean_row * 1.25) + 64;
     cap = std::max<long long>(cap, (long long)m->max_row + 16);
@@ -296,8 +296,8 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
     int ctas = want_ctas > 0 ? want_ctas : 2;
     // shrink towards the shared-memory budget of `ctas` CTAs per SM
     const long long budget = SMEM_MAX / ctas - 1536;
-    if ((long long)stages * (cap * 12 + fixed) > budget) {
-        long long fit = (budget / stages - fixed) / 12;
+    if ((long long)stages * (cap * SPMV_ENTRY_BYTES + fixed) > budget) {
+        long long fit = (budget / stages - fixed) / SPMV_ENTRY_BYTES;
         fit = (fit / 32) * 32;
         if (fit < (long long)m->max_row + 16) return false;
         cap = fit;
@@ -309,7 +309,7 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
     for (size_t i = 0; i < tile_row.size(); ++i) tile_nz[i] = h_ptr[tile_row[i]];
 
     out.kind = 0; out.lanes = lanes; out.threads = threads; out.stages = stages; out.cap = (int)cap;
-    out.smem = spmv_tma_smem_bytes((int)cap, stages, threads, lanes);
+    out.smem = (size_t)stages * spmv_stage_bytes((int)cap, rpt, SPMV_EPI_SLICES);
     int by_smem = (int)std::max<long long>(1, SMEM_MAX / (long long)(out.smem + 1536));
     out.ctas_per_sm = std::max(1, std::min({by_smem, 2048 / (threads + 32), want_ctas > 0 ? want_ctas : 8}));
     out.ntiles = nt;
@@ -347,7 +347,7 @@ SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y
     a.kc.tail = TailDesc{TAIL_NONE, FIN_NONE, 0, 0, 0, 0, 0};
     a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
     a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
-    a.x = m->vec(x_id); a.y = m->vec(y_id);
+    a.nv = 1; a.x[0] = m->vec(x_id); a.y[0] = m->vec(y_id);
     a.epi = EpiArgs{};
     a.wait_halo = (m->world > 1 && m->comm.recv_mask != 0) ? 1 : 0;
     return a;
@@ -361,12 +361,12 @@ void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a
         cudaEvent_t e0, e1;
         BICG_CUDA(cudaEventCreate(&e0)); BICG_CUDA(cudaEventCreate(&e1));
         BICG_CUDA(cudaEventRecord(e0, st));
-        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, st);
+        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, true, a, st);
         if (rc) fatal("bicgstab_b200: SpMV launch failed: %s", cudaGetErrorString((cudaError_t)rc));
         BICG_CUDA(cudaEventRecord(e1, st));
         c.prof_ev.push_back(e0); c.prof_ev.push_back(e1); c.prof_class.push_back(prof_class);
     } else {
-        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, a, st);
+        int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, p.smem, true, a, st);
         if (rc) fatal("bicgstab_b200: SpMV launch failed (kind %d lanes %d threads %d grid %d smem %zu): %s",
                       p.kind, p.lanes, p.threads, p.grid, p.smem, cudaGetErrorString((cudaError_t)rc));
     }

@@ -597,8 +597,9 @@ struct Mega {
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
                 if (sub == 0) epi_load<EPI>(row, e0, e1, e2, e3);
             }
-            const double acc = row_product<LANES, UNR>(value, column, x, j, e);
-            if (valid && sub == 0) row_done<EPI>(row, acc, e0, e1, e2, e3, y, dot);
+            double acc[1];
+            row_product<LANES, UNR, 1>(value, column, {x}, j, e, acc);
+            if (valid && sub == 0) row_done<EPI>(row, acc[0], e0, e1, e2, e3, y, dot);
             __syncwarp();
             if (lane == 0) mbar_arrive(smem_u32(&sh.empty_bar[s]));
         }

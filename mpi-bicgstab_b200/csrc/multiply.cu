@@ -1,8 +1,9 @@
 // multiply.cu -- y_j = alpha (A + sigma_j I) x_j + beta y_j, j < nvec, on a resident matrix: bicg_matrix_multiply (synchronous,
 // host or device vectors) and bicg_matrix_multiply_async (device vectors, on the caller's stream, capturable).
 //
-// The work is the batched SpMV of spmv.cu on the handle's SpMV plan: a launch takes up to MUL_NV_MAX vectors and streams
-// the matrix once for all of them, so every row sum is the one bicg_spmv computes for that vector alone.  At one rank the
+// The work is the SpMV kernels of spmv.cu with the multiply's epilogue, on the handle's SpMV plan: a launch takes up to
+// MUL_NV_MAX vectors and streams the matrix once for all of them, so every row sum is the one bicg_spmv computes for that
+// vector alone.  At one rank the
 // kernels gather straight from the caller's x_j and write straight into y_j.  With peers the ghost columns of x_j come from
 // the ghost tail of an arena vector (MUL_SLOT[k], the slots of shift_check.cu): the owner copies x_j's own rows into that
 // vector, so the kernel reads one extended vector, and pushes the boundary runs into the same slot on its neighbours.  Each
@@ -68,20 +69,20 @@ void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, doub
     const SpmvPlan &p = m->plan;
     const long long n = m->n_loc;
     HaloBatches hb(m, st);
-    MultiplyArgs a{};
+    SpmvArgs a{};
     a.kc = hb.kc;
     a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
     a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
     a.alpha = alpha; a.beta = beta;
     a.wait_halo = hb.wait_halo;
-    const size_t smem = p.kind == 0 ? multiply_tma_smem_bytes(p.cap, p.stages, p.threads, p.lanes) : 0;
+    const size_t smem = p.kind == 0 ? (size_t)p.stages * spmv_stage_bytes(p.cap, p.threads / p.lanes, 0) : 0;
     for (int j0 = 0; j0 < nvec; j0 += MUL_NV_MAX) {
         const int nv = std::min(MUL_NV_MAX, nvec - j0);
         a.nv = nv;
         a.sigma = sigma ? sigma + j0 : nullptr;
         for (int v = 0; v < MUL_NV_MAX; ++v) a.y[v] = y + (j0 + std::min(v, nv - 1)) * n;
         hb.stage(x, j0, nv, a.x);
-        const int rc = launch_multiply(p.kind, p.lanes, p.threads, p.grid, smem, multiply_nv(nv), a, st);
+        const int rc = launch_spmv(p.kind, p.lanes, p.threads, p.grid, smem, false, a, st);
         if (rc) fatal("bicgstab_b200: multiply launch failed (kind %d lanes %d threads %d grid %d vectors %d): %s", p.kind, p.lanes,
                       p.threads, p.grid, nv, cudaGetErrorString((cudaError_t)rc));
         ++ctx().launches;

@@ -237,7 +237,7 @@ void PhaseLauncher::spmv(int x_id, int y_id, TailDesc tail, int ndot, const doub
 {
     SpmvArgs a = make_spmv_args(m, m->plan, x_id, y_id);
     a.kc.tail = tail;
-    a.shift_sigma = shift_sigma;
+    a.sigma = shift_sigma;
     const double *as[4] = {a0, a1, a2, a3}, *bs[4] = {b0, b1, b2, b3};
     for (int k = 0; k < ndot; ++k) epi_add_dot(a.epi, as[k], bs[k]);
     launch_spmv_plan(m, m->plan, a, stream, 0);

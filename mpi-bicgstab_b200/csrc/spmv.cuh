@@ -13,6 +13,11 @@ struct EpiArgs {
     int ia[4], ib[4];
 };
 
+// One argument block for both epilogues of the SpMV kernels (spmv.cu).  The solver's SpMV: y[0] = A x[0] (+ sigma[0] x[0]),
+// with the dots of `epi` fused and reduced in the tail.  The batched multiply of bicg_matrix_multiply (multiply.cu):
+// y_v = alpha (A + sigma_v I) x_v + beta y_v, v < nv, one pass over the matrix for nv vectors.  Both run the same plan,
+// tiles and row loop, so every row sum is bit-identical between them.
+constexpr int MUL_NV_MAX = 8;        // vectors one launch can take (the largest instantiated NV)
 struct SpmvArgs {
     KernelCommon kc;
     // device CSR of this rank's rows over the extended local column space [own columns | ghost columns]
@@ -28,43 +33,29 @@ struct SpmvArgs {
     int ntiles;
     int cap;                    // stage capacity in entries (multiple of 32)
     int stages;                 // 2..4
-    const double *x;            // input vector, extended layout
-    double       *y;            // output, own rows
-    EpiArgs epi;
-    int wait_halo;              // 1: x's ghost part is filled by peers; wait for their halo flags first
-    const double *shift_sigma;  // not null: y = A x + (*shift_sigma) x  (shifted systems, shifted_switching_solver.c:386, 404)
-};
-
-// The batched multiply y_v = alpha (A + sigma_v I) x_v + beta y_v, v < nv, of bicg_matrix_multiply (multiply.cu): one pass
-// over the matrix serves nv vectors.  Same plan, tiles and lanes as the SpMV above, so every row sum is bit-identical to it.
-constexpr int MUL_NV_MAX = 8;        // vectors one launch can take (the largest instantiated NV)
-struct MultiplyArgs {
-    KernelCommon kc;                 // tail: the closing barrier with peers, none at one rank
-    const double   *val;
-    const unsigned *col;
-    const unsigned *ptr;
-    int rows;
-    const int      *tile_row;
-    const unsigned *tile_nz;
-    int ntiles, cap, stages;
-    int nv;                          // vectors of this launch, 1 .. MUL_NV_MAX
+    int nv;                          // vectors of this launch, 1 .. MUL_NV_MAX (the solver's SpMV: 1)
     const double *x[MUL_NV_MAX];     // x_v over the extended column space; slots v >= nv repeat x[nv - 1] and are not written
     double       *y[MUL_NV_MAX];     // y_v, own rows
-    const double *sigma;             // nv device values, or null: no shift term
-    double alpha, beta;              // beta == 0: y is not read
-    int wait_halo;                   // 1: the ghost part of every x_v is filled by peers; wait for their halo flags first
+    const double *sigma;             // nv device values, or null: no shift term (shifted systems, shifted_switching_solver.c:386, 404)
+    double alpha, beta;              // multiply epilogue; beta == 0: y is not read
+    EpiArgs epi;                     // solver epilogue
+    int wait_halo;                   // 1: x's ghost part is filled by peers; wait for their halo flags first
 };
-// the smallest instantiated NV that holds nv vectors (nv <= MUL_NV_MAX)
-int multiply_nv(int nv);
-int launch_multiply(int kind, int lanes, int threads, int grid, size_t smem_bytes, int NV, const MultiplyArgs &a, cudaStream_t st);
-size_t multiply_tma_smem_bytes(int cap, int stages, int threads, int lanes);
+
+// Bytes of one TMA stage of a tile of rpt rows: [val cap*8][nepi epilogue slices of PROW*8][col cap*4][ptr PROW*4],
+// PROW = rpt + PROW_PAD.  The solver's stages hold SPMV_EPI_SLICES epilogue slices, the multiply's none.
+constexpr int SPMV_EPI_SLICES = 4;
+constexpr int SPMV_ENTRY_BYTES = 12;   // val + col of one staged entry
+__host__ __device__ constexpr size_t spmv_stage_bytes(int cap, int rpt, int nepi)
+{
+    return (size_t)cap * SPMV_ENTRY_BYTES + (size_t)(rpt + PROW_PAD) * (size_t)(4 + 8 * nepi);
+}
 
 // kind 0: warp-specialised TMA tile kernel, kind 1: row-split kernel.  threads (consumer threads) only matters for kind 0.
-// Returns cudaError_t as int.
-int launch_spmv(int kind, int lanes, int threads, int grid, size_t smem_bytes, const SpmvArgs &a, cudaStream_t st);
+// solver: the solver's epilogue (a.nv == 1), else the multiply's for a.nv vectors.  Returns cudaError_t as int.
+int launch_spmv(int kind, int lanes, int threads, int grid, size_t smem_bytes, bool solver, const SpmvArgs &a, cudaStream_t st);
 // one-time opt-in to > 48 KB dynamic shared memory for every instantiation
 int spmv_setup_attributes();
-size_t spmv_tma_smem_bytes(int cap, int stages, int threads, int lanes);
 // add a dot term (a . b) to an epilogue; null pointer = the y just computed
 void epi_add_dot(EpiArgs &e, const double *a, const double *b);
 

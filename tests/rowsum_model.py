@@ -1,4 +1,4 @@
-"""A bitwise CPU model of the SpMV row sums (csrc/dev.cuh: row_product, row_products, lanes_sum) and of the epilogues the
+"""A bitwise CPU model of the SpMV row sums (csrc/dev.cuh: row_product, lanes_sum) and of the epilogues the
 header pins (include/bicgstab_b200.h: the batched multiply and the value gradient), in numpy with a correctly rounded fma.
 
 fma(a, b, c) is Boldo and Melquiond's emulation: the exact product as two_prod (Veltkamp split) and two_sum with c, the two
