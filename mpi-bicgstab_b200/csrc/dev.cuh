@@ -206,6 +206,34 @@ __device__ __forceinline__ double ld_coherent(const double *p)
     asm volatile("ld.global.f64 %0, [%1];" : "=d"(v) : "l"(p));
     return v;
 }
+// ---- L2 eviction priority of one access: ld / st .L2::cache_hint carrying a createpolicy value ------------------------
+// L1 behaves as for a plain ld.global / st.global; like ld_coherent, the loads never take the non-coherent path.
+__device__ __forceinline__ unsigned long long l2_evict_first_policy()
+{
+    unsigned long long pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ double ld_hint(const double *p, unsigned long long pol)
+{
+    double v;
+    asm volatile("ld.global.L2::cache_hint.f64 %0, [%1], %2;" : "=d"(v) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ double2 ld_hint2(const double *p, unsigned long long pol)
+{
+    double2 v;
+    asm volatile("ld.global.L2::cache_hint.v2.f64 {%0, %1}, [%2], %3;" : "=d"(v.x), "=d"(v.y) : "l"(p), "l"(pol));
+    return v;
+}
+__device__ __forceinline__ void st_hint(double *p, double v, unsigned long long pol)
+{
+    asm volatile("st.global.L2::cache_hint.f64 [%0], %1, %2;" ::"l"(p), "d"(v), "l"(pol));
+}
+__device__ __forceinline__ void st_hint2(double *p, double2 v, unsigned long long pol)
+{
+    asm volatile("st.global.L2::cache_hint.v2.f64 [%0], {%1, %2}, %3;" ::"l"(p), "d"(v.x), "d"(v.y), "l"(pol));
+}
 __device__ __forceinline__ unsigned long long globaltimer_ns()
 {
     unsigned long long t;

@@ -43,12 +43,6 @@ constexpr int RED_THREADS = MEGA_MAX_CTAS;          // one polled slot per threa
 constexpr int RED_WARPS = RED_THREADS / 32;
 struct StageHdr { int row0, row1; unsigned a0; int rowa; unsigned lo, hi; int flag; int pad_; };   // lo, hi: the tile's entries relative to a0
 
-__device__ __forceinline__ unsigned long long l2_evict_first_policy()
-{
-    unsigned long long pol;
-    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
-    return pol;
-}
 __device__ __forceinline__ void tma_load_1d_hint(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar,
                                                  unsigned long long pol)
 {
@@ -214,6 +208,9 @@ struct Mega {
     const double *rs_val; const unsigned short *rs_col; const unsigned *rs_ptr;
 
     __device__ Mega(const MegaArgs &args, MegaShared &s) : a(args), sh(s) {}
+
+    // the policy of run_bicgstab's evict-first accesses: made where a phase begins, not held in a register across the loop
+    static __device__ __forceinline__ Hint evict_first() { return Hint{l2_evict_first_policy()}; }
 
     __device__ bool stop_now() const { return sh.sc.done != 0 || sh.sc.error != 0; }
     __device__ void fail() { sh.flags[3] = 1; }
@@ -463,21 +460,22 @@ struct Mega {
     }
 
     // ---------------------------------------------------------------- SpMV over this CTA's tiles ----------
-    template <int EPI>
-    __device__ void spmv(const double *x, double *y, double (&dot)[4])
+    // far: the L2 policy of the r# loads of EPI_RH_Y (run_bicgstab's table); every other access of the SpMV is plain
+    template <int EPI, class F = Plain>
+    __device__ void spmv(const double *x, double *y, double (&dot)[4], F far = {})
     {
         if constexpr (LANES == 1) {
-            if (resident) { spmv_res<EPI>(x, y, dot); return; }
+            if (resident) { spmv_res<EPI>(x, y, dot, far); return; }
         }
-        if (packed) spmv_impl<EPI, true, true>(x, y, dot);
-        else if (coded) spmv_impl<EPI, true, false>(x, y, dot);
-        else spmv_impl<EPI, false, false>(x, y, dot);
+        if (packed) spmv_impl<EPI, true, true>(x, y, dot, far);
+        else if (coded) spmv_impl<EPI, true, false>(x, y, dot, far);
+        else spmv_impl<EPI, false, false>(x, y, dot, far);
     }
     // one row's epilogue operands (EPI_RH_Y: r#; EPI_QY_YY: q, kept in v.r; EPI_CA4: r#, r, s, z), loaded before its gathers
-    template <int EPI>
-    __device__ __forceinline__ void epi_load(int row, double &e0, double &e1, double &e2, double &e3) const
+    template <int EPI, class F>
+    __device__ __forceinline__ void epi_load(int row, double &e0, double &e1, double &e2, double &e3, F far) const
     {
-        if (EPI == EPI_RH_Y) e0 = a.v.rh[row];
+        if (EPI == EPI_RH_Y) e0 = ld1(a.v.rh + row, far);
         if (EPI == EPI_QY_YY) e0 = a.v.r[row];
         if (EPI == EPI_CA4) { e0 = a.v.rh[row]; e1 = a.v.r[row]; e2 = a.v.s[row]; e3 = a.v.z[row]; }
     }
@@ -497,8 +495,8 @@ struct Mega {
     // columns); a row's entries are accumulated in storage order, like spmv_impl.  Loads are unconditional on clamped indices
     // (always a valid entry of this slice; no predicate per load, so the U gathers of a pass are in flight together), only the
     // multiply-adds are guarded.
-    template <int EPI>
-    __device__ void spmv_res(const double *x, double *y, double (&dot)[4])
+    template <int EPI, class F>
+    __device__ void spmv_res(const double *x, double *y, double (&dot)[4], F far)
     {
         constexpr int U = 16;
         const double *xo = x + rp.w.obase, *xg = x + rp.w.gbase;
@@ -511,7 +509,7 @@ struct Mega {
             unsigned j = rs_ptr[r];
             const unsigned e = rs_ptr[r + 1];
             double e0 = 0.0, e1 = 0.0, e2 = 0.0, e3 = 0.0;     // epilogue operands: in flight during the gathers
-            epi_load<EPI>(row, e0, e1, e2, e3);
+            epi_load<EPI>(row, e0, e1, e2, e3, far);
             double acc = 0.0;
             while (j < e) {                                    // never entered when the slice is empty
                 double xv[U];
@@ -535,8 +533,8 @@ struct Mega {
     // both formats), each turned back into the column with one select and one add before its gather.
     // PACKED (CODED CTAs only): the stage's value area holds the three planes of the packed values -- vlo at 0, vmid at
     // 4 cap bytes, vhi at 6 cap bytes -- each value put back together by PackedVal.
-    template <int EPI, bool CODED, bool PACKED>
-    __device__ void spmv_impl(const double *x, double *y, double (&dot)[4])
+    template <int EPI, bool CODED, bool PACKED, class F>
+    __device__ void spmv_impl(const double *x, double *y, double (&dot)[4], F far)
     {
         const int stages = a.stages, cap = a.cap;
         const int sub = tid % LANES, row_in_tile = tid / LANES;
@@ -579,7 +577,7 @@ struct Mega {
                 if (h.flag == 2) {
                     if (tid == 0) {
                         double e0 = 0.0, e1 = 0.0, e2 = 0.0, e3 = 0.0;
-                        epi_load<EPI>(h.row0, e0, e1, e2, e3);
+                        epi_load<EPI>(h.row0, e0, e1, e2, e3, far);
                         row_done<EPI>(h.row0, carry, e0, e1, e2, e3, y, dot);
                     }
                     carry = 0.0;
@@ -595,7 +593,7 @@ struct Mega {
             if (valid) {
                 j = (int)(sptr[row - h.rowa] - h.a0) + sub;
                 e = (int)(sptr[row - h.rowa + 1] - h.a0);
-                if (sub == 0) epi_load<EPI>(row, e0, e1, e2, e3);
+                if (sub == 0) epi_load<EPI>(row, e0, e1, e2, e3, far);
             }
             double acc[1];
             row_product<LANES, UNR, 1>(value, column, {x}, j, e, acc);
@@ -607,18 +605,18 @@ struct Mega {
 
     // ---------------------------------------------------------------- vector phase over the CTA's own rows --
     // row_lo is a multiple of 16 and every arena vector is 128-byte aligned: 16-byte accesses, two in flight per
-    // vector and thread
-    template <int PH>
-    __device__ void vec(double *dot)
+    // vector and thread; far: the L2 policy of the phase's far accesses (body)
+    template <int PH, class F = Plain>
+    __device__ void vec(double *dot, F far = {})
     {
         Coef c;
         c.al = sh.sc.alpha; c.be = sh.sc.beta; c.om = sh.sc.omega;
         c.nbo = -c.be * c.om;
         const int hi2 = row_lo + ((row_hi - row_lo) & ~1);
         int i = row_lo + 2 * tid;
-        for (; i + 2 * CT < hi2; i += 4 * CT) body<PH, Pairs<2, 2 * CT>>(a.v, i, c, dot);
-        for (; i < hi2; i += 2 * CT) body<PH, Pairs<1, 2 * CT>>(a.v, i, c, dot);
-        if (tid == 0 && hi2 < row_hi) body<PH, Contig<1>>(a.v, hi2, c, dot);
+        for (; i + 2 * CT < hi2; i += 4 * CT) body<PH, Pairs<2, 2 * CT>>(a.v, i, c, dot, far);
+        for (; i < hi2; i += 2 * CT) body<PH, Pairs<1, 2 * CT>>(a.v, i, c, dot, far);
+        if (tid == 0 && hi2 < row_hi) body<PH, Contig<1>>(a.v, hi2, c, dot, far);
     }
     // ---------------------------------------------------------------- multi-GPU helpers ---------------------
     // releasing arrival + wait for EVERY CTA of this GPU (all == true) or for the CTAs owning the gathered columns
@@ -779,6 +777,25 @@ struct Mega {
     }
     // ---------------------------------------------------------------- solver.c:86-127 -----------------------
     // __noinline__: inlined into the kernel body, it makes the four 512-thread kernels spill under their 96-register cap
+    //
+    // L2 policy of every vector access of an iteration.  Six vectors of n doubles cycle through it (p, s, r# = rh,
+    // r = q, y, x: 77 MB at T', against the H100's 50 MB of L2, beside the evict-first matrix stream).  An access whose
+    // next use lies behind most of the other vectors is marked evict-first, so that the four that are re-used soon
+    // (p, s, r, y) keep L2 to themselves; all others are plain.
+    //   phase                  access                         policy       next use of the vector
+    //   SpMV s = A p           gather p, store s              plain        XR / Q
+    //                          load rh (EPI_RH_Y)             evict-first  XR, behind q, y
+    //   PH_BICG_Q              load r, s; store r (= q)       plain        SpMV y = A q / P
+    //   SpMV y = A q           gather q, load q; store y      plain        XR
+    //   PH_BICG_XR             load x; store x                evict-first  XR of the next iteration
+    //                          load y                         evict-first  none: the next SpMV 2 overwrites y
+    //                          load rh                        evict-first  SpMV 1 of the next iteration, behind p, s
+    //                          load p, r; store r             plain        P
+    //   PH_BICG_P              load s                         evict-first  none: the next SpMV 1 overwrites s
+    //                          load p, r; store p             plain        SpMV s = A p
+    // Each of the five demotions was measured on its own (T', H100 80GB HBM3, 700 W: 272.5 us per iteration without
+    // any, 260.9 with all five, 263.5 to 265.3 with any one left plain).  The policy value is made where a phase
+    // begins (evict_first()).  run_bicgstab_multi keeps plain accesses: a rank's share of the vectors is 1 / N of them.
     __device__ __noinline__ void run_bicgstab()
     {
         double d4[4], d2[2], d1[1], d0[1];
@@ -786,7 +803,7 @@ struct Mega {
         while (true) {
             mark(0);
             d4[0] = d4[1] = d4[2] = d4[3] = 0.0;
-            spmv<EPI_RH_Y>(a.v.p, a.v.s, d4);                               // s = A p, (r#,s)           :88-91
+            spmv<EPI_RH_Y>(a.v.p, a.v.s, d4, evict_first());                // s = A p, (r#,s)           :88-91
             mark(1);
             d1[0] = d4[0];
             reduce<1>(d1, FIN_BICG_ALPHA, true);                            // alpha                      :93
@@ -803,12 +820,12 @@ struct Mega {
             reduce<2>(d2, FIN_BICG_OMEGA);                                  // omega                      :104
             mark(6);
             d2[0] = d2[1] = 0.0;
-            vec<PH_BICG_XR>(d2);                                            // x, r, (r,r), (r#,r)        :105-114
+            vec<PH_BICG_XR>(d2, evict_first());                             // x, r, (r,r), (r#,r)        :105-114
             mark(7);
             reduce<2>(d2, FIN_BICG_BETA);                                   // beta, k++, loop test       :116-120
             mark(8);
             if (stop_now()) break;
-            vec<PH_BICG_P>(d0);                                             // p                          :117-119
+            vec<PH_BICG_P>(d0, evict_first());                              // p                          :117-119
             mark(9);
             sync_nbr();
             mark(10);

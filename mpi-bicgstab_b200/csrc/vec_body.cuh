@@ -7,29 +7,41 @@ namespace bicg {
 
 template <int W> struct Pk { double v[W]; };
 
-template <int W> __device__ __forceinline__ Pk<W> ld(const double *p, int i);
-template <> __device__ __forceinline__ Pk<1> ld<1>(const double *p, int i) { Pk<1> r; r.v[0] = p[i]; return r; }
-template <> __device__ __forceinline__ Pk<2> ld<2>(const double *p, int i)
+// L2 policy of one access: Plain = no hint (plain ld / st, what every phase kernel of vec.cu uses); Hint = the access
+// carries a createpolicy value (dev.cuh: ld_hint, st_hint), e.g. evict-first for a vector whose next use is too far
+// away for L2 to keep it (mega.cu: run_bicgstab)
+struct Plain {};
+struct Hint { unsigned long long pol; };
+
+__device__ __forceinline__ double ld1(const double *p, Plain) { return *p; }
+__device__ __forceinline__ double ld1(const double *p, Hint h) { return ld_hint(p, h.pol); }
+__device__ __forceinline__ double2 ld2(const double *p, Plain) { return *reinterpret_cast<const double2 *>(p); }
+__device__ __forceinline__ double2 ld2(const double *p, Hint h) { return ld_hint2(p, h.pol); }
+__device__ __forceinline__ void st1(double *p, double v, Plain) { *p = v; }
+__device__ __forceinline__ void st1(double *p, double v, Hint h) { st_hint(p, v, h.pol); }
+__device__ __forceinline__ void st2(double *p, double2 v, Plain) { *reinterpret_cast<double2 *>(p) = v; }
+__device__ __forceinline__ void st2(double *p, double2 v, Hint h) { st_hint2(p, v, h.pol); }
+
+// W contiguous doubles: one 8-byte access for W = 1, 16-byte accesses otherwise
+template <int W, class H> __device__ __forceinline__ Pk<W> ld(const double *p, int i, H h)
 {
-    const double2 t = *reinterpret_cast<const double2 *>(p + i);
-    Pk<2> r; r.v[0] = t.x; r.v[1] = t.y; return r;
+    Pk<W> r;
+    if constexpr (W == 1) {
+        r.v[0] = ld1(p + i, h);
+    } else {
+#pragma unroll
+        for (int k = 0; k < W; k += 2) { const double2 t = ld2(p + i + k, h); r.v[k] = t.x; r.v[k + 1] = t.y; }
+    }
+    return r;
 }
-template <> __device__ __forceinline__ Pk<4> ld<4>(const double *p, int i)
+template <int W, class H> __device__ __forceinline__ void st(double *p, int i, const Pk<W> &a, H h)
 {
-    const double2 t = *reinterpret_cast<const double2 *>(p + i);
-    const double2 u = *reinterpret_cast<const double2 *>(p + i + 2);
-    Pk<4> r; r.v[0] = t.x; r.v[1] = t.y; r.v[2] = u.x; r.v[3] = u.y; return r;
-}
-template <int W> __device__ __forceinline__ void st(double *p, int i, const Pk<W> &a);
-template <> __device__ __forceinline__ void st<1>(double *p, int i, const Pk<1> &a) { p[i] = a.v[0]; }
-template <> __device__ __forceinline__ void st<2>(double *p, int i, const Pk<2> &a)
-{
-    *reinterpret_cast<double2 *>(p + i) = make_double2(a.v[0], a.v[1]);
-}
-template <> __device__ __forceinline__ void st<4>(double *p, int i, const Pk<4> &a)
-{
-    *reinterpret_cast<double2 *>(p + i) = make_double2(a.v[0], a.v[1]);
-    *reinterpret_cast<double2 *>(p + i + 2) = make_double2(a.v[2], a.v[3]);
+    if constexpr (W == 1) {
+        st1(p + i, a.v[0], h);
+    } else {
+#pragma unroll
+        for (int k = 0; k < W; k += 2) st2(p + i + k, make_double2(a.v[k], a.v[k + 1]), h);
+    }
 }
 
 __host__ __device__ constexpr int phase_ndot(int ph)
@@ -40,52 +52,60 @@ __host__ __device__ constexpr int phase_ndot(int ph)
 
 
 // access policies: W contiguous doubles (vector loads), or W doubles STRIDE apart (one per step of a
-// thread-strided loop, so W independent loads are in flight per vector)
+// thread-strided loop, so W independent loads are in flight per vector); each access takes the L2 policy h
 template <int W_> struct Contig {
     static constexpr int W = W_;
-    static __device__ __forceinline__ Pk<W_> ld(const double *p, int i) { return bicg::ld<W_>(p, i); }
-    static __device__ __forceinline__ void st(double *p, int i, const Pk<W_> &a) { bicg::st<W_>(p, i, a); }
+    template <class H = Plain>
+    static __device__ __forceinline__ Pk<W_> ld(const double *p, int i, H h = {}) { return bicg::ld<W_>(p, i, h); }
+    template <class H = Plain>
+    static __device__ __forceinline__ void st(double *p, int i, const Pk<W_> &a, H h = {}) { bicg::st<W_>(p, i, a, h); }
 };
 template <int W_, int STRIDE> struct Strided {
     static constexpr int W = W_;
-    static __device__ __forceinline__ Pk<W_> ld(const double *p, int i)
+    template <class H = Plain>
+    static __device__ __forceinline__ Pk<W_> ld(const double *p, int i, H h = {})
     {
         Pk<W_> r;
 #pragma unroll
-        for (int k = 0; k < W_; ++k) r.v[k] = p[i + k * STRIDE];
+        for (int k = 0; k < W_; ++k) r.v[k] = ld1(p + i + k * STRIDE, h);
         return r;
     }
-    static __device__ __forceinline__ void st(double *p, int i, const Pk<W_> &a)
+    template <class H = Plain>
+    static __device__ __forceinline__ void st(double *p, int i, const Pk<W_> &a, H h = {})
     {
 #pragma unroll
-        for (int k = 0; k < W_; ++k) p[i + k * STRIDE] = a.v[k];
+        for (int k = 0; k < W_; ++k) st1(p + i + k * STRIDE, a.v[k], h);
     }
 };
 
 // K double2 accesses STRIDE doubles apart (persistent kernel: K independent 16-byte loads in flight per vector)
 template <int K, int STRIDE> struct Pairs {
     static constexpr int W = 2 * K;
-    static __device__ __forceinline__ Pk<W> ld(const double *p, int i)
+    template <class H = Plain>
+    static __device__ __forceinline__ Pk<W> ld(const double *p, int i, H h = {})
     {
         Pk<W> r;
 #pragma unroll
         for (int k = 0; k < K; ++k) {
-            const double2 t = *reinterpret_cast<const double2 *>(p + i + k * STRIDE);
+            const double2 t = ld2(p + i + k * STRIDE, h);
             r.v[2 * k] = t.x; r.v[2 * k + 1] = t.y;
         }
         return r;
     }
-    static __device__ __forceinline__ void st(double *p, int i, const Pk<W> &a)
+    template <class H = Plain>
+    static __device__ __forceinline__ void st(double *p, int i, const Pk<W> &a, H h = {})
     {
 #pragma unroll
-        for (int k = 0; k < K; ++k) *reinterpret_cast<double2 *>(p + i + k * STRIDE) = make_double2(a.v[2 * k], a.v[2 * k + 1]);
+        for (int k = 0; k < K; ++k) st2(p + i + k * STRIDE, make_double2(a.v[2 * k], a.v[2 * k + 1]), h);
     }
 };
 
 struct Coef { double al, be, om, nbo; };
 
-template <int PH, class L>
-__device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, double *dot)
+// far: the L2 policy of the accesses of PH_BICG_XR and PH_BICG_P whose next use is too far away for L2 to keep the vector
+// (mega.cu: run_bicgstab's table); every other access is plain
+template <int PH, class L, class F = Plain>
+__device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, double *dot, F far = {})
 {
     constexpr int W = L::W;
     if constexpr (PH == PH_BICG_INIT || PH == PH_INIT_R) {
@@ -103,7 +123,7 @@ __device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, dou
         for (int k = 0; k < W; ++k) r.v[k] = fma(-c.al, s.v[k], r.v[k]);
         L::st(v.r, i, r);
     } else if constexpr (PH == PH_BICG_XR) {
-        Pk<W> x = L::ld(v.x, i), p = L::ld(v.p, i), r = L::ld(v.r, i), y = L::ld(v.y, i), rh = L::ld(v.rh, i);
+        Pk<W> x = L::ld(v.x, i, far), p = L::ld(v.p, i), r = L::ld(v.r, i), y = L::ld(v.y, i, far), rh = L::ld(v.rh, i, far);
 #pragma unroll
         for (int k = 0; k < W; ++k) {
             x.v[k] = fma(c.al, p.v[k], x.v[k]);
@@ -112,9 +132,9 @@ __device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, dou
             dot[0] = fma(r.v[k], r.v[k], dot[0]);
             dot[1] = fma(rh.v[k], r.v[k], dot[1]);
         }
-        L::st(v.x, i, x); L::st(v.r, i, r);
+        L::st(v.x, i, x, far); L::st(v.r, i, r);
     } else if constexpr (PH == PH_BICG_P) {
-        Pk<W> p = L::ld(v.p, i), r = L::ld(v.r, i), s = L::ld(v.s, i);
+        Pk<W> p = L::ld(v.p, i), r = L::ld(v.r, i), s = L::ld(v.s, i, far);
 #pragma unroll
         for (int k = 0; k < W; ++k) {
             double t = c.be * p.v[k];
@@ -216,7 +236,7 @@ __device__ __forceinline__ void body(const VecPtrs &v, int i, const Coef &c, dou
             dot[4] = fma(r.v[k], r.v[k], dot[4]);
         }
     }
-    (void)v; (void)i; (void)c; (void)dot;
+    (void)v; (void)i; (void)c; (void)dot; (void)far;
 }
 
 
