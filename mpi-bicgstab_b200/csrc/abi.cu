@@ -1,6 +1,8 @@
 // abi.cu -- the extern "C" surface of libbicgstab_b200.so (include/bicgstab_b200.h).
 // Part 1: the reference's own entry points (solver.h:10-13, matrix.h:51) on host pointers.
-// Part 2: bicg_* extensions.
+// Part 2: bicg_* extensions: communication, options, the handle's lifetime, results of the last call, the library's stream
+// and host memory, and the calls around internal functions that other code calls too.  Every other bicg_* entry point on a
+// handle is defined in the file that does its work.
 #include "engine.hpp"
 
 #include <cmath>
@@ -210,26 +212,6 @@ void bicg_matrix_invalidate(const CSR_Matrix *diag)
     else c.cache[(const void *)m] = m;
 }
 
-int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, int device_vectors)
-{
-    return matrix_set_values(m, diag_val, offd_val, device_vectors != 0, false, nullptr);
-}
-int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream)
-{
-    return matrix_set_values(m, diag_val, offd_val, true, true, (cudaStream_t)stream);
-}
-int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma) { return matrix_shift_diagonal(m, sigma); }
-int bicg_matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, void *stream)
-{
-    return matrix_shift_diagonal_async(m, sigma, (cudaStream_t)stream);
-}
-int bicg_matrix_shift_diagonal_async_prepare(bicg_matrix *m) { return matrix_shift_diagonal_async_prepare(m); }
-bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m) { return matrix_create_transpose(m); }
-int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src) { return matrix_transpose_values(mt, src, false, nullptr); }
-int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream)
-{
-    return matrix_transpose_values(mt, src, true, (cudaStream_t)stream);
-}
 int bicg_matrix_block_nz(const bicg_matrix *m, unsigned *diag_nz, unsigned *offd_nz)
 {
     if (!m || !diag_nz || !offd_nz) return -1;
@@ -242,37 +224,7 @@ int bicg_solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nr
 {
     return solve(m, method, x, r, krr, nrr, device_vectors, stats);
 }
-int bicg_solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, void *stream, bicg_result *result)
-{
-    return solve_async(m, method, x, r, krr, nrr, (cudaStream_t)stream, result);
-}
-int bicg_solve_async_prepare(bicg_matrix *m, int method) { return solve_async_prepare(m, method); }
-int bicg_matrix_history(bicg_matrix *m, double *out, int cap) { return matrix_history(m, out, cap); }
 int bicg_spmv(bicg_matrix *m, const double *x_loc, double *y_loc) { return spmv_host(m, x_loc, y_loc, nullptr); }
-int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                         int device_vectors)
-{
-    return matrix_multiply(m, nvec, x, y, alpha, beta, sigma, device_vectors != 0);
-}
-int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                               void *stream)
-{
-    return matrix_multiply_async(m, nvec, x, y, alpha, beta, sigma, (cudaStream_t)stream);
-}
-int bicg_matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
-                           double *diag_out, double *offd_out, int device_vectors)
-{
-    return matrix_value_grad(m, nvec, u, v, alpha, beta, diag_out, offd_out, device_vectors != 0);
-}
-int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
-                                 double *diag_out, double *offd_out, void *stream)
-{
-    return matrix_value_grad_async(m, nvec, u, v, alpha, beta, diag_out, offd_out, (cudaStream_t)stream);
-}
-int bicg_matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, void *stream)
-{
-    return matrix_dots_async(m, nvec, u, v, out, (cudaStream_t)stream);
-}
 int bicg_shifted_solve(bicg_matrix *m, double *x_set, double *r, const double *sigma, int sigma_len, int seed, bicg_stats *stats)
 {
     Context &c = ctx();
@@ -292,28 +244,17 @@ int bicg_shifted_solve_dev(bicg_matrix *m, int method, double *x_set, double *r,
                            bicg_stats *stats)
 {
     Context &c = ctx();
-    // collective: a rank with bad arguments must not leave the others waiting for it in the solve's halo exchanges and
-    // reductions, so every rank learns every rank's verdict, method, sigma_len and seed before any of them starts
+    // collective (the solve's halo exchanges and reductions): every rank's verdict, method, sigma_len and seed
     const bool known = method == BICG_SHIFTED_SWITCHING || method == BICG_SHIFTED_LOP || method == BICG_SHIFTED_PIPE_LOP ||
                        method == BICG_SHIFTED_LOPBICG;
-    struct Args { int bad, method, len, seed; } mine{!m || !x_set || !r || !sigma || !known || sigma_len <= 0 || seed < 0 ||
-                                                     seed >= sigma_len, method, sigma_len, seed};
-    std::vector<Args> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(Args));
-    for (const Args &a : all)
-        if (a.bad || a.method != method || a.len != sigma_len || a.seed != seed) return -1;
+    if (!ranks_agree(!m || !x_set || !r || !sigma || !known || sigma_len <= 0 || seed < 0 || seed >= sigma_len,
+                     {method, sigma_len, seed}))
+        return -1;
     c.ensure();
     const int k = shifted_solve(m, method, x_set, r, sigma, sigma_len, seed, true);
     if (stats) *stats = c.last_stats;
     return k;
 }
-int bicg_shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
-                             void *stream, bicg_shift_result *result, int *stop_iter)
-{
-    return shifted_solve_async(m, method, x_set, r, sigma, sigma_len, seed, (cudaStream_t)stream, result, stop_iter);
-}
-int bicg_shifted_solve_async_prepare(bicg_matrix *m, int method, int sigma_len) { return shifted_async_prepare(m, method, sigma_len); }
-int bicg_matrix_shift_history(bicg_matrix *m, double *out, int cap) { return matrix_shift_history(m, out, cap); }
 int bicg_last_shift_info(int *seed, int *stop_iter, int cap)
 {
     Context &c = ctx();
@@ -333,13 +274,8 @@ int bicg_shift_residuals(bicg_matrix *m, const double *x_set, const double *b, c
                          double *out)
 {
     Context &c = ctx();
-    // collective: a rank with bad arguments must not leave the others waiting for it in the residual pass, so every rank
-    // learns every rank's verdict (and sigma_len, which must agree) before any of them starts
-    struct Args { int bad, len; } mine{sigma_len <= 0 || !m || !x_set || !b || !sigma || !out, sigma_len};
-    std::vector<Args> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(Args));
-    for (const Args &a : all)
-        if (a.bad || a.len != sigma_len) return -1;
+    // collective (the residual pass): every rank's verdict and sigma_len
+    if (!ranks_agree(sigma_len <= 0 || !m || !x_set || !b || !sigma || !out, {sigma_len})) return -1;
     c.ensure();
     const size_t n = (size_t)m->n_loc;
     const double *dx = x_set, *db = b;
@@ -355,7 +291,6 @@ int bicg_shift_residuals(bicg_matrix *m, const double *x_set, const double *b, c
     for (int j = 0; j < sigma_len; ++j) out[j] = err[(size_t)j];
     return 0;
 }
-int bicg_spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes) { return spmv_time(m, reps, ms, bytes); }
 
 int bicg_last_history(double *out, int cap)
 {

@@ -92,16 +92,15 @@ __global__ void __launch_bounds__(DOT_THREADS) dot_sum_kernel(const __grid_const
 
 } // namespace
 
-int matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, cudaStream_t st)
+} // namespace bicg
+
+extern "C" int bicg_matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, void *stream)
 {
+    using namespace bicg;
     if (!m || !u || !v || !out || nvec <= 0) return -1;
     Context &c = ctx();
     c.ensure();
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    async_handle_init(m);
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
+    const cudaStream_t st = (cudaStream_t)stream;
     PhaseLauncher pl(m, st);
     const long long n = m->n_loc;
     DotArgs a{};
@@ -109,23 +108,22 @@ int matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v
     a.nchunks = (int)((n + DOT_CHUNK - 1) / DOT_CHUNK);
     a.part = m->vec(V_T);              // MAX_DOTS * nchunks <= ghost_off doubles: 8 <= 16 for n <= DOT_CHUNK, else <= n / 512 + 8 < n
     const int grid = std::max(1, std::min(a.nchunks, c.sm_count * 8));
-    for (int j0 = 0; j0 < nvec; j0 += MAX_DOTS) {
-        const int nv = std::min(MAX_DOTS, nvec - j0);
-        a.nv = nv;
-        for (int k = 0; k < MAX_DOTS; ++k) {
-            a.u[k] = u + (j0 + std::min(k, nv - 1)) * n;
-            a.v[k] = v + (j0 + std::min(k, nv - 1)) * n;
+    stream_ordered({m}, st, capturing(st), [&] {
+        for (int j0 = 0; j0 < nvec; j0 += MAX_DOTS) {
+            const int nv = std::min(MAX_DOTS, nvec - j0);
+            a.nv = nv;
+            for (int k = 0; k < MAX_DOTS; ++k) {
+                a.u[k] = u + (j0 + std::min(k, nv - 1)) * n;
+                a.v[k] = v + (j0 + std::min(k, nv - 1)) * n;
+            }
+            a.out = out + j0;
+            a.kc = pl.common(tail_store(nv));
+            if (a.nchunks) dot_chunk_kernel<<<grid, DOT_THREADS, 0, st>>>(a);
+            BICG_CUDA(cudaGetLastError());
+            dot_sum_kernel<<<1, DOT_THREADS, 0, st>>>(a);
+            BICG_CUDA(cudaGetLastError());
+            c.launches += 2;
         }
-        a.out = out + j0;
-        a.kc = pl.common(tail_store(nv));
-        if (a.nchunks) dot_chunk_kernel<<<grid, DOT_THREADS, 0, st>>>(a);
-        BICG_CUDA(cudaGetLastError());
-        dot_sum_kernel<<<1, DOT_THREADS, 0, st>>>(a);
-        BICG_CUDA(cudaGetLastError());
-        c.launches += 2;
-    }
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    });
     return 0;
 }
-
-} // namespace bicg

@@ -298,31 +298,32 @@ bicg_matrix *matrix_create(const CSR_Matrix *diag, const CSR_Matrix *offd, const
 void matrix_destroy(bicg_matrix *m);
 double matrix_upload_ms(bicg_matrix *m);
 bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, bool *fresh);
-// bicg_matrix_set_values (async = false: on the library's stream, returns once done) and bicg_matrix_set_values_async (on st)
-int  matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st);
-int  matrix_shift_diagonal(bicg_matrix *m, double sigma);     // bicg_matrix_shift_diagonal
-// bicg_matrix_shift_diagonal_async (on st) and its prepare step
-int  matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, cudaStream_t st);
-int  matrix_shift_diagonal_async_prepare(bicg_matrix *m);
 // the persistent kernel's value tables and packed values from d_val, on st: what creation and every value update run last
 void launch_value_tables(const bicg_matrix *m, cudaStream_t st);
-// transpose.cu: bicg_matrix_create_transpose, bicg_matrix_transpose_values (async = false: on the library's stream, returns
-// once done) and bicg_matrix_transpose_values_async (on st)
-bicg_matrix *matrix_create_transpose(bicg_matrix *m);
-int  matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src, bool async, cudaStream_t st);
 // solve.cu
 int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *st);
-// bicg_solve_async / bicg_solve_async_prepare / bicg_matrix_history (include/bicgstab_b200.h)
-int  solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, cudaStream_t st, bicg_result *result);
-int  solve_async_prepare(bicg_matrix *m, int method);
-int  matrix_history(bicg_matrix *m, double *out, int cap);
-// every synchronous entry point that touches a handle first makes the library's stream wait for the handle's last
-// asynchronous work (free when there is none)
+
+// calls.cu: what the entry points on a handle do around their work.
+// Every synchronous entry point that touches a handle first makes the library's stream wait for the handle's last
+// asynchronous work (free when there is none).
 void wait_handle(bicg_matrix *m);
-void drop_async_loop(AsyncLoop &L);        // frees the prepared kernel-per-phase loop of one method
-// The device-side loop of every kernel-per-phase solve, shared by solve.cu and the shifted solvers.  async_handle_init: the
-// handle's first asynchronous use (its last-work event, recorded on the library's stream).
+// the handle's first asynchronous use: creates its last-work event, recorded on the library's stream
 void async_handle_init(bicg_matrix *m);
+bool capturing(cudaStream_t st);           // st is capturing into a graph
+// An asynchronous call's work on st: st waits for the last work of every handle, enqueue() runs, and its work becomes the
+// last work of every handle.  captured: the wait and the record are external nodes of the capture, so that every replay waits
+// for the handles' last work at replay time and later calls wait for the replay.
+void stream_ordered(std::initializer_list<bicg_matrix *> handles, cudaStream_t st, bool captured, const std::function<void()> &enqueue);
+// Collective, host only: false on every rank when any rank is bad or passed other `same` values than this one.  A rank with bad
+// arguments must not leave the others waiting for it in collective work on the device.
+bool ranks_agree(bool bad, std::initializer_list<long long> same);
+// a device-side wait for a peer or another CTA timed out (Scalars::error) during the operation `during`: exit(1)
+[[noreturn]] void timeout_fatal(const bicg_matrix *m, const char *during);
+// the end of a synchronous call: synchronises the library's stream, then timeout_fatal if m's Scalars::error is set
+void sync_checked(bicg_matrix *m, const char *during);
+
+void drop_async_loop(AsyncLoop &L);        // frees the prepared kernel-per-phase loop of one method
+// The device-side loop of every kernel-per-phase solve, shared by solve.cu and the shifted solvers.
 cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args);
 cudaGraphNode_t add_conditional_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, cudaGraphConditionalHandle h,
                                      cudaGraphConditionalNodeType type, cudaGraph_t *body);
@@ -334,14 +335,8 @@ cudaGraphNode_t add_while_node(bicg_matrix *m, cudaGraph_t g, const cudaGraphNod
 // capture, or else the prepared executable graph `exec` of that node
 void enqueue_while(bicg_matrix *m, cudaStream_t st, int batches, int krr, int nrr, cudaGraphExec_t exec,
                    const std::function<cudaGraphNode_t(cudaGraph_t, const cudaGraphNode_t *, size_t)> &add);
-// bicg_shifted_solve_async / _prepare / bicg_matrix_shift_history (shifted.cu)
-int  shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int sigma_len, int seed,
-                         cudaStream_t st, bicg_shift_result *result, int *stop_iter);
-int  shifted_async_prepare(bicg_matrix *m, int method, int sigma_len);
-int  matrix_shift_history(bicg_matrix *m, double *out, int cap);
-void drop_shift_work(bicg_matrix *m);      // matrix_destroy: every workspace, its graphs and the retired buffers
+void drop_shift_work(bicg_matrix *m);      // matrix_destroy: every workspace, its graphs and the retired buffers (shifted.cu)
 int  spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full_or_null);
-int  spmv_time(bicg_matrix *m, int reps, double *ms, double *bytes);
 void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist);
 void print_times(double seconds, double iters);          // "Total time" / "Avg time/iter" (= seconds / iters), then flush
 void reset_scalars(bicg_matrix *m, double tol, int max_iter);   // Scalars of a new solve (enqueued on the stream)
@@ -359,20 +354,6 @@ std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long 
 std::vector<double> shift_relative_errors(bicg_matrix *m, const double *d_x, long long ldx, const double *d_b, const double *sigma, int L);
 // an empty cross-GPU reduction on st: every rank has finished what it enqueued on the handle before (with peers only)
 void peer_barrier(bicg_matrix *m, cudaStream_t st);
-// multiply.cu: bicg_matrix_multiply (device_vectors: x, y are device pointers; sigma is a host array) and
-// bicg_matrix_multiply_async (x, y and sigma device pointers, on st)
-int  matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                     bool device_vectors);
-int  matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                           cudaStream_t st);
-// value_grad.cu: bicg_matrix_value_grad (device_vectors: u, v, diag_out and offd_out are device pointers) and
-// bicg_matrix_value_grad_async (device pointers, on st)
-int  matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta, double *diag_out,
-                       double *offd_out, bool device_vectors);
-int  matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
-                             double *diag_out, double *offd_out, cudaStream_t st);
-// dots.cu: bicg_matrix_dots_async (device pointers, on st)
-int  matrix_dots_async(bicg_matrix *m, int nvec, const double *u, const double *v, double *out, cudaStream_t st);
 // helpers shared by matrix.cu / solve.cu
 SpmvArgs make_spmv_args(const bicg_matrix *m, const SpmvPlan &p, int x_id, int y_id);
 void launch_spmv_plan(const bicg_matrix *m, const SpmvPlan &p, const SpmvArgs &a, cudaStream_t st, int prof_class = 0);

@@ -986,127 +986,6 @@ void matrix_destroy(bicg_matrix *m)
     delete m;
 }
 
-// ------------------------------------------------------------------------------------------------
-// value updates: everything but d_val and what matrix_create derived from it (the value tables and packed values of the
-// persistent kernel's plan) depends on the pattern alone and stays
-// ------------------------------------------------------------------------------------------------
-int matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, bool async, cudaStream_t st)
-{
-    if (!m || !diag_val) return -1;
-    Context &c = ctx();
-    c.ensure();
-    const size_t no = m->nnz_offd, nd = m->nnz - no;
-    if (no && !offd_val) return -1;
-    bool captured = false;
-    if (async) {
-        cudaStreamCaptureStatus cs;
-        BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-        captured = cs != cudaStreamCaptureStatusNone;
-        async_handle_init(m);
-        BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    } else {
-        wait_handle(m);
-        st = c.stream;
-    }
-    double *stage = nullptr;                  // host values with offd entries: staged through a pool block, as at creation
-    if (!device_ptrs && no) {
-        stage = (double *)c.dev_alloc((nd + no) * sizeof(double));
-        if (nd) c.h2d(stage, diag_val, nd * sizeof(double));
-        c.h2d(stage + nd, offd_val, no * sizeof(double));
-        diag_val = stage; offd_val = stage + nd;
-    }
-    if (!no) {
-        if (nd && device_ptrs) BICG_CUDA(cudaMemcpyAsync(m->d_val, diag_val, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        else if (nd) c.h2d(m->d_val, diag_val, nd * sizeof(double));
-    } else {
-        const size_t np1 = (size_t)m->n_loc + 1;
-        merge_values_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_blk_ptr, m->d_blk_ptr + np1, diag_val, offd_val, m->d_val);
-        BICG_CUDA(cudaGetLastError());
-    }
-    launch_value_tables(m, st);
-    if (async) {
-        BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
-    } else {
-        BICG_CUDA(cudaStreamSynchronize(c.stream));
-        c.dev_free(stage);
-    }
-    return 0;
-}
-
-// d_diag_pos and diag_missing, found at the first call (on the library's stream, synchronising); the pattern never changes
-static void find_diag_pos(bicg_matrix *m)
-{
-    if (m->d_diag_pos) return;
-    Context &c = ctx();
-    m->d_diag_pos = (int *)c.dev_alloc(((size_t)m->n_loc + 1) * sizeof(int));      // + the count of rows without one
-    int missing = 0;
-    BICG_CUDA(cudaMemsetAsync(m->d_diag_pos + m->n_loc, 0, sizeof(int), c.stream));
-    diag_pos_kernel<<<row_blocks(m->n_loc), 256, 0, c.stream>>>(m->n_loc, m->d_ptr, m->d_col, m->d_diag_pos, m->d_diag_pos + m->n_loc);
-    BICG_CUDA(cudaGetLastError());
-    BICG_CUDA(cudaMemcpyAsync(&missing, m->d_diag_pos + m->n_loc, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    m->diag_missing = missing > 0;
-}
-
-int matrix_shift_diagonal(bicg_matrix *m, double sigma)
-{
-    if (!m) return -1;
-    Context &c = ctx();
-    c.ensure();
-    wait_handle(m);
-    const int blocks = row_blocks(m->n_loc);
-    find_diag_pos(m);
-    if (m->diag_missing) return -1;           // the reference exits here (matrix.c:547-550); nothing has been changed
-    shift_diag_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
-    BICG_CUDA(cudaGetLastError());
-    launch_value_tables(m, c.stream);
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    return 0;
-}
-
-int matrix_shift_diagonal_async_prepare(bicg_matrix *m)
-{
-    Context &c = ctx();
-    // collective: a rank that refuses must not leave the others waiting in the collective work that follows a shift
-    int bad = 1;
-    if (m) {
-        c.ensure();
-        wait_handle(m);
-        find_diag_pos(m);
-        bad = m->diag_missing ? 1 : 0;
-    }
-    std::vector<int> all((size_t)c.world);
-    c.host_allgather(&bad, all.data(), sizeof(int));
-    bool any = false;
-    for (int b : all) any = any || b != 0;
-    if (!m) return -1;
-    m->diag_prepared = true;
-    m->diag_refused = any;
-    return any ? -1 : 0;
-}
-
-int matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, cudaStream_t st)
-{
-    if (!m || !sigma) return -1;
-    Context &c = ctx();
-    c.ensure();
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    if (!m->diag_prepared) {
-        if (captured) return -2;
-        if (matrix_shift_diagonal_async_prepare(m) != 0) return -1;
-    }
-    if (m->diag_missing || m->diag_refused) return -1;        // nothing has been changed
-    async_handle_init(m);
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    shift_diag_dev_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
-    BICG_CUDA(cudaGetLastError());
-    launch_value_tables(m, st);
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
-    return 0;
-}
-
 // Content fingerprint of the caller's blocks: sizes + up to 8192 evenly spaced samples of val / col / ptr of both blocks
 // (FNV-1a).  The upload cache is keyed by the host pointer; the fingerprint catches what the pointer cannot -- a
 // different matrix in a recycled allocation, or values changed in place everywhere (diagonal shift, rescaling:
@@ -1164,4 +1043,126 @@ bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, c
     return m;
 }
 
+// ------------------------------------------------------------------------------------------------
+// value updates: everything but d_val and what matrix_create derived from it (the value tables and packed values of the
+// persistent kernel's plan) depends on the pattern alone and stays
+// ------------------------------------------------------------------------------------------------
+// d_val from the caller's values (device pointers, or host pointers when there are no offd entries), then the value tables, on st
+static void enqueue_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, cudaStream_t st)
+{
+    const size_t no = m->nnz_offd, nd = m->nnz - no;
+    if (!no) {
+        if (nd && device_ptrs) BICG_CUDA(cudaMemcpyAsync(m->d_val, diag_val, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        else if (nd) ctx().h2d(m->d_val, diag_val, nd * sizeof(double));
+    } else {
+        const size_t np1 = (size_t)m->n_loc + 1;
+        merge_values_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_blk_ptr, m->d_blk_ptr + np1, diag_val, offd_val, m->d_val);
+        BICG_CUDA(cudaGetLastError());
+    }
+    launch_value_tables(m, st);
+}
+
+// d_diag_pos and diag_missing, found at the first call (on the library's stream, synchronising); the pattern never changes
+static void find_diag_pos(bicg_matrix *m)
+{
+    if (m->d_diag_pos) return;
+    Context &c = ctx();
+    m->d_diag_pos = (int *)c.dev_alloc(((size_t)m->n_loc + 1) * sizeof(int));      // + the count of rows without one
+    int missing = 0;
+    BICG_CUDA(cudaMemsetAsync(m->d_diag_pos + m->n_loc, 0, sizeof(int), c.stream));
+    diag_pos_kernel<<<row_blocks(m->n_loc), 256, 0, c.stream>>>(m->n_loc, m->d_ptr, m->d_col, m->d_diag_pos, m->d_diag_pos + m->n_loc);
+    BICG_CUDA(cudaGetLastError());
+    BICG_CUDA(cudaMemcpyAsync(&missing, m->d_diag_pos + m->n_loc, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    m->diag_missing = missing > 0;
+}
+
 } // namespace bicg
+
+extern "C" int bicg_matrix_set_values(bicg_matrix *m, const double *diag_val, const double *offd_val, int device_vectors)
+{
+    using namespace bicg;
+    if (!m || !diag_val) return -1;
+    Context &c = ctx();
+    c.ensure();
+    const size_t no = m->nnz_offd, nd = m->nnz - no;
+    if (no && !offd_val) return -1;
+    wait_handle(m);
+    double *stage = nullptr;                  // host values with offd entries: staged through a pool block, as at creation
+    if (!device_vectors && no) {
+        stage = (double *)c.dev_alloc((nd + no) * sizeof(double));
+        if (nd) c.h2d(stage, diag_val, nd * sizeof(double));
+        c.h2d(stage + nd, offd_val, no * sizeof(double));
+        diag_val = stage; offd_val = stage + nd;
+    }
+    enqueue_values(m, diag_val, offd_val, device_vectors != 0, c.stream);
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    c.dev_free(stage);
+    return 0;
+}
+
+extern "C" int bicg_matrix_set_values_async(bicg_matrix *m, const double *diag_val, const double *offd_val, void *stream)
+{
+    using namespace bicg;
+    if (!m || !diag_val) return -1;
+    ctx().ensure();
+    if (m->nnz_offd && !offd_val) return -1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    stream_ordered({m}, st, capturing(st), [&] { enqueue_values(m, diag_val, offd_val, true, st); });
+    return 0;
+}
+
+extern "C" int bicg_matrix_shift_diagonal(bicg_matrix *m, double sigma)
+{
+    using namespace bicg;
+    if (!m) return -1;
+    Context &c = ctx();
+    c.ensure();
+    wait_handle(m);
+    const int blocks = row_blocks(m->n_loc);
+    find_diag_pos(m);
+    if (m->diag_missing) return -1;           // the reference exits here (matrix.c:547-550); nothing has been changed
+    shift_diag_kernel<<<blocks, 256, 0, c.stream>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
+    BICG_CUDA(cudaGetLastError());
+    launch_value_tables(m, c.stream);
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    return 0;
+}
+
+extern "C" int bicg_matrix_shift_diagonal_async_prepare(bicg_matrix *m)
+{
+    using namespace bicg;
+    // collective: a rank that refuses must not leave the others waiting in the collective work that follows a shift
+    bool bad = true;
+    if (m) {
+        ctx().ensure();
+        wait_handle(m);
+        find_diag_pos(m);
+        bad = m->diag_missing;
+    }
+    const bool agree = ranks_agree(bad, {});
+    if (!m) return -1;
+    m->diag_prepared = true;
+    m->diag_refused = !agree;
+    return agree ? 0 : -1;
+}
+
+extern "C" int bicg_matrix_shift_diagonal_async(bicg_matrix *m, const double *sigma, void *stream)
+{
+    using namespace bicg;
+    if (!m || !sigma) return -1;
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool captured = capturing(st);
+    if (!m->diag_prepared) {
+        if (captured) return -2;
+        if (bicg_matrix_shift_diagonal_async_prepare(m) != 0) return -1;
+    }
+    if (m->diag_missing || m->diag_refused) return -1;        // nothing has been changed
+    stream_ordered({m}, st, captured, [&] {
+        shift_diag_dev_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_diag_pos, sigma, m->d_val);
+        BICG_CUDA(cudaGetLastError());
+        launch_value_tables(m, st);
+    });
+    return 0;
+}

@@ -91,17 +91,15 @@ void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, doub
 
 } // namespace
 
-int matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                    bool device_vectors)
+} // namespace bicg
+
+extern "C" int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
+                                    const double *sigma, int device_vectors)
 {
+    using namespace bicg;
     Context &c = ctx();
-    // collective: a rank with bad arguments must not leave the others waiting for it in the halo exchange and the barrier, so
-    // every rank learns every rank's verdict, nvec and whether it passed sigma before any of them starts
-    struct Args { int bad, nvec, shifted; } mine{bad_args(m, nvec, x, y) ? 1 : 0, nvec, sigma ? 1 : 0};
-    std::vector<Args> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(Args));
-    for (const Args &o : all)
-        if (o.bad || o.nvec != nvec || o.shifted != mine.shifted) return -1;
+    // collective (the halo exchange and the barrier): every rank's verdict, nvec and whether it passed sigma
+    if (!ranks_agree(bad_args(m, nvec, x, y), {nvec, sigma ? 1 : 0})) return -1;
     c.ensure();
     wait_handle(m);
     const size_t bytes = (size_t)nvec * (size_t)m->n_loc * sizeof(double);
@@ -119,28 +117,18 @@ int matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double
     }
     enqueue_multiply(m, nvec, dx, dy, alpha, beta, d_sigma, c.stream);
     if (!device_vectors) BICG_CUDA(cudaMemcpyAsync(y, dy, bytes, cudaMemcpyDeviceToHost, c.stream));
-    int error = 0;
-    BICG_CUDA(cudaMemcpyAsync(&error, &m->d_sc->error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU during a multiply", m->rank);
+    sync_checked(m, "a multiply");
     c.dev_free(tmp); c.dev_free(d_sigma);
     return 0;
 }
 
-int matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                          cudaStream_t st)
+extern "C" int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
+                                          const double *sigma, void *stream)
 {
+    using namespace bicg;
     if (bad_args(m, nvec, x, y)) return -1;
-    Context &c = ctx();
-    c.ensure();
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    async_handle_init(m);
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    enqueue_multiply(m, nvec, x, y, alpha, beta, sigma, st);
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    stream_ordered({m}, st, capturing(st), [&] { enqueue_multiply(m, nvec, x, y, alpha, beta, sigma, st); });
     return 0;
 }
-
-} // namespace bicg

@@ -192,7 +192,7 @@ std::vector<double> shift_residual_sums(bicg_matrix *m, const double *d_x, long 
     Scalars hs{};
     if (peers) BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted residual check", m->rank);
+    if (hs.error) timeout_fatal(m, "the shifted residual check");
     c.dev_free(d_sigma); c.dev_free(d_part); c.dev_free(d_sum);
     c.host_allgather(mine.data(), all.data(), (size_t)W * sizeof(double));
     std::vector<double> tot(all.begin(), all.begin() + W);

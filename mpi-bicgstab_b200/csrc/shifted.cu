@@ -592,57 +592,64 @@ int shifted_solve(bicg_matrix *m, int method, double *x_set, double *r, const do
     }
 }
 
-int shifted_async_prepare(bicg_matrix *m, int method, int L)
+void drop_shift_work(bicg_matrix *m)
 {
     Context &c = ctx();
-    // collective, as bicg_shifted_solve_dev: every rank learns every rank's verdict, method and sigma_len
-    struct Args { int bad, method, len; } mine{!m || !shift_method_known(method) || L <= 0, method, L};
-    std::vector<Args> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(Args));
-    for (const Args &a : all)
-        if (a.bad || a.method != method || a.len != L) return -1;
-    c.ensure();
-    async_handle_init(m);
-    // what this enqueues on the library's stream (the history record's and the template's initial values) goes behind the
-    // handle's last work and ahead of the next call on it
-    wait_handle(m);
-    if (!m->d_shift_last) {
-        m->d_shift_last = (ShiftHistRef *)c.dev_alloc(sizeof(ShiftHistRef));
-        BICG_CUDA(cudaMemsetAsync(m->d_shift_last, 0, sizeof(ShiftHistRef), c.stream));
-    }
-    shift_work(m, method, L);
-    BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
-    return 0;
+    for (ShiftWork &ws : m->shift_ws) drop_work(m, ws, false);
+    for (void *p : m->shift_retired) c.dev_free(p);
+    m->shift_retired.clear();
+    if (m->d_shift_last) c.dev_free(m->d_shift_last);
+    m->d_shift_last = nullptr;
 }
-int shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed,
-                        cudaStream_t st, bicg_shift_result *result, int *stop_iter)
+
+} // namespace bicg
+
+extern "C" int bicg_shifted_solve_async_prepare(bicg_matrix *m, int method, int L)
 {
+    using namespace bicg;
     Context &c = ctx();
+    // collective, as bicg_shifted_solve_dev: every rank's verdict, method and sigma_len
+    if (!ranks_agree(!m || !shift_method_known(method) || L <= 0, {method, L})) return -1;
     c.ensure();
-    if (!m || !x_set || !r || !sigma || !shift_method_known(method) || L <= 0 || seed < 0 || seed >= L) return -1;
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    if (!shift_async_prepared(m, method, L)) {
-        if (captured) return -2;
-        if (shifted_async_prepare(m, method, L) != 0) return -1;
-    }
-    // the order of the plain asynchronous solve (solve_async): behind the handle's last work, which this call then is
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    if (captured) m->captured = true;
-    ShiftWork &ws = m->shift_ws[shift_family(method)];
-    switch (method) {
-    case BICG_SHIFTED_SWITCHING: switching_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
-    case BICG_SHIFTED_LOPBICG:   switching_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
-    case BICG_SHIFTED_LOP:       lop_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
-    default:                     lop_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
-    }
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    // on the library's stream: the history record's and the template's initial values
+    stream_ordered({m}, c.stream, false, [&] {
+        if (!m->d_shift_last) {
+            m->d_shift_last = (ShiftHistRef *)c.dev_alloc(sizeof(ShiftHistRef));
+            BICG_CUDA(cudaMemsetAsync(m->d_shift_last, 0, sizeof(ShiftHistRef), c.stream));
+        }
+        shift_work(m, method, L);
+    });
     return 0;
 }
 
-int matrix_shift_history(bicg_matrix *m, double *out, int cap)
+extern "C" int bicg_shifted_solve_async(bicg_matrix *m, int method, double *x_set, double *r, const double *sigma, int L, int seed,
+                                        void *stream, bicg_shift_result *result, int *stop_iter)
 {
+    using namespace bicg;
+    ctx().ensure();
+    if (!m || !x_set || !r || !sigma || !shift_method_known(method) || L <= 0 || seed < 0 || seed >= L) return -1;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool captured = capturing(st);
+    if (!shift_async_prepared(m, method, L)) {
+        if (captured) return -2;
+        if (bicg_shifted_solve_async_prepare(m, method, L) != 0) return -1;
+    }
+    if (captured) m->captured = true;
+    ShiftWork &ws = m->shift_ws[shift_family(method)];
+    stream_ordered({m}, st, captured, [&] {
+        switch (method) {
+        case BICG_SHIFTED_SWITCHING: switching_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
+        case BICG_SHIFTED_LOPBICG:   switching_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
+        case BICG_SHIFTED_LOP:       lop_solve_async(m, ws, false, x_set, r, sigma, seed, st, result, stop_iter); break;
+        default:                     lop_solve_async(m, ws, true, x_set, r, sigma, seed, st, result, stop_iter); break;
+        }
+    });
+    return 0;
+}
+
+extern "C" int bicg_matrix_shift_history(bicg_matrix *m, double *out, int cap)
+{
+    using namespace bicg;
     Context &c = ctx();
     c.ensure();
     if (!m) return -1;
@@ -657,15 +664,3 @@ int matrix_shift_history(bicg_matrix *m, double *out, int cap)
     }
     return ref.n;
 }
-
-void drop_shift_work(bicg_matrix *m)
-{
-    Context &c = ctx();
-    for (ShiftWork &ws : m->shift_ws) drop_work(m, ws, false);
-    for (void *p : m->shift_retired) c.dev_free(p);
-    m->shift_retired.clear();
-    if (m->d_shift_last) c.dev_free(m->d_shift_last);
-    m->d_shift_last = nullptr;
-}
-
-} // namespace bicg

@@ -172,7 +172,7 @@ struct ShiftedSolve {
         AsyncLoopState ls;
         BICG_CUDA(cudaMemcpyAsync(&ls, m->d_loop, sizeof(AsyncLoopState), cudaMemcpyDeviceToHost, st));
         BICG_CUDA(cudaStreamSynchronize(st));
-        if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU in the shifted solver", m->rank);
+        if (hs.error) timeout_fatal(m, "a shifted solve");
         bodies = ls.count;
         BICG_CUDA(cudaEventElapsedTime(&ms, e0, e1));
         cudaEventDestroy(e0); cudaEventDestroy(e1);

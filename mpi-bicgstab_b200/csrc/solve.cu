@@ -104,23 +104,6 @@ void drop_async_loop(AsyncLoop &L)
     L = AsyncLoop();
 }
 
-void wait_handle(bicg_matrix *m)
-{
-    if (m && m->ev_last) BICG_CUDA(cudaStreamWaitEvent(ctx().stream, m->ev_last, 0));
-}
-
-void async_handle_init(bicg_matrix *m)
-{
-    Context &c = ctx();
-    if (!m->ev_last) {
-        // the handle's first asynchronous use: matrix_create returns with the upload and the plan's encoding kernels still in
-        // flight on the library's stream, and a synchronous call may have left work there too, so the handle's last work
-        // starts out as everything enqueued on that stream so far
-        BICG_CUDA(cudaEventCreateWithFlags(&m->ev_last, cudaEventDisableTiming));
-        BICG_CUDA(cudaEventRecord(m->ev_last, c.stream));
-    }
-}
-
 cudaGraphNode_t add_kernel_node(cudaGraph_t g, const cudaGraphNode_t *deps, size_t ndeps, const void *fn, void **args)
 {
     cudaKernelNodeParams p{};
@@ -524,12 +507,6 @@ void print_reference_lines(const bicg_stats &st, const std::vector<double> &hist
 
 namespace {
 
-[[noreturn]] void timeout_fatal(const bicg_matrix *m)
-{
-    fatal("bicgstab_b200: rank %d timed out after %d s waiting for a peer GPU / another CTA (halo flag or reduction "
-          "mailbox; BICG_PEER_TIMEOUT_S raises the bound)", m->rank, ctx().cfg.peer_timeout_s);
-}
-
 // The enqueue half of a solve on stream `st`: inputs, scalars, the init phases, the loop, the outputs.  marks: four events
 // recorded before and after the inputs, after the loop and after the outputs (bicg_solve's timing), or null.  The loop is the
 // persistent kernel where it runs, else the WHILE node of the kernel-per-phase loop; bicg_profile_solve (Context::prof_on)
@@ -608,7 +585,7 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     if (device_loop) BICG_CUDA(cudaMemcpyAsync(&ls, m->d_loop, sizeof(AsyncLoopState), cudaMemcpyDeviceToHost, c.stream));
     BICG_CUDA(cudaStreamSynchronize(c.stream));
 
-    if (hs.error) timeout_fatal(m);
+    if (hs.error) timeout_fatal(m, "a solve");
     if (m->d_trace && use_mega && method == BICG_METHOD_BICGSTAB) {
         // BICG_MEGA_TRACE=1: where CTA 0 and the middle CTA of the persistent kernel spent their time, averaged over the iterations
         const int iters = std::min(hs.k - 1, (int)MEGA_TRACE_ITERS);
@@ -682,56 +659,6 @@ int solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, in
     return st.iters;
 }
 
-int solve_async_prepare(bicg_matrix *m, int method)
-{
-    Context &c = ctx();
-    c.ensure();
-    if (!m || method < 0 || method > 3) return -1;
-    ensure_hist(m, c.cfg.max_iter);
-    async_handle_init(m);
-    if (method == BICG_METHOD_PIPE_RR) prepare_device_loop(m, BICG_METHOD_PIPE);    // what PIPE_RR with krr <= 0 runs
-    prepare_device_loop(m, method);
-    return 0;
-}
-
-int solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, cudaStream_t st, bicg_result *result)
-{
-    Context &c = ctx();
-    c.ensure();
-    if (!m || !x || !r || method < 0 || method > 3) return -1;
-    if (method == BICG_METHOD_PIPE_RR && krr <= 0) method = BICG_METHOD_PIPE;
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    if (!captured) solve_async_prepare(m, method);
-    else if (!async_prepared(m, method)) return -2;
-    // the handle's device state is shared by every call on it; inside a capture the wait and the record become nodes that
-    // order the replays behind the handle's last work at replay time
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    if (captured) m->captured = true;
-    enqueue_solve(m, method, x, r, krr, nrr, true, st, nullptr);
-    if (result) result_kernel<<<1, 1, 0, st>>>(m->d_sc, result);
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
-    return 0;
-}
-
-int matrix_history(bicg_matrix *m, double *out, int cap)
-{
-    Context &c = ctx();
-    c.ensure();
-    wait_handle(m);
-    Scalars hs;
-    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (hs.error) timeout_fatal(m);
-    const int n = hs.k + 1;
-    if (out && cap > 0) {
-        BICG_CUDA(cudaMemcpyAsync(out, m->d_hist, (size_t)std::min(n, cap) * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
-        BICG_CUDA(cudaStreamSynchronize(c.stream));
-    }
-    return n;
-}
-
 // y_loc = A x_loc with host pointers (the kernel behind MPI_csr_spmv_ovlap, matrix.c:428-441)
 int spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full)
 {
@@ -749,10 +676,7 @@ int spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full
     // MPI_Iallgatherv it replaces (matrix.c:432).
     seq.spmv(V_X, V_AX, m->world > 1 ? tail_allreduce(FIN_NONE, 0) : tail_none());
     BICG_CUDA(cudaMemcpyAsync(y_loc, m->vec(V_AX), vbytes, cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    Scalars hs;
-    BICG_CUDA(cudaMemcpy(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost));
-    if (hs.error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU during SpMV", m->rank);
+    sync_checked(m, "an SpMV");
     if (x_full) {
         // the reference leaves the gathered vector in the caller's scratch (matrix.c:432); we only ever hold
         // the own part plus the halo, so fill what we have: own rows, then the received ghost runs
@@ -769,8 +693,62 @@ int spmv_host(bicg_matrix *m, const double *x_loc, double *y_loc, double *x_full
     return 0;
 }
 
-int spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
+} // namespace bicg
+
+extern "C" int bicg_solve_async_prepare(bicg_matrix *m, int method)
 {
+    using namespace bicg;
+    Context &c = ctx();
+    c.ensure();
+    if (!m || method < 0 || method > 3) return -1;
+    ensure_hist(m, c.cfg.max_iter);
+    async_handle_init(m);
+    if (method == BICG_METHOD_PIPE_RR) prepare_device_loop(m, BICG_METHOD_PIPE);    // what PIPE_RR with krr <= 0 runs
+    prepare_device_loop(m, method);
+    return 0;
+}
+
+extern "C" int bicg_solve_async(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, void *stream,
+                                bicg_result *result)
+{
+    using namespace bicg;
+    Context &c = ctx();
+    c.ensure();
+    if (!m || !x || !r || method < 0 || method > 3) return -1;
+    if (method == BICG_METHOD_PIPE_RR && krr <= 0) method = BICG_METHOD_PIPE;
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool captured = capturing(st);
+    if (!captured) bicg_solve_async_prepare(m, method);
+    else if (!async_prepared(m, method)) return -2;
+    if (captured) m->captured = true;
+    stream_ordered({m}, st, captured, [&] {
+        enqueue_solve(m, method, x, r, krr, nrr, true, st, nullptr);
+        if (result) result_kernel<<<1, 1, 0, st>>>(m->d_sc, result);
+    });
+    return 0;
+}
+
+extern "C" int bicg_matrix_history(bicg_matrix *m, double *out, int cap)
+{
+    using namespace bicg;
+    Context &c = ctx();
+    c.ensure();
+    wait_handle(m);
+    Scalars hs;
+    BICG_CUDA(cudaMemcpyAsync(&hs, m->d_sc, sizeof(Scalars), cudaMemcpyDeviceToHost, c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
+    if (hs.error) timeout_fatal(m, "the last solve on the handle");
+    const int n = hs.k + 1;
+    if (out && cap > 0) {
+        BICG_CUDA(cudaMemcpyAsync(out, m->d_hist, (size_t)std::min(n, cap) * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
+        BICG_CUDA(cudaStreamSynchronize(c.stream));
+    }
+    return n;
+}
+
+extern "C" int bicg_spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
+{
+    using namespace bicg;
     Context &c = ctx();
     c.ensure();
     wait_handle(m);
@@ -796,8 +774,6 @@ int spmv_time(bicg_matrix *m, int reps, double *ms_out, double *bytes_out)
     if (bytes_out) *bytes_out = 12.0 * (double)m->nnz + 28.0 * (double)m->n_loc;
     return 0;
 }
-
-} // namespace bicg
 
 // ------------------------------------------------------------------------------------------------
 // test hooks (K-level parity: single fused phases and epilogue dots on caller-supplied vectors; single rank)

@@ -66,6 +66,12 @@ void enqueue_refresh(bicg_matrix *mt, const bicg_matrix *src, cudaStream_t st)
     launch_value_tables(mt, st);
 }
 
+// the -1 case of both refresh calls: mt is not a transpose of src
+bool transpose_bad(const bicg_matrix *mt, const bicg_matrix *src)
+{
+    return !mt || !src || !mt->t_src_uid || mt->t_src_uid != src->uid;
+}
+
 template <class T> void d2h(std::vector<T> &out, const T *d, size_t n)
 {
     out.resize(n);
@@ -77,8 +83,11 @@ struct TEntry { unsigned gi; int src; };
 
 } // namespace
 
-bicg_matrix *matrix_create_transpose(bicg_matrix *m)
+} // namespace bicg
+
+extern "C" bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m)
 {
+    using namespace bicg;
     Context &c = ctx();
     // collective: every rank learns whether any rank passed a null handle, and every rank's row count (the partition of m)
     struct Mine { int ok, n_loc; } mine{m ? 1 : 0, m ? m->n_loc : 0};
@@ -216,48 +225,30 @@ bicg_matrix *matrix_create_transpose(bicg_matrix *m)
     }
     // the values: the refresh every later bicg_matrix_transpose_values runs
     enqueue_refresh(mt, m, c.stream);
-    int error = 0;
-    BICG_CUDA(cudaMemcpyAsync(&error, &mt->d_sc->error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU while creating a transpose", me);
+    sync_checked(mt, "the creation of a transpose");
     return mt;
 }
 
-int matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src, bool async, cudaStream_t st)
+extern "C" int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src)
 {
-    auto bad = [&] { return !mt || !src || !mt->t_src_uid || mt->t_src_uid != src->uid; };
+    using namespace bicg;
     Context &c = ctx();
-    if (async) {
-        if (bad()) return -1;
-        c.ensure();
-        cudaStreamCaptureStatus cs;
-        BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-        const bool captured = cs != cudaStreamCaptureStatusNone;
-        async_handle_init(mt);
-        async_handle_init(src);
-        const unsigned wflag = captured ? cudaEventWaitExternal : 0;
-        BICG_CUDA(cudaStreamWaitEvent(st, mt->ev_last, wflag));
-        BICG_CUDA(cudaStreamWaitEvent(st, src->ev_last, wflag));
-        enqueue_refresh(mt, src, st);
-        const unsigned rflag = captured ? cudaEventRecordExternal : cudaEventRecordDefault;
-        BICG_CUDA(cudaEventRecordWithFlags(mt->ev_last, st, rflag));
-        BICG_CUDA(cudaEventRecordWithFlags(src->ev_last, st, rflag));
-        return 0;
-    }
-    // collective: a rank with bad arguments must not leave the others waiting in the barriers
-    int mine = bad() ? 1 : 0;
-    std::vector<int> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(int));
-    for (int o : all) if (o) return -1;
+    // collective (the barriers of the refresh): every rank's verdict
+    if (!ranks_agree(transpose_bad(mt, src), {})) return -1;
     c.ensure();
     wait_handle(mt);
     wait_handle(src);
     enqueue_refresh(mt, src, c.stream);
-    int error = 0;
-    BICG_CUDA(cudaMemcpyAsync(&error, &mt->d_sc->error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU during a transpose refresh", mt->rank);
+    sync_checked(mt, "a transpose refresh");
     return 0;
 }
 
-} // namespace bicg
+extern "C" int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream)
+{
+    using namespace bicg;
+    if (transpose_bad(mt, src)) return -1;
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    stream_ordered({mt, src}, st, capturing(st), [&] { enqueue_refresh(mt, src, st); });
+    return 0;
+}

@@ -144,16 +144,15 @@ void enqueue_value_grad(bicg_matrix *m, int nvec, const double *u, const double 
 
 } // namespace
 
-int matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta, double *diag_out,
-                      double *offd_out, bool device_vectors)
+} // namespace bicg
+
+extern "C" int bicg_matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                                      double *diag_out, double *offd_out, int device_vectors)
 {
+    using namespace bicg;
     Context &c = ctx();
-    // collective: a rank with bad arguments must not leave the others waiting for it in the halo exchange and the barrier
-    struct Args { int bad, nvec; } mine{bad_args(m, nvec, u, v, diag_out, offd_out) ? 1 : 0, nvec};
-    std::vector<Args> all((size_t)c.world);
-    c.host_allgather(&mine, all.data(), sizeof(Args));
-    for (const Args &o : all)
-        if (o.bad || o.nvec != nvec) return -1;
+    // collective (the halo exchange and the barrier): every rank's verdict and nvec
+    if (!ranks_agree(bad_args(m, nvec, u, v, diag_out, offd_out), {nvec})) return -1;
     c.ensure();
     wait_handle(m);
     const size_t vbytes = (size_t)nvec * (size_t)m->n_loc * sizeof(double);
@@ -178,31 +177,21 @@ int matrix_value_grad(bicg_matrix *m, int nvec, const double *u, const double *v
         if (nd) BICG_CUDA(cudaMemcpyAsync(diag_out, dd, nd * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
         if (no) BICG_CUDA(cudaMemcpyAsync(offd_out, dof, no * sizeof(double), cudaMemcpyDeviceToHost, c.stream));
     }
-    int error = 0;
-    BICG_CUDA(cudaMemcpyAsync(&error, &m->d_sc->error, sizeof(int), cudaMemcpyDeviceToHost, c.stream));
-    BICG_CUDA(cudaStreamSynchronize(c.stream));
-    if (error) fatal("bicgstab_b200: rank %d timed out waiting for a peer GPU during a value gradient", m->rank);
+    sync_checked(m, "a value gradient");
     c.dev_free(tmp);
     return 0;
 }
 
-int matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
-                            double *diag_out, double *offd_out, cudaStream_t st)
+extern "C" int bicg_matrix_value_grad_async(bicg_matrix *m, int nvec, const double *u, const double *v, double alpha, double beta,
+                                            double *diag_out, double *offd_out, void *stream)
 {
+    using namespace bicg;
     if (bad_args(m, nvec, u, v, diag_out, offd_out)) return -1;
-    Context &c = ctx();
-    c.ensure();
-    cudaStreamCaptureStatus cs;
-    BICG_CUDA(cudaStreamIsCapturing(st, &cs));
-    const bool captured = cs != cudaStreamCaptureStatusNone;
-    async_handle_init(m);
-    BICG_CUDA(cudaStreamWaitEvent(st, m->ev_last, captured ? cudaEventWaitExternal : 0));
-    enqueue_value_grad(m, nvec, u, v, alpha, beta, diag_out, offd_out, st);
-    BICG_CUDA(cudaEventRecordWithFlags(m->ev_last, st, captured ? cudaEventRecordExternal : cudaEventRecordDefault));
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    stream_ordered({m}, st, capturing(st), [&] { enqueue_value_grad(m, nvec, u, v, alpha, beta, diag_out, offd_out, st); });
     return 0;
 }
-
-} // namespace bicg
 
 extern "C" int bicg_debug_value_grad_layout(bicg_matrix *m, int lanes, const unsigned *blk_ptr)
 {
