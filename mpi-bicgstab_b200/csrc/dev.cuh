@@ -126,12 +126,22 @@ __device__ __forceinline__ void mbar_wait(unsigned bar, unsigned parity)
 {
     while (!mbar_try_wait(bar, parity)) { }
 }
-// 1-D TMA bulk copy global -> shared, completion counted in bytes on an mbarrier.  16-byte aligned
-// addresses and a multiple-of-16 size are required.
-__device__ __forceinline__ void tma_load_1d(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar)
+// L2 policy of one access: Plain = no hint; Hint = the access carries a createpolicy value (l2_evict_first_policy), e.g.
+// evict-first for the matrix stream or for a vector whose next use is too far away for L2 to keep it (mega.cu: run_bicgstab)
+struct Plain {};
+struct Hint { unsigned long long pol; };
+
+// 1-D TMA bulk copy global -> shared, completion counted in bytes on an mbarrier, optionally with an L2 policy.
+// 16-byte aligned addresses and a multiple-of-16 size are required.
+__device__ __forceinline__ void tma_load_1d(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar, Plain = {})
 {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                  ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+__device__ __forceinline__ void tma_load_1d(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar, Hint h)
+{
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
+                 ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar), "l"(h.pol) : "memory");
 }
 
 __device__ __forceinline__ void mbar_arrive(unsigned bar)
@@ -281,9 +291,52 @@ __device__ __forceinline__ void merge_row(int i, const unsigned *__restrict__ dp
 // ------------------------------------------------------------------------------------------------
 constexpr int PROW_PAD = 8;       // extra ptr / epilogue slots per stage for the 16-byte alignment window
 
+// Shared memory one CTA may opt into on sm_90, static and dynamic together (227 KB of the SM's 228 KB).
+constexpr int SMEM_OPTIN_BYTES = 227 * 1024;
+// What the TMA tile planner (matrix.cu: build_tma_plan) shares out among the CTAs it places on one SM, 4 KB under the SM's
+// 228 KB; the planner takes a further 1536 B off each CTA's share before it sizes the CTA's stages.
+constexpr long long TMA_PLAN_SMEM_BYTES = 224 * 1024;
+// What the persistent kernel's planner (matrix.cu: build_mega_plan) gives its one CTA per SM, stages or resident slice:
+// beside the 3.4 KB of the kernel's static shared memory it stays under SMEM_OPTIN_BYTES.
+constexpr long long MEGA_PLAN_SMEM_BYTES = 222 * 1024;
+// opt a kernel into the most dynamic shared memory its static shared memory leaves
+template <class Kernel>
+cudaError_t smem_optin(Kernel k)
+{
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, k);
+    if (e != cudaSuccess) return e;
+    return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_OPTIN_BYTES - (int)fa.sharedSizeBytes);
+}
+
+// One stage of a tile of rpt rows and up to cap entries, in byte offsets from the stage's start:
+//   [values: cap x 8 B][nepi epilogue slices: prow x 8 B each][columns: cap x 4 B][row pointers: prow x 4 B],  prow = rpt + PROW_PAD.
+// Packed values fill the value area as three planes (4-, 2- and 1-byte) at 0, vmid() and vhi(); 16-bit column codes fill
+// the first half of the column area.  A stage keeps this size whatever format it holds.
+constexpr int SPMV_ENTRY_BYTES = 12;   // value + column of one staged entry
+__host__ __device__ constexpr size_t spmv_stage_bytes(int cap, int rpt, int nepi)
+{
+    return (size_t)cap * SPMV_ENTRY_BYTES + (size_t)(rpt + PROW_PAD) * (size_t)(4 + 8 * nepi);
+}
+struct StageLayout {
+    int cap, prow, nepi;
+    __host__ __device__ constexpr StageLayout(int cap_, int rpt, int nepi_) : cap(cap_), prow(rpt + PROW_PAD), nepi(nepi_) {}
+    __host__ __device__ constexpr size_t bytes() const { return spmv_stage_bytes(cap, prow - PROW_PAD, nepi); }
+    // the areas of the stage that starts at st
+    __device__ __forceinline__ const double *vals(const unsigned char *st) const { return reinterpret_cast<const double *>(st); }
+    __host__ __device__ constexpr size_t vmid_off() const { return (size_t)cap * 4u; }
+    __host__ __device__ constexpr size_t vhi_off() const { return (size_t)cap * 6u; }
+    __device__ __forceinline__ const unsigned char *vmid(const unsigned char *st) const { return st + vmid_off(); }
+    __device__ __forceinline__ const unsigned char *vhi(const unsigned char *st) const { return st + vhi_off(); }
+    __device__ __forceinline__ const double *epi(const unsigned char *st, int v = 0) const { return vals(st) + cap + v * prow; }
+    __device__ __forceinline__ const unsigned *cols(const unsigned char *st) const { return reinterpret_cast<const unsigned *>(epi(st, nepi)); }
+    __device__ __forceinline__ const unsigned short *codes(const unsigned char *st) const { return reinterpret_cast<const unsigned short *>(cols(st)); }
+    __device__ __forceinline__ const unsigned *ptrs(const unsigned char *st) const { return cols(st) + cap; }
+};
+
 // The part of the arrays that one tile of rows [row0, row1) with entries [p0, p1) puts into a stage: entries
 // [a0, a0 + cnt) and row pointers [rowa, rowa + cntp), widened to whole 16-byte units for the bulk copies.  `al` is the
-// alignment mask of the entry window: 3 for 4-byte columns, 7 for 2-byte column codes.
+// alignment mask of the entry window (TileFormat::align).
 struct TileWindow { unsigned a0, cnt; int rowa, cntp; };
 __device__ __forceinline__ TileWindow tile_window(int row0, int row1, unsigned p0, unsigned p1, unsigned al)
 {
@@ -293,6 +346,108 @@ __device__ __forceinline__ TileWindow tile_window(int row0, int row1, unsigned p
     w.rowa = row0 & ~3;
     w.cntp = ((row1 + 1 + 3) & ~3) - w.rowa;
     return w;
+}
+
+// What the producer put into a stage: rows [row0, row1), entries from a0 and row pointers from rowa (the TileWindow).  The
+// persistent kernel's stages also carry the tile's entries [lo, hi) relative to a0 and its chunk flag (MegaArgs::tile_flag);
+// the tile kernel's stages, which never hold chunk tiles, keep the 16-byte header.
+struct StageHdr { int row0, row1; unsigned a0; int rowa; };
+struct ChunkStageHdr : StageHdr { unsigned lo, hi; int flag; int pad_; };
+
+// The ring of up to 4 stages, in shared memory: a "full" mbarrier per stage that the producer's bulk copies complete, an
+// "empty" one on which every consumer warp arrives once it is done with the stage, and the stage headers (Hdr: StageHdr
+// or ChunkStageHdr).  Visit v of the
+// ring uses stage v % stages; its parity is that of v / stages.  Visits are counted in int or unsigned (I), as the caller
+// counts them.
+template <class Hdr>
+struct StageRing {
+    unsigned long long full[4], empty[4];
+    Hdr hdr[4];
+
+    // thread 0, before a CTA barrier
+    __device__ __forceinline__ void init(int stages, unsigned consumer_warps)
+    {
+        for (int s = 0; s < stages; ++s) {
+            mbar_init(smem_u32(&full[s]), 1u);
+            mbar_init(smem_u32(&empty[s]), consumer_warps);
+        }
+        mbar_fence_init();
+    }
+    __device__ __forceinline__ unsigned full_bar(int s) { return smem_u32(&full[s]); }
+    // producer: the stage of visit v, once the consumers have released it (from the second lap on); -1 as soon as stop()
+    // is true, while waiting or after
+    template <class I, class Stop>
+    __device__ __forceinline__ int acquire(I v, I stages, Stop stop)
+    {
+        const int s = (int)(v % stages);
+        if (v >= stages) {
+            const unsigned par = (unsigned)(v / stages - 1) & 1u;
+            while (!mbar_try_wait(smem_u32(&empty[s]), par))
+                if (stop()) return -1;
+        }
+        return stop() ? -1 : s;
+    }
+    template <class I>
+    __device__ __forceinline__ int acquire(I v, I stages) { return acquire(v, stages, [] { return false; }); }
+    // consumer: the stage of visit v, once its bulk copies have landed
+    template <class I>
+    __device__ __forceinline__ int wait(I v, I stages)
+    {
+        const int s = (int)(v % stages);
+        mbar_wait(smem_u32(&full[s]), (unsigned)(v / stages) & 1u);
+        return s;
+    }
+    // consumer: every thread of the warp is done with stage s
+    __device__ __forceinline__ void release(int s)
+    {
+        __syncwarp();
+        if ((threadIdx.x & 31) == 0) mbar_arrive(smem_u32(&empty[s]));
+    }
+};
+
+// How a tile is streamed into its stage: 8-byte values or the three planes of packed values, 32-bit columns or 16-bit
+// codes, nepi epilogue slices, and the L2 policy of the value and column copies (Plain or Hint).
+template <class H = Plain>
+struct TileFormat {
+    bool packed, coded;
+    int nepi;
+    H pol;
+    // a bulk copy moves whole 16-byte units: the entry window is aligned to 4 entries for 4-byte columns, 8 for 2-byte
+    // codes and 16 for the 1-byte plane of packed values
+    __device__ __forceinline__ unsigned align() const { return packed ? 15u : (coded ? 7u : 3u); }
+    __device__ __forceinline__ unsigned col_bytes() const { return coded ? 2u : 4u; }
+    __device__ __forceinline__ unsigned val_bytes() const { return packed ? 7u : 8u; }
+};
+// The arrays a tile is copied from: val is the 8-byte values or the low plane of packed values, col the 32-bit columns
+// or the 16-bit codes.
+struct TileSrc {
+    const void *val;
+    const unsigned short *vmid;
+    const unsigned char *vhi;
+    const void *col;
+    const unsigned *ptr;
+};
+struct NoEpi { __device__ const double *operator()(int) const { return nullptr; } };
+// Producer: the bulk copies of window w into stage st (layout L) and the byte count they complete on its full barrier.
+// epi(v): epilogue vector v, v < f.nepi, whose rows [w.rowa, w.rowa + w.cntp) go to slice v.
+template <class H, class Epi = NoEpi>
+__device__ __forceinline__ void tile_issue(const unsigned char *st, const StageLayout &L, unsigned bar, const TileFormat<H> &f,
+                                           const TileWindow &w, const TileSrc &src, Epi epi = {})
+{
+    mbar_arrive_expect_tx(bar, w.cnt * (f.val_bytes() + f.col_bytes()) + (unsigned)w.cntp * 4u + (unsigned)(f.nepi * w.cntp) * 8u);
+    if (w.cnt) {
+        if (f.packed) {
+            tma_load_1d(smem_u32(st), (const unsigned *)src.val + w.a0, w.cnt * 4u, bar, f.pol);
+            tma_load_1d(smem_u32(L.vmid(st)), src.vmid + w.a0, w.cnt * 2u, bar, f.pol);
+            tma_load_1d(smem_u32(L.vhi(st)), src.vhi + w.a0, w.cnt, bar, f.pol);
+        } else {
+            tma_load_1d(smem_u32(L.vals(st)), (const double *)src.val + w.a0, w.cnt * 8u, bar, f.pol);
+        }
+        tma_load_1d(smem_u32(L.cols(st)), (const char *)src.col + (size_t)w.a0 * f.col_bytes(), w.cnt * f.col_bytes(), bar, f.pol);
+    }
+    tma_load_1d(smem_u32(L.ptrs(st)), src.ptr + w.rowa, (unsigned)w.cntp * 4u, bar);
+    for (int v = 0; v < f.nepi; ++v)
+        tma_load_1d(smem_u32(L.epi(st, v)), epi(v) + w.rowa, (unsigned)w.cntp * 8u, bar);
 }
 
 // One row's product with NV vectors x[v] over the staged entries [j, e) (j already includes the thread's offset in its

@@ -287,7 +287,6 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
 {
     Context &c = ctx();
     const int rpt = threads / lanes;
-    const long long SMEM_MAX = 224 * 1024;
     const long long fixed = (long long)spmv_stage_bytes(0, rpt, SPMV_EPI_SLICES);   // a stage's bytes beside the entries
     // stage capacity: a full tile of average rows with 25 % head-room, never less than the longest row
     long long cap = (long long)std::ceil(rpt * m->mean_row * 1.25) + 64;
@@ -295,7 +294,7 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
     cap = round_up(cap, 32);
     int ctas = want_ctas > 0 ? want_ctas : 2;
     // shrink towards the shared-memory budget of `ctas` CTAs per SM
-    const long long budget = SMEM_MAX / ctas - 1536;
+    const long long budget = TMA_PLAN_SMEM_BYTES / ctas - 1536;
     if ((long long)stages * (cap * SPMV_ENTRY_BYTES + fixed) > budget) {
         long long fit = (budget / stages - fixed) / SPMV_ENTRY_BYTES;
         fit = (fit / 32) * 32;
@@ -310,7 +309,7 @@ static bool build_tma_plan(const bicg_matrix *m, const unsigned *h_ptr, int lane
 
     out.kind = 0; out.lanes = lanes; out.threads = threads; out.stages = stages; out.cap = (int)cap;
     out.smem = (size_t)stages * spmv_stage_bytes((int)cap, rpt, SPMV_EPI_SLICES);
-    int by_smem = (int)std::max<long long>(1, SMEM_MAX / (long long)(out.smem + 1536));
+    int by_smem = (int)std::max<long long>(1, TMA_PLAN_SMEM_BYTES / (long long)(out.smem + 1536));
     out.ctas_per_sm = std::max(1, std::min({by_smem, 2048 / (threads + 32), want_ctas > 0 ? want_ctas : 8}));
     out.ntiles = nt;
     out.grid = std::max(1, std::min(nt, c.sm_count * out.ctas_per_sm));
@@ -511,7 +510,6 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
     mp.ok = false;
     if (m->n_loc < 1) return;                       // the plan is always built; BICG_MEGA gates its use per solve
     const int G = std::min(c.sm_count, MEGA_MAX_CTAS);
-    const long long SMEM_MAX = 222 * 1024;
     const int lanes = c.cfg.mega_lanes > 0 ? c.cfg.mega_lanes : mega_lanes_for(m->mean_row);
     // BICG_MEGA=1 (default): the persistent kernel where it wins -- thread-per-row plans (banded matrices, short rows).  On
     // long-row matrices (cfg 5: 32 random entries per row) the loop is bound by L2 sector throughput of the gathers, not by
@@ -528,12 +526,13 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
         // are cut by the planner: greedy tiles + chunked long rows (plan.cpp).  The producer loads a tile's entries from a
         // window aligned to 16 entries at both ends (16-byte bulk copies of the 1-byte plane of packed values): up to 30
         // more than the tile.
-        const int cap_limit = (int)(((SMEM_MAX / 2 - (long long)(rpt + 8) * 4) / 12) / 32 * 32) - 64;   // cap = roundup(max + 30, 32) must still fit twice
+        const long long fixed = (long long)spmv_stage_bytes(0, rpt, 0);              // a stage's bytes beside the entries
+        const int cap_limit = (int)(((MEGA_PLAN_SMEM_BYTES / 2 - fixed) / SPMV_ENTRY_BYTES) / 32 * 32) - 64;   // cap = roundup(max + 30, 32) must still fit twice
         const unsigned max_tile_nnz = plan_cta_tiles(h_ptr, m->n_loc, G, rpt, row_extra.empty() ? nullptr : row_extra.data(),
                                                      c.cfg.boundary_weight, tile_row, cta_tile, cap_limit, &tile_nz, &tile_flag, c.cfg.row_weight);
         const int cap = round_up((long long)max_tile_nnz + 30, 32);
-        const long long stage = (long long)cap * 12 + (long long)(rpt + 8) * 4;
-        int stages = (int)std::min<long long>(4, SMEM_MAX / stage);
+        const long long stage = (long long)spmv_stage_bytes(cap, rpt, 0);
+        int stages = (int)std::min<long long>(4, MEGA_PLAN_SMEM_BYTES / stage);
         if (stages < 2) continue;                       // cannot happen with the cap-limited plan; kept as a guard
         bool chunked = false;
         for (int f : tile_flag) chunked = chunked || f != 0;
@@ -549,7 +548,7 @@ static void build_mega_plan(bicg_matrix *m, const unsigned *h_ptr, const std::ve
                 const int r0 = tile_row[(size_t)cta_tile[(size_t)g]], r1 = tile_row[(size_t)cta_tile[(size_t)g + 1]];
                 need = std::max(need, mega_resident_bytes(h_ptr[r1] - h_ptr[r0], r1 - r0));
             }
-            if (need <= (size_t)SMEM_MAX) mp.res_smem = std::max<size_t>(need, 16);
+            if (need <= (size_t)MEGA_PLAN_SMEM_BYTES) mp.res_smem = std::max<size_t>(need, 16);
         }
         mp.ntiles = (int)tile_row.size() - 1;
         mp.cta_row.assign((size_t)G + 1, m->n_loc);

@@ -41,14 +41,7 @@ namespace {
 
 constexpr int RED_THREADS = MEGA_MAX_CTAS;          // one polled slot per thread
 constexpr int RED_WARPS = RED_THREADS / 32;
-struct StageHdr { int row0, row1; unsigned a0; int rowa; unsigned lo, hi; int flag; int pad_; };   // lo, hi: the tile's entries relative to a0
 
-__device__ __forceinline__ void tma_load_1d_hint(unsigned dst_smem, const void *src, unsigned bytes, unsigned bar,
-                                                 unsigned long long pol)
-{
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
-                 ::"r"(dst_smem), "l"(src), "r"(bytes), "r"(bar), "l"(pol) : "memory");
-}
 // Polling etiquette: the first probes go out back to back (the last arriver normally finds everything in place), after
 // that the thread sleeps 64 .. 256 ns between probes -- 132 CTAs spinning flat out on the same 132 cache lines delay the
 // very stores they are waiting for.
@@ -88,9 +81,8 @@ struct MegaShared {
     double red[RED_WARPS][MAIL_VALS];
     double contrib[MAX_RANKS][MAIL_VALS];
     double scratch[32 * MAX_DOTS];
-    unsigned long long full_bar[4], empty_bar[4];
-    StageHdr hdr[4];
-    unsigned vadj[VAL_TABLE_MAX];             // the CTA's value table as PackedVal adds it (packed CTAs only)
+    StageRing<ChunkStageHdr> ring;
+    unsigned vadj[VAL_TABLE_MAX];            // the CTA's value table as PackedVal adds it (packed CTAs only)
     volatile int flags[4];                    // [1] producer stop, [2] consumed visits, [3] a wait timed out
 };
 
@@ -172,16 +164,16 @@ struct PackedVal {
         return __hiloint2double((int)(hm + lds_u32(adj + (hm >> 20) * 4u)), (int)lo);
     }
 };
-// entry idx of the planes of a stage that starts at shared address st and holds cap entries (spmv_impl<..., PACKED>)
-__device__ __forceinline__ PackedVal val_load(unsigned adj, unsigned st, unsigned cap, unsigned idx)
+// entry idx of the planes of a stage that starts at shared address st (layout L)
+__device__ __forceinline__ PackedVal val_load(unsigned adj, unsigned st, const StageLayout &L, unsigned idx)
 {
-    const unsigned lo = lds_u32(st + idx * 4u), mid = lds_u16(st + cap * 4u + idx * 2u), hi = lds_u8(st + cap * 6u + idx);
+    const unsigned lo = lds_u32(st + idx * 4u), mid = lds_u16(st + (unsigned)L.vmid_off() + idx * 2u), hi = lds_u8(st + (unsigned)L.vhi_off() + idx);
     return PackedVal{(hi << 16) | mid, lo, adj};
 }
 
 template <int CT, int LANES>
 struct Mega {
-    static constexpr int RPT = CT / LANES, PROW = RPT + PROW_PAD, NCW = CT / 32, UNR = (LANES == 1) ? 16 : 8;
+    static constexpr int RPT = CT / LANES, NCW = CT / 32, UNR = (LANES == 1) ? 16 : 8;
     static_assert(CT >= RED_THREADS, "the slot reduction uses one thread per CTA slot");
 
     const MegaArgs &a;
@@ -529,32 +521,31 @@ struct Mega {
         }
     }
 
-    // CODED: the stage's column area holds the CTA's 16-bit column codes (its first half; the stage layout is the same for
-    // both formats), each turned back into the column with one select and one add before its gather.
-    // PACKED (CODED CTAs only): the stage's value area holds the three planes of the packed values -- vlo at 0, vmid at
-    // 4 cap bytes, vhi at 6 cap bytes -- each value put back together by PackedVal.
+    // CODED: the stage holds the CTA's 16-bit column codes, each turned back into the column with one select and one add
+    // before its gather.  PACKED (CODED CTAs only): the stage holds the three planes of the packed values, each value put
+    // back together by PackedVal.
     template <int EPI, bool CODED, bool PACKED, class F>
     __device__ void spmv_impl(const double *x, double *y, double (&dot)[4], F far)
     {
-        const int stages = a.stages, cap = a.cap;
+        const int stages = a.stages;
+        const StageLayout L(a.cap, RPT, 0);
         const int sub = tid % LANES, row_in_tile = tid / LANES;
         const ColWindow w = rp.w;
         double carry = 0.0;
         for (int lt = 0; lt < my_tiles; ++lt, ++vis) {
-            const int s = (int)(vis % (unsigned)stages);
-            mbar_wait(smem_u32(&sh.full_bar[s]), (vis / (unsigned)stages) & 1u);
+            const int s = sh.ring.wait(vis, (unsigned)stages);
             const unsigned char *st = dyn + (size_t)s * stage_bytes;
-            const double   *sval = reinterpret_cast<const double *>(st);
-            const unsigned *scol = reinterpret_cast<const unsigned *>(sval + cap);
-            const unsigned short *scode = reinterpret_cast<const unsigned short *>(scol);
-            const unsigned *sptr = scol + cap;
+            const double   *sval = L.vals(st);
+            const unsigned *scol = L.cols(st);
+            const unsigned short *scode = L.codes(st);
+            const unsigned *sptr = L.ptrs(st);
             const unsigned sts = PACKED ? smem_u32(st) : 0u, adj = PACKED ? smem_u32(sh.vadj) : 0u;
             auto column = [&](unsigned idx) { return CODED ? col_decode(w, scode[idx]) : scol[idx]; };
             auto value = [&](unsigned idx) {
-                if constexpr (PACKED) return val_load(adj, sts, (unsigned)cap, idx);
+                if constexpr (PACKED) return val_load(adj, sts, L, idx);
                 else return sval[idx];
             };
-            const StageHdr h = sh.hdr[s];
+            const ChunkStageHdr h = sh.ring.hdr[s];
             if (h.flag != 0) {
                 // one chunk of a row longer than a stage: the whole CTA multiplies it, the row's partial sum is carried
                 // from chunk to chunk in `carry` (same value in every thread) and the row is finished by its last chunk
@@ -582,8 +573,7 @@ struct Mega {
                     }
                     carry = 0.0;
                 }
-                __syncwarp();
-                if (lane == 0) mbar_arrive(smem_u32(&sh.empty_bar[s]));
+                sh.ring.release(s);
                 continue;
             }
             const int row = h.row0 + row_in_tile;
@@ -598,8 +588,7 @@ struct Mega {
             double acc[1];
             row_product<LANES, UNR, 1>(value, column, {x}, j, e, acc);
             if (valid && sub == 0) row_done<EPI>(row, acc[0], e0, e1, e2, e3, y, dot);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&sh.empty_bar[s]));
+            sh.ring.release(s);
         }
     }
 
@@ -914,78 +903,45 @@ __global__ void __launch_bounds__(CT + 32, 1) bicg_mega_kernel(const __grid_cons
     __shared__ __align__(16) MegaShared sh;
 
     const int tid = threadIdx.x;
-    const int stages = a.stages, cap = a.cap;
+    const int stages = a.stages;
     if (tid == 0) {
-        for (int s = 0; s < stages; ++s) {
-            mbar_init(smem_u32(&sh.full_bar[s]), 1u);
-            mbar_init(smem_u32(&sh.empty_bar[s]), (unsigned)M::NCW);
-        }
         sh.flags[0] = sh.flags[1] = sh.flags[2] = sh.flags[3] = 0;
-        mbar_fence_init();
+        sh.ring.init(stages, (unsigned)M::NCW);
     }
     __syncthreads();
 
     const int t0 = a.cta_tile[blockIdx.x], t1 = a.cta_tile[blockIdx.x + 1];
     const int my_tiles = t1 - t0;
-    const size_t stage_bytes = (size_t)cap * 12 + (size_t)M::PROW * 4;
+    const StageLayout L(a.cap, M::RPT, 0);
 
     if (tid >= CT) {
         // ============================ producer warp: streams this CTA's tiles round and round ==============
         const ResidentPlan rp = tid == CT ? resident_plan(a, t0, t1, LANES) : ResidentPlan{};
         if (tid == CT && my_tiles > 0 && !rp.on) {
             volatile int *flags = sh.flags;
-            const unsigned long long pol = l2_evict_first_policy();
-            // 16-bit codes: 2 bytes per entry; a bulk copy moves whole 16-byte units, so the entry window of a tile is
-            // aligned to 8 entries (4 suffice for 4-byte columns), and to 16 for the 1-byte plane of packed values; the
-            // plan's stage capacity covers the widest window
             const bool coded = streams_codes(a, rp, my_tiles);
             const bool packed = streams_values(a, coded);
-            const unsigned al = packed ? 15u : (coded ? 7u : 3u), cbytes = coded ? 2u : 4u, vbytes = packed ? 7u : 8u;
-            const void *cols = coded ? (const void *)a.col16 : (const void *)a.col;
+            const TileFormat<Hint> f{packed, coded, 0, Hint{l2_evict_first_policy()}};
+            const TileSrc src{packed ? (const void *)a.vlo : (const void *)a.val, a.vmid, a.vhi,
+                              coded ? (const void *)a.col16 : (const void *)a.col, a.ptr};
             unsigned v = 0;
-            bool stop = false;
             for (;; ++v) {
-                const int s = (int)(v % (unsigned)stages);
-                if (v >= (unsigned)stages) {
-                    const unsigned par = (v / (unsigned)stages - 1u) & 1u;
-                    while (!mbar_try_wait(smem_u32(&sh.empty_bar[s]), par)) {
-                        if (flags[1]) { stop = true; break; }
-                    }
-                }
-                if (stop || flags[1]) break;
+                const int s = sh.ring.acquire(v, (unsigned)stages, [&] { return flags[1] != 0; });
+                if (s < 0) break;
                 const int t = t0 + (int)(v % (unsigned)my_tiles);
                 const int row0 = a.tile_row[t], row1 = a.tile_row[t + 1];
                 const unsigned p0 = a.tile_nz[t], p1 = a.tile_nz[t + 1];
-                const auto [a0, cnt, rowa, cntp] = tile_window(row0, row1, p0, p1, al);
-                unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
-                double   *sval = reinterpret_cast<double *>(st);
-                unsigned *scol = reinterpret_cast<unsigned *>(sval + cap);
-                unsigned *sptr = scol + cap;
-                sh.hdr[s] = StageHdr{row0, row1, a0, rowa, p0 - a0, p1 - a0, a.tile_flag ? a.tile_flag[t] : 0, 0};
-                const unsigned bar = smem_u32(&sh.full_bar[s]);
-                mbar_arrive_expect_tx(bar, cnt * (vbytes + cbytes) + (unsigned)cntp * 4u);
-                if (cnt) {
-                    const void *csrc = (const char *)cols + (size_t)a0 * cbytes;
-                    if (packed) {                               // the stage layout of spmv_impl<..., PACKED>
-                        tma_load_1d_hint(smem_u32(st), a.vlo + a0, cnt * 4u, bar, pol);
-                        tma_load_1d_hint(smem_u32(st + (size_t)cap * 4u), a.vmid + a0, cnt * 2u, bar, pol);
-                        tma_load_1d_hint(smem_u32(st + (size_t)cap * 6u), a.vhi + a0, cnt, bar, pol);
-                    } else {
-                        tma_load_1d_hint(smem_u32(sval), a.val + a0, cnt * 8u, bar, pol);
-                    }
-                    tma_load_1d_hint(smem_u32(scol), csrc, cnt * cbytes, bar, pol);
-                }
-                tma_load_1d(smem_u32(sptr), a.ptr + rowa, (unsigned)cntp * 4u, bar);
+                const TileWindow w = tile_window(row0, row1, p0, p1, f.align());
+                sh.ring.hdr[s] = ChunkStageHdr{{row0, row1, w.a0, w.rowa}, p0 - w.a0, p1 - w.a0, a.tile_flag ? a.tile_flag[t] : 0, 0};
+                tile_issue(dyn_smem + (size_t)s * L.bytes(), L, sh.ring.full_bar(s), f, w, src);
             }
             // drain: bulk copies already issued must land before the CTA may retire its shared memory
-            const unsigned consumed = (unsigned)flags[2];
-            for (unsigned w = consumed; w < v; ++w)
-                mbar_wait(smem_u32(&sh.full_bar[w % (unsigned)stages]), (w / (unsigned)stages) & 1u);
+            for (unsigned w = (unsigned)flags[2]; w < v; ++w) sh.ring.wait(w, (unsigned)stages);
         }
     } else {
         // ============================ consumer warps: the solver ============================================
         M m(a, sh);
-        m.dyn = dyn_smem; m.tid = tid; m.lane = tid & 31; m.my_tiles = my_tiles; m.vis = 0u; m.stage_bytes = stage_bytes;
+        m.dyn = dyn_smem; m.tid = tid; m.lane = tid & 31; m.my_tiles = my_tiles; m.vis = 0u; m.stage_bytes = L.bytes();
         m.row_lo = a.tile_row[t0]; m.row_hi = a.tile_row[t1];
         m.trace_it = 0;
         m.trace_who = blockIdx.x == 0 ? 0 : (blockIdx.x == gridDim.x / 2 ? 1 : -1);
@@ -1160,21 +1116,11 @@ cudaError_t launch(const MegaArgs &a, int grid, size_t smem, cudaStream_t st)
     void *params[1] = {(void *)&a};
     return cudaLaunchCooperativeKernel((const void *)bicg_mega_kernel<CT, LANES>, dim3(grid), dim3(CT + 32), params, smem, st);
 }
-template <int CT, int LANES>
-cudaError_t set_attr()
-{
-    cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, bicg_mega_kernel<CT, LANES>);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(bicg_mega_kernel<CT, LANES>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                227 * 1024 - (int)fa.sharedSizeBytes);
-}
-
 } // namespace
 
 size_t mega_smem_bytes(int cap, int stages, int threads, int lanes)
 {
-    return (size_t)stages * ((size_t)cap * 12u + (size_t)(threads / lanes + PROW_PAD) * 4u);
+    return (size_t)stages * spmv_stage_bytes(cap, threads / lanes, 0);
 }
 
 bool mega_has_variant(int threads, int lanes)
@@ -1186,11 +1132,11 @@ bool mega_has_variant(int threads, int lanes)
 int mega_setup_attributes()
 {
     cudaError_t e;
-    if ((e = set_attr<256, 1>()) != cudaSuccess) return (int)e;
-    if ((e = set_attr<512, 1>()) != cudaSuccess) return (int)e;
-    if ((e = set_attr<512, 4>()) != cudaSuccess) return (int)e;
-    if ((e = set_attr<512, 8>()) != cudaSuccess) return (int)e;
-    if ((e = set_attr<512, 32>()) != cudaSuccess) return (int)e;
+    if ((e = smem_optin(bicg_mega_kernel<256, 1>)) != cudaSuccess) return (int)e;
+    if ((e = smem_optin(bicg_mega_kernel<512, 1>)) != cudaSuccess) return (int)e;
+    if ((e = smem_optin(bicg_mega_kernel<512, 4>)) != cudaSuccess) return (int)e;
+    if ((e = smem_optin(bicg_mega_kernel<512, 8>)) != cudaSuccess) return (int)e;
+    if ((e = smem_optin(bicg_mega_kernel<512, 32>)) != cudaSuccess) return (int)e;
     return 0;
 }
 

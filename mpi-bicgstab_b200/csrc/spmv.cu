@@ -86,8 +86,6 @@ __device__ __forceinline__ void spmv_tail(const KernelCommon &kc, double (&dot)[
     }
 }
 
-struct StageHdr { int row0, row1; unsigned a0; int rowa; };
-
 template <int LANES, int CTHREADS, int NV, bool SOLVER>
 __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_constant__ SpmvArgs a)
 {
@@ -95,29 +93,19 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
         if (a.kc.sc->done) return;
 
     constexpr int RPT = CTHREADS / LANES;            // rows per tile
-    constexpr int PROW = RPT + PROW_PAD;
     constexpr int NCW = CTHREADS / 32;               // consumer warps
     constexpr int UNR = row_unr<LANES, NV>();
-    constexpr int NEPI = SOLVER ? SPMV_EPI_SLICES : 0;
 
     extern __shared__ __align__(128) unsigned char dyn_smem[];
-    __shared__ __align__(8) unsigned long long full_bar[4], empty_bar[4];
-    __shared__ StageHdr hdr[4];
+    __shared__ __align__(8) StageRing<StageHdr> ring;
     __shared__ double scratch[SOLVER ? 32 * 4 : 32];
 
     const int tid = threadIdx.x;
-    const int stages = a.stages, cap = a.cap;
-    const size_t stage_bytes = spmv_stage_bytes(cap, RPT, NEPI);
+    const int stages = a.stages;
+    const StageLayout L(a.cap, RPT, SOLVER ? SPMV_EPI_SLICES : 0);
     const int my_tiles = (a.ntiles > (int)blockIdx.x) ? (a.ntiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x : 0;
-    const int nvec = SOLVER ? a.epi.nvec : 0;        // epilogue vectors streamed per tile
 
-    if (tid == 0) {
-        for (int s = 0; s < stages; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1u);
-            mbar_init(smem_u32(&empty_bar[s]), (unsigned)NCW);
-        }
-        mbar_fence_init();
-    }
+    if (tid == 0) ring.init(stages, (unsigned)NCW);
     __syncthreads();
 
     double dot[4] = {0.0, 0.0, 0.0, 0.0};
@@ -125,26 +113,16 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
     if (tid >= CTHREADS) {
         // ===================================== producer warp ==========================================
         if (tid == CTHREADS) {
+            // 8-byte values, 32-bit columns, no L2 policy; the solver streams its epilogue vectors
+            const TileFormat<> f{false, false, SOLVER ? a.epi.nvec : 0, {}};
             for (int i = 0; i < my_tiles; ++i) {
-                const int t = (int)blockIdx.x + i * (int)gridDim.x, s = i % stages;
+                const int t = (int)blockIdx.x + i * (int)gridDim.x;
                 const int row0 = a.tile_row[t], row1 = a.tile_row[t + 1];
-                const auto [a0, cnt, rowa, cntp] = tile_window(row0, row1, a.tile_nz[t], a.tile_nz[t + 1], 3u);
-                if (i >= stages) mbar_wait(smem_u32(&empty_bar[s]), (unsigned)(i / stages - 1) & 1u);
-                unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
-                double   *sval = reinterpret_cast<double *>(st);
-                double   *sepi = sval + cap;
-                unsigned *scol = reinterpret_cast<unsigned *>(sepi + NEPI * PROW);
-                unsigned *sptr = scol + cap;
-                hdr[s] = StageHdr{row0, row1, a0, rowa};
-                const unsigned bar = smem_u32(&full_bar[s]);
-                mbar_arrive_expect_tx(bar, cnt * 12u + (unsigned)cntp * 4u + (unsigned)(nvec * cntp) * 8u);
-                if (cnt) {
-                    tma_load_1d(smem_u32(sval), a.val + a0, cnt * 8u, bar);
-                    tma_load_1d(smem_u32(scol), a.col + a0, cnt * 4u, bar);
-                }
-                tma_load_1d(smem_u32(sptr), a.ptr + rowa, (unsigned)cntp * 4u, bar);
-                for (int v = 0; v < nvec; ++v)
-                    tma_load_1d(smem_u32(sepi + v * PROW), a.epi.vec[v] + rowa, (unsigned)cntp * 8u, bar);
+                const TileWindow w = tile_window(row0, row1, a.tile_nz[t], a.tile_nz[t + 1], f.align());
+                const int s = ring.acquire(i, stages);
+                ring.hdr[s] = StageHdr{row0, row1, w.a0, w.rowa};
+                tile_issue(dyn_smem + (size_t)s * L.bytes(), L, ring.full_bar(s), f, w, TileSrc{a.val, nullptr, nullptr, a.col, a.ptr},
+                           [&](int v) { return a.epi.vec[v]; });
             }
         }
     } else {
@@ -166,15 +144,13 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
         const int ndot = SOLVER ? a.epi.ndot : 0;
 
         for (int i = 0; i < my_tiles; ++i) {
-            const int s = i % stages;
-            mbar_wait(smem_u32(&full_bar[s]), (unsigned)(i / stages) & 1u);
-
-            const unsigned char *st = dyn_smem + (size_t)s * stage_bytes;
-            const double   *sval = reinterpret_cast<const double *>(st);
-            const double   *sepi = sval + cap;
-            const unsigned *scol = reinterpret_cast<const unsigned *>(sepi + NEPI * PROW);
-            const unsigned *sptr = scol + cap;
-            const StageHdr h = hdr[s];
+            const int s = ring.wait(i, stages);
+            const unsigned char *st = dyn_smem + (size_t)s * L.bytes();
+            const double   *sval = L.vals(st);
+            const double   *sepi = L.epi(st);
+            const unsigned *scol = L.cols(st);
+            const unsigned *sptr = L.ptrs(st);
+            const StageHdr h = ring.hdr[s];
             const int row = h.row0 + row_in_tile;
             const bool valid = row < h.row1;
             int j = 0, e = 0;
@@ -186,14 +162,13 @@ __global__ void __launch_bounds__(CTHREADS + 32, 1) spmv_ws_kernel(const __grid_
             row_product<LANES, UNR, NV>([&](int idx) { return sval[idx]; }, [&](int idx) { return scol[idx]; }, x, j, e, acc);
             if (valid && lane == 0) {
                 if constexpr (SOLVER) {
-                    const int ro = row - h.rowa;           // by value: nvcc then forms the slice offsets as it did inline
-                    solver_store(a, row, acc[0], [=](int v) { return sepi[v * PROW + ro]; }, ndot, dot);
+                    const int ro = row - h.rowa, prow = L.prow;   // by value: nvcc then forms the slice offsets as it did inline
+                    solver_store(a, row, acc[0], [=](int v) { return sepi[v * prow + ro]; }, ndot, dot);
                 } else {
                     multiply_store<NV>(a, row, acc);
                 }
             }
-            __syncwarp();
-            if ((tid & 31) == 0) mbar_arrive(smem_u32(&empty_bar[s]));   // this warp is done with stage s
+            ring.release(s);
         }
     }
 
@@ -287,22 +262,13 @@ cudaError_t launch_nv(int kind, int lanes, int threads, int grid, size_t smem, c
     }
 }
 
-// opt-in limit is 227 KB per CTA *including* the kernel's static shared memory
-template <class Kernel>
-cudaError_t set_attr(Kernel k)
-{
-    cudaFuncAttributes fa;
-    cudaError_t e = cudaFuncGetAttributes(&fa, k);
-    if (e != cudaSuccess) return e;
-    return cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - (int)fa.sharedSizeBytes);
-}
 template <int NV, bool SOLVER, int LANES>
 cudaError_t set_attr_l()
 {
     cudaError_t e;
-    if ((e = set_attr(spmv_ws_kernel<LANES, 128, NV, SOLVER>)) != cudaSuccess) return e;
-    if ((e = set_attr(spmv_ws_kernel<LANES, 256, NV, SOLVER>)) != cudaSuccess) return e;
-    return set_attr(spmv_ws_kernel<LANES, 512, NV, SOLVER>);
+    if ((e = smem_optin(spmv_ws_kernel<LANES, 128, NV, SOLVER>)) != cudaSuccess) return e;
+    if ((e = smem_optin(spmv_ws_kernel<LANES, 256, NV, SOLVER>)) != cudaSuccess) return e;
+    return smem_optin(spmv_ws_kernel<LANES, 512, NV, SOLVER>);
 }
 template <int NV, bool SOLVER>
 cudaError_t set_attr_nv()

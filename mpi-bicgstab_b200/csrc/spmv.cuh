@@ -42,14 +42,8 @@ struct SpmvArgs {
     int wait_halo;                   // 1: x's ghost part is filled by peers; wait for their halo flags first
 };
 
-// Bytes of one TMA stage of a tile of rpt rows: [val cap*8][nepi epilogue slices of PROW*8][col cap*4][ptr PROW*4],
-// PROW = rpt + PROW_PAD.  The solver's stages hold SPMV_EPI_SLICES epilogue slices, the multiply's none.
+// epilogue slices of the solver's stages (dev.cuh: StageLayout); the multiply's stages have none
 constexpr int SPMV_EPI_SLICES = 4;
-constexpr int SPMV_ENTRY_BYTES = 12;   // val + col of one staged entry
-__host__ __device__ constexpr size_t spmv_stage_bytes(int cap, int rpt, int nepi)
-{
-    return (size_t)cap * SPMV_ENTRY_BYTES + (size_t)(rpt + PROW_PAD) * (size_t)(4 + 8 * nepi);
-}
 
 // kind 0: warp-specialised TMA tile kernel, kind 1: row-split kernel.  threads (consumer threads) only matters for kind 0.
 // solver: the solver's epilogue (a.nv == 1), else the multiply's for a.nv vectors.  Returns cudaError_t as int.

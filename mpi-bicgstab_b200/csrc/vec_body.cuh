@@ -7,12 +7,7 @@ namespace bicg {
 
 template <int W> struct Pk { double v[W]; };
 
-// L2 policy of one access: Plain = no hint (plain ld / st, what every phase kernel of vec.cu uses); Hint = the access
-// carries a createpolicy value (dev.cuh: ld_hint, st_hint), e.g. evict-first for a vector whose next use is too far
-// away for L2 to keep it (mega.cu: run_bicgstab)
-struct Plain {};
-struct Hint { unsigned long long pol; };
-
+// the accesses of one L2 policy (dev.cuh: Plain, Hint); every phase kernel of vec.cu uses Plain
 __device__ __forceinline__ double ld1(const double *p, Plain) { return *p; }
 __device__ __forceinline__ double ld1(const double *p, Hint h) { return ld_hint(p, h.pol); }
 __device__ __forceinline__ double2 ld2(const double *p, Plain) { return *reinterpret_cast<const double2 *>(p); }
