@@ -239,6 +239,28 @@ int bicg_matrix_transpose_values(bicg_matrix *mt, bicg_matrix *src);
 int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *src, void *stream);
 int bicg_matrix_block_nz(const bicg_matrix *m, unsigned *diag_nz, unsigned *offd_nz);
 
+/* Entry vectors between a handle and its transpose: the permutation bicg_matrix_transpose_values applies to the values, on any
+ * vector of one double per stored entry, in both directions (what differentiating through that refresh needs).
+ *
+ * bicg_matrix_transpose_entries_async, reverse = 0: in (in_diag, in_offd) is in src's block order (the order
+ * bicg_matrix_set_values takes on src); out (out_diag, out_offd) receives, in mt's block order, exactly the values
+ * bicg_matrix_transpose_values would give mt if src held `in`, so bicg_matrix_set_values(mt, out) then leaves mt with the bits
+ * of that refresh.  reverse = 1: the inverse permutation, from mt's block order back to src's.  Both directions are pure
+ * copies, so reverse after forward gives back every bit of `in`, duplicates and explicit zeros included.  in_offd / out_offd
+ * may be null where their handle has no offd entries (always with one rank).
+ *
+ * Device pointers, read and written in stream order on the caller's CUDA stream `stream` behind both handles' earlier work, and
+ * both handles' next work waits for it: no host synchronisation, allocation, pageable copy or output, no prepare step (there
+ * is no -2), and it works inside a stream capture.  Neither handle's values change.  Returns 0, or -1 for a null mt, src,
+ * in_diag or out_diag, reverse not 0 or 1, an mt that is not a transpose of src, a null in_offd or out_offd where its handle
+ * has offd entries, or an output range overlapping an input range; these are checked before the device is touched.
+ * Collective like bicg_matrix_transpose_values_async: with peers, the entries whose row of the other matrix another rank owns
+ * are stored into that rank's receive region (forward: mt's; reverse: a second region of the transpose's arena on the source
+ * entry's rank, sized at bicg_matrix_create_transpose), between two empty cross-GPU reductions.  A peer timeout is reported
+ * by the next synchronous call on mt. */
+int bicg_matrix_transpose_entries_async(bicg_matrix *mt, bicg_matrix *src, int reverse, const double *in_diag,
+                                        const double *in_offd, double *out_diag, double *out_offd, void *stream);
+
 enum { BICG_METHOD_BICGSTAB = 0, BICG_METHOD_CA = 1, BICG_METHOD_PIPE = 2, BICG_METHOD_PIPE_RR = 3 };
 
 typedef struct {
@@ -418,6 +440,28 @@ int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, double *y, d
                          const double *sigma, int device_vectors);
 int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta,
                                const double *sigma, void *stream);
+
+/* The multiply with caller weights on the handle's pattern: y_j = alpha A_W x_j + beta y_j for j < nvec on this rank's rows,
+ * where A_W is the handle's pattern holding W instead of its values.  W comes in bicg_matrix_set_values' block order: w_diag
+ * has diag nz entries and w_offd offd nz entries (bicg_matrix_block_nz); w_offd may be null only where the handle has no offd
+ * entries.  This is the product the derivative of bicg_matrix_value_grad needs, without a second resident copy of the matrix.
+ *
+ * Arithmetic: bit-identical to bicg_matrix_multiply_async with sigma null on a handle whose values were set to W (same plan,
+ * lanes, order, beta and NaN rules); so with W equal to the handle's values, it is bit-identical to that multiply.  The
+ * handle's values, value tables and persistent-kernel plan are not touched.
+ *
+ * Device pointers, with the ordering and collectivity of bicg_matrix_multiply_async (ghost columns of x_j from the neighbours,
+ * an empty cross-GPU reduction per batch).  W is read in place where the merged order is the block order and the SpMV's tile
+ * copies stay inside w_diag (the row-split plan, or w_diag 16-byte aligned with nnz a multiple of 4); otherwise it is first
+ * staged into merged order in a buffer on the handle.  bicg_matrix_multiply_values_async_prepare allocates that buffer on
+ * every handle where some W may need it (offd entries, or the tile plan), outside any capture; an uncaptured call allocates it
+ * itself.  Returns 0; -1 for a null handle, w_diag, x or y, nvec <= 0, a null w_offd on a handle with offd entries, x
+ * overlapping y, or W overlapping y, checked before the device is touched; -2 inside a stream capture when the prepare has
+ * not run and W needs the staging buffer (the capture stays valid).  The prepare returns 0, or -1 for a null handle; it may
+ * synchronise. */
+int bicg_matrix_multiply_values_async(bicg_matrix *m, int nvec, const double *w_diag, const double *w_offd,
+                                      const double *x, double *y, double alpha, double beta, void *stream);
+int bicg_matrix_multiply_values_async_prepare(bicg_matrix *m);
 
 /* The gradient with respect to the stored values of a resident matrix: for x_j = A^-1 b_j and a loss L, with
  * lambda_j = A^-T dL/dx_j (a solve on the handle of bicg_matrix_create_transpose), dL/da_e = -sum_j lambda_j[i] x_j[c] for every

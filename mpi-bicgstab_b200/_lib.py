@@ -86,6 +86,9 @@ SYMBOLS = {
                                        C.c_int]),
     "bicg_matrix_multiply_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                              C.c_void_p]),
+    "bicg_matrix_multiply_values_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_double, C.c_double, C.c_void_p]),
+    "bicg_matrix_multiply_values_async_prepare": (C.c_int, [C.c_void_p]),
     "bicg_matrix_value_grad": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                          C.c_void_p, C.c_int]),
     "bicg_matrix_value_grad_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
@@ -97,6 +100,8 @@ SYMBOLS = {
     "bicg_matrix_create_transpose": (C.c_void_p, [C.c_void_p]),
     "bicg_matrix_transpose_values": (C.c_int, [C.c_void_p, C.c_void_p]),
     "bicg_matrix_transpose_values_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "bicg_matrix_transpose_entries_async": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                      C.c_void_p, C.c_void_p]),
     "bicg_matrix_block_nz": (C.c_int, [C.c_void_p, _P(C.c_uint), _P(C.c_uint)]),
     "bicg_solve": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, _P(bicg_stats)]),
     "bicg_solve_async": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),

@@ -420,6 +420,7 @@ class DeviceMatrix:
     """A device-resident matrix handle (bicg_matrix): upload once, solve / multiply many times."""
 
     _t = None                  # the transpose prepare_autograd made (or the first backward that needed one)
+    _src = None                # on that transpose: the handle it was made from (not owned; destroy() leaves it alone)
 
     def __init__(self, blk, handle=None):
         """blk: the MatrixBlock to upload; or, with `handle`, an existing bicg_matrix that this object takes over (then blk only
@@ -747,6 +748,96 @@ class DeviceMatrix:
             raise ValueError(f"bicg_matrix_multiply_async failed with {rc}")
         return y
 
+    def _entry_args(self, name, diag, offd):
+        """(name, tensor, expected shape) of an entry vector of this handle in its block order: diag.nz entries, then offd.nz
+        entries where the handle has offd entries (offd may be None where it has none)"""
+        import torch
+        for n_, t in ((name + "_diag", diag), (name + "_offd", offd)):
+            if t is not None and not isinstance(t, torch.Tensor):
+                raise TypeError(f"{n_}: need a CUDA float64 tensor, got {type(t).__name__}")
+        args = [(name + "_diag", diag, (int(self.blk.diag.nz),))]
+        if offd is not None:
+            args.append((name + "_offd", offd, (int(self.blk.offd.nz),)))
+        elif self._has_offd():
+            raise ValueError(f"{name}_offd: the offd block has {int(self.blk.offd.nz)} entries, got None")
+        return args
+
+    def multiply_values_async(self, w_diag, w_offd, x, y=None, alpha=1.0, beta=0.0, stream=None):
+        """bicg_matrix_multiply_values_async: y_j = alpha A_W x_j + beta y_j for every row x_j of x, where A_W is this handle's
+        pattern holding the weights W = (w_diag, w_offd) in set_values' block order instead of its values; bit-identical to
+        multiply_async on a handle whose values were set to W.  Contiguous CUDA float64 tensors only: x of shape (n_loc,) or
+        (nvec, n_loc), y the same (allocated when None; then beta must be 0).  Enqueued on `stream` (default: torch's current
+        stream) behind the handle's earlier work with no host synchronisation.  Inside torch.cuda.graph, call
+        prepare_multiply_values_async first.  Collective over the ranks.  Returns y."""
+        import torch
+        for name, t in (("x", x), ("y", y)):
+            if t is not None and not isinstance(t, torch.Tensor):
+                raise TypeError(f"{name}: multiply_values_async takes CUDA tensors only, got {type(t).__name__}")
+        shape = self._multiply_shape(x)
+        nvec = shape[0] if len(shape) == 2 else 1
+        allocated = y is None
+        if allocated:
+            if beta != 0.0:
+                raise ValueError("y: needed when beta != 0")
+            y = x.new_empty(shape, dtype=torch.float64)
+        wargs = self._entry_args("w", w_diag, w_offd)
+        ptrs = _checked_cuda_vectors(("x", x, shape), ("y", y, shape), *wargs)
+        if stream is None:
+            stream = torch.cuda.current_stream(x.device)
+        if allocated and stream != torch.cuda.current_stream(x.device):
+            y.record_stream(stream)               # written on `stream`, not on the one it was allocated on
+        rc = lib.bicg_matrix_multiply_values_async(self.h, nvec, ptrs[2], ptrs[3] if len(ptrs) > 3 else None, ptrs[0], ptrs[1],
+                                                   float(alpha), float(beta), C.c_void_p(stream.cuda_stream))
+        if rc == -2:
+            raise RuntimeError("multiply_values_async inside a stream capture needs prepare_multiply_values_async() first")
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_multiply_values_async failed with {rc}")
+        return y
+
+    def prepare_multiply_values_async(self):
+        """bicg_matrix_multiply_values_async_prepare: allocate the buffer multiply_values_async stages weights into where it
+        cannot read them in place (a handle with offd entries, or on the TMA tile plan), outside any capture; afterwards
+        multiply_values_async works inside torch.cuda.graph with any weights."""
+        if lib.bicg_matrix_multiply_values_async_prepare(self.h) != 0:
+            raise ValueError("bicg_matrix_multiply_values_async_prepare failed")
+
+    def transpose_entries_async(self, src, in_diag, in_offd=None, reverse=False, out=None, stream=None):
+        """bicg_matrix_transpose_entries_async, with this handle the transpose of the DeviceMatrix src: reverse=False maps an
+        entry vector (in_diag, in_offd) in src's block order to this handle's, exactly as transpose_values maps src's values;
+        reverse=True maps one in this handle's order back to src's.  Pure copies: reverse after forward gives back every bit.
+        out: (out_diag, out_offd) to write, allocated when None (out_offd None where the output side has no offd entries).
+        Contiguous CUDA float64 tensors only, enqueued on `stream` (default: torch's current stream) behind both handles'
+        earlier work with no host synchronisation; works inside torch.cuda.graph with no prepare step.  Collective over the
+        ranks.  Returns (out_diag, out_offd)."""
+        import torch
+        if not isinstance(src, DeviceMatrix):
+            raise TypeError(f"src: need a DeviceMatrix, got {type(src).__name__}")
+        a, b = (self, src) if reverse else (src, self)
+        iargs = a._entry_args("in", in_diag, in_offd)
+        allocated = out is None
+        if allocated:
+            if not isinstance(in_diag, torch.Tensor):
+                raise TypeError(f"in_diag: need a CUDA float64 tensor, got {type(in_diag).__name__}")
+            out = (in_diag.new_empty((int(b.blk.diag.nz),)),
+                   in_diag.new_empty((int(b.blk.offd.nz),)) if b._has_offd() else None)
+        if not (isinstance(out, (tuple, list)) and len(out) == 2):
+            raise TypeError("out: need a pair (out_diag, out_offd)")
+        oargs = b._entry_args("out", out[0], out[1])
+        ptrs = _checked_cuda_vectors(*iargs, *oargs)
+        ip, op_ = ptrs[:len(iargs)], ptrs[len(iargs):]
+        if stream is None:
+            stream = torch.cuda.current_stream(in_diag.device)
+        if allocated and stream != torch.cuda.current_stream(in_diag.device):
+            for t in out:
+                if t is not None:
+                    t.record_stream(stream)       # written on `stream`, not on the one it was allocated on
+        rc = lib.bicg_matrix_transpose_entries_async(self.h, src.h, 1 if reverse else 0, ip[0], ip[1] if len(ip) > 1 else None,
+                                                     op_[0], op_[1] if len(op_) > 1 else None, C.c_void_p(stream.cuda_stream))
+        if rc != 0:
+            raise ValueError(f"bicg_matrix_transpose_entries_async failed with {rc} (src is not the matrix this one was "
+                             f"transposed from, or out overlaps the input)")
+        return out[0], (out[1] if len(op_) > 1 else None)
+
     def _has_offd(self):
         """whether the handle holds offd entries (with one rank the offd block is ignored)"""
         return int(self.blk.offd.nz) > 0 and lib.bicg_comm_world() > 1
@@ -819,33 +910,42 @@ class DeviceMatrix:
         """What solve_autograd and multiply_autograd on this handle need inside torch.cuda.graph: creates and keeps this
         handle's transpose (transpose(): host work, collective over the ranks) and runs prepare_async(method) on both handles.
         Call it outside any capture.  destroy() destroys the transpose too."""
-        if self._t is None:
-            self._t = self.transpose()
+        t = self._adjoint()
         self.prepare_async(method)
-        self._t.prepare_async(method)
+        t.prepare_async(method)
+        self.prepare_multiply_values_async()
+        t.prepare_multiply_values_async()
 
     def prepare_shifted_autograd(self, method, sigma_len, adjoint_method="bicgstab"):
         """What shifted_solve_autograd on this handle needs inside torch.cuda.graph: creates and keeps the transpose as
         prepare_autograd does, runs prepare_shifted_async(method, sigma_len) here and prepare_async(adjoint_method) on the
         transpose, and finds the transpose's diagonal positions for shift_diagonal_async.  Call it outside any capture.
         Collective over the ranks; raises ValueError on every rank when a row of A^T on any rank has no diagonal entry."""
-        if self._t is None:
-            self._t = self.transpose()
+        t = self._adjoint()
         self.prepare_shifted_async(method, sigma_len)
-        self._t.prepare_async(adjoint_method)
-        if lib.bicg_matrix_shift_diagonal_async_prepare(self._t.h) != 0:
+        t.prepare_async(adjoint_method)
+        if lib.bicg_matrix_shift_diagonal_async_prepare(t.h) != 0:
             raise ValueError("prepare_shifted_autograd: a row of A^T has no diagonal entry (a column of A without one, on this or "
                              "another rank), so A^T + sigma I cannot be formed by shifting stored entries")
+        # a second backward solves with A + sigma_j I here; a matrix without a stored diagonal entry in every row is refused
+        # then, when that shift is asked for, so first-order use of such a matrix still works
+        self.prepare_async(adjoint_method)
+        lib.bicg_matrix_shift_diagonal_async_prepare(self.h)
+        self.prepare_multiply_values_async()
+        t.prepare_multiply_values_async()
 
     def _adjoint(self):
         """The transpose the backward of a differentiable solve or multiply runs on: the one prepare_autograd made, else created
-        here, which a stream capture cannot hold."""
+        here, which a stream capture cannot hold.  For a transpose made here, its source: (A^T)^T is never created."""
+        if self._src is not None:
+            return self._src
         if self._t is None:
             import torch
             if torch.cuda.is_current_stream_capturing():
                 raise RuntimeError("a backward through this DeviceMatrix inside a CUDA graph capture needs "
                                    "dm.prepare_autograd(method) before the capture: creating the transpose is host work")
             self._t = self.transpose()
+            self._t._src = self
         return self._t
 
     def spmv(self, x_loc):
@@ -892,6 +992,7 @@ class DeviceMatrix:
         if self._t is not None:
             self._t.destroy()
             self._t = None
+        self._src = None
         if self.h:
             lib.bicg_matrix_destroy(self.h)
             self.h = None

@@ -7,6 +7,8 @@
 #include "vec.cuh"
 #include "mega.cuh"
 
+#include <algorithm>
+#include <cstdint>
 #include <cstdio>
 #include <cstdlib>
 #include <functional>
@@ -286,6 +288,21 @@ struct bicg_matrix {
     double *d_trecv = nullptr;
     size_t t_nrecv = 0;
     double *peer_trecv[bicg::MAX_RANKS] = {};
+    // the same tables over the block orders set_values takes, for bicg_matrix_transpose_entries_async (an entry's block index
+    // is j for diag entry j, diag nz + j for offd entry j; they alias d_tperm / d_tpush where block and merged order agree):
+    // d_tbperm[b] is the source block index entry b of this handle is copied from (>= 0) or ~slot; d_tbpush pushes source
+    // block indices.  The reverse direction: d_trpush sends each received entry (src: this handle's block index) back to the
+    // reverse region of the source's rank, at d_trecv + t_rev_off there, whose entry e belongs to source block index
+    // d_trev_src[e] (e < t_npush: the entries this rank pushes forward, in push order)
+    int *d_tbperm = nullptr;
+    bicg::TransposePush *d_tbpush = nullptr;
+    bicg::TransposePush *d_trpush = nullptr;
+    int t_nrpush = 0;
+    int *d_trev_src = nullptr;
+    size_t t_rev_off = 0;
+    // bicg_matrix_multiply_values_async: caller weights staged into merged order (nnz + 16 doubles), where they cannot be read
+    // in place; allocated by bicg_matrix_multiply_values_async_prepare
+    double *d_wval = nullptr;
 
     double *vec(int id) const { return vec_base + (long long)id * vstride; }
 };
@@ -300,6 +317,14 @@ double matrix_upload_ms(bicg_matrix *m);
 bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, const INFO_Matrix *info, bool *fresh);
 // the persistent kernel's value tables and packed values from d_val, on st: what creation and every value update run last
 void launch_value_tables(const bicg_matrix *m, cudaStream_t st);
+// device values in the block order set_values takes -> out in m's merged order (nnz doubles), on st
+void merge_values(const bicg_matrix *m, const double *diag_val, const double *offd_val, double *out, cudaStream_t st);
+// [a, a + abytes) and [b, b + bbytes) overlap; an empty range counts as one byte
+inline bool overlaps(const void *a, size_t abytes, const void *b, size_t bbytes)
+{
+    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+    return a0 < b0 + std::max<size_t>(bbytes, 1) && b0 < a0 + std::max<size_t>(abytes, 1);
+}
 // solve.cu
 int  solve(bicg_matrix *m, int method, double *x, double *r, int krr, int nrr, int device_vectors, bicg_stats *st);
 

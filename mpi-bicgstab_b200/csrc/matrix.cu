@@ -980,6 +980,9 @@ void matrix_destroy(bicg_matrix *m)
     c.dev_free(m->d_val); c.dev_free(m->d_col); c.dev_free(m->d_ptr);
     c.dev_free(m->d_blk_ptr); c.dev_free(m->d_diag_pos);
     c.dev_free(m->d_tperm); c.dev_free(m->d_tpush);
+    if (m->d_tbperm != m->d_tperm) c.dev_free(m->d_tbperm);
+    if (m->d_tbpush != m->d_tpush) c.dev_free(m->d_tbpush);
+    c.dev_free(m->d_trpush); c.dev_free(m->d_trev_src); c.dev_free(m->d_wval);
     if (m->world > 1) c.arena_pool.emplace(m->arena_bytes, Context::ArenaRec{m->arena, m->arena_bytes, m->arena_id, m->arena_handle});
     else c.dev_free(m->arena);
     delete m;
@@ -1046,17 +1049,26 @@ bicg_matrix *matrix_get_cached(const CSR_Matrix *diag, const CSR_Matrix *offd, c
 // value updates: everything but d_val and what matrix_create derived from it (the value tables and packed values of the
 // persistent kernel's plan) depends on the pattern alone and stays
 // ------------------------------------------------------------------------------------------------
+void merge_values(const bicg_matrix *m, const double *diag_val, const double *offd_val, double *out, cudaStream_t st)
+{
+    const size_t no = m->nnz_offd, nd = m->nnz - no;
+    if (!no) {
+        if (nd) BICG_CUDA(cudaMemcpyAsync(out, diag_val, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
+        return;
+    }
+    const size_t np1 = (size_t)m->n_loc + 1;
+    merge_values_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_blk_ptr, m->d_blk_ptr + np1, diag_val, offd_val, out);
+    BICG_CUDA(cudaGetLastError());
+}
+
 // d_val from the caller's values (device pointers, or host pointers when there are no offd entries), then the value tables, on st
 static void enqueue_values(bicg_matrix *m, const double *diag_val, const double *offd_val, bool device_ptrs, cudaStream_t st)
 {
     const size_t no = m->nnz_offd, nd = m->nnz - no;
-    if (!no) {
-        if (nd && device_ptrs) BICG_CUDA(cudaMemcpyAsync(m->d_val, diag_val, nd * sizeof(double), cudaMemcpyDeviceToDevice, st));
-        else if (nd) ctx().h2d(m->d_val, diag_val, nd * sizeof(double));
+    if (!no && !device_ptrs) {
+        if (nd) ctx().h2d(m->d_val, diag_val, nd * sizeof(double));
     } else {
-        const size_t np1 = (size_t)m->n_loc + 1;
-        merge_values_kernel<<<row_blocks(m->n_loc), 256, 0, st>>>(m->n_loc, m->d_blk_ptr, m->d_blk_ptr + np1, diag_val, offd_val, m->d_val);
-        BICG_CUDA(cudaGetLastError());
+        merge_values(m, diag_val, offd_val, m->d_val, st);
     }
     launch_value_tables(m, st);
 }

@@ -9,6 +9,10 @@
 // vector, so the kernel reads one extended vector, and pushes the boundary runs into the same slot on its neighbours.  Each
 // launch then ends in an empty cross-GPU reduction, so no rank pushes the next batch into a slot a peer is still reading.
 // HaloBatches does this staging for the value gradient (value_grad.cu) too.
+//
+// bicg_matrix_multiply_values_async runs the same launches with caller weights W in place of the handle's values: the kernels
+// read their values through SpmvArgs::val, which points at W itself where W's block order is the merged order and the tile
+// kernel's bulk copies stay inside it, and otherwise at m->d_wval, into which W is first staged (merge_values).
 #include "engine.hpp"
 
 #include <algorithm>
@@ -29,6 +33,16 @@ bool bad_args(const bicg_matrix *m, int nvec, const double *x, const double *y)
     const uintptr_t bytes = std::max<uintptr_t>((uintptr_t)nvec * (uintptr_t)m->n_loc * sizeof(double), sizeof(double));
     const uintptr_t x0 = (uintptr_t)x, y0 = (uintptr_t)y;
     return x0 < y0 + bytes && y0 < x0 + bytes;
+}
+
+// W is staged into merged order where it has offd entries, and on the tile plan unless the tile kernel's bulk copies, which
+// read whole 16-byte units from 16-byte aligned addresses, stay inside w_diag: W 16-byte aligned, nnz a multiple of 4.  Only
+// the row-split plan without offd entries never needs the staging buffer.
+bool weights_may_stage(const bicg_matrix *m) { return m->nnz_offd || m->plan.kind == 0; }
+bool weights_in_place(const bicg_matrix *m, const double *w_diag)
+{
+    if (m->nnz_offd) return false;
+    return m->plan.kind != 0 || ((uintptr_t)w_diag % 16 == 0 && m->nnz % 4 == 0);
 }
 
 } // namespace
@@ -62,16 +76,16 @@ void HaloBatches::stage(const double *x, int j0, int nv, const double *(&xs)[MUL
 
 namespace {
 
-// every batch of one multiply on st: x, y device pointers, sigma nvec device values or null
-void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, double alpha, double beta, const double *sigma,
-                      cudaStream_t st)
+// every batch of one multiply on st with the values val (merged order): x, y device pointers, sigma nvec device values or null
+void enqueue_multiply(bicg_matrix *m, const double *val, int nvec, const double *x, double *y, double alpha, double beta,
+                      const double *sigma, cudaStream_t st)
 {
     const SpmvPlan &p = m->plan;
     const long long n = m->n_loc;
     HaloBatches hb(m, st);
     SpmvArgs a{};
     a.kc = hb.kc;
-    a.val = m->d_val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
+    a.val = val; a.col = m->d_col; a.ptr = m->d_ptr; a.rows = m->n_loc;
     a.tile_row = p.d_tile_row; a.tile_nz = p.d_tile_nz; a.ntiles = p.ntiles; a.cap = p.cap; a.stages = p.stages;
     a.alpha = alpha; a.beta = beta;
     a.wait_halo = hb.wait_halo;
@@ -87,6 +101,17 @@ void enqueue_multiply(bicg_matrix *m, int nvec, const double *x, double *y, doub
                       p.threads, p.grid, nv, cudaGetErrorString((cudaError_t)rc));
         ++ctx().launches;
     }
+}
+
+// m->d_wval, outside any capture
+void alloc_weights(bicg_matrix *m)
+{
+    if (m->d_wval) return;
+    Context &c = ctx();
+    wait_handle(m);
+    m->d_wval = (double *)c.dev_alloc((m->nnz + 16) * sizeof(double));
+    BICG_CUDA(cudaMemsetAsync(m->d_wval, 0, (m->nnz + 16) * sizeof(double), c.stream));
+    BICG_CUDA(cudaStreamSynchronize(c.stream));
 }
 
 } // namespace
@@ -115,7 +140,7 @@ extern "C" int bicg_matrix_multiply(bicg_matrix *m, int nvec, const double *x, d
         d_sigma = (double *)c.dev_alloc((size_t)nvec * sizeof(double));
         BICG_CUDA(cudaMemcpyAsync(d_sigma, sigma, (size_t)nvec * sizeof(double), cudaMemcpyHostToDevice, c.stream));
     }
-    enqueue_multiply(m, nvec, dx, dy, alpha, beta, d_sigma, c.stream);
+    enqueue_multiply(m, m->d_val, nvec, dx, dy, alpha, beta, d_sigma, c.stream);
     if (!device_vectors) BICG_CUDA(cudaMemcpyAsync(y, dy, bytes, cudaMemcpyDeviceToHost, c.stream));
     sync_checked(m, "a multiply");
     c.dev_free(tmp); c.dev_free(d_sigma);
@@ -129,6 +154,38 @@ extern "C" int bicg_matrix_multiply_async(bicg_matrix *m, int nvec, const double
     if (bad_args(m, nvec, x, y)) return -1;
     ctx().ensure();
     const cudaStream_t st = (cudaStream_t)stream;
-    stream_ordered({m}, st, capturing(st), [&] { enqueue_multiply(m, nvec, x, y, alpha, beta, sigma, st); });
+    stream_ordered({m}, st, capturing(st), [&] { enqueue_multiply(m, m->d_val, nvec, x, y, alpha, beta, sigma, st); });
+    return 0;
+}
+
+extern "C" int bicg_matrix_multiply_values_async_prepare(bicg_matrix *m)
+{
+    using namespace bicg;
+    if (!m) return -1;
+    ctx().ensure();
+    if (weights_may_stage(m)) alloc_weights(m);
+    return 0;
+}
+
+extern "C" int bicg_matrix_multiply_values_async(bicg_matrix *m, int nvec, const double *w_diag, const double *w_offd,
+                                                 const double *x, double *y, double alpha, double beta, void *stream)
+{
+    using namespace bicg;
+    if (bad_args(m, nvec, x, y) || !w_diag || (m->nnz_offd && !w_offd)) return -1;
+    const size_t no = m->nnz_offd, nd = m->nnz - no;
+    const size_t ybytes = (size_t)nvec * (size_t)m->n_loc * sizeof(double);
+    if (overlaps(w_diag, nd * sizeof(double), y, ybytes) || (no && overlaps(w_offd, no * sizeof(double), y, ybytes))) return -1;
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    const bool captured = capturing(st);
+    const bool in_place = weights_in_place(m, w_diag);
+    if (!in_place && !m->d_wval) {
+        if (captured) return -2;
+        alloc_weights(m);
+    }
+    stream_ordered({m}, st, captured, [&] {
+        if (!in_place) merge_values(m, w_diag, w_offd, m->d_wval, st);
+        enqueue_multiply(m, in_place ? w_diag : m->d_wval, nvec, x, y, alpha, beta, nullptr, st);
+    });
     return 0;
 }

@@ -11,6 +11,11 @@
 // d_val through d_tperm; one whose row of A another rank owns comes from the receive region in the transpose's arena, which
 // that rank fills first with a push kernel through the IPC mapping.  Then the value tables are rebuilt by the pass every value
 // update runs.  Nothing here is in a solver loop.
+//
+// Entry permutation (bicg_matrix_transpose_entries_async): the refresh's copies on caller vectors in the block orders
+// set_values takes, forward (source -> transpose) through the same push and gather over block-order tables, and reverse
+// through the opposite traffic: every transposed entry that came from another rank goes back into a second region of that
+// rank's receive area, from which it is scattered to its source position.  All tables are built here at creation.
 #include "engine.hpp"
 
 #include <algorithm>
@@ -22,48 +27,112 @@ namespace {
 
 struct PushDst { double *recv[MAX_RANKS]; };
 
-// the source's values that other ranks' transposes hold, into their receive regions
-__global__ void __launch_bounds__(256) transpose_push_kernel(const double *__restrict__ src_val, const TransposePush *__restrict__ runs,
-                                                             int n, const __grid_constant__ PushDst dst)
+// an entry vector read by index: merged values (diag = d_val, nd = nnz), or the two blocks set_values takes (index b < nd is
+// diag entry b, else offd entry b - nd)
+struct Entries {
+    const double *diag, *offd;
+    size_t nd;
+    __device__ __forceinline__ double operator[](size_t b) const { return b < nd ? diag[b] : offd[b - nd]; }
+};
+struct OutEntries {
+    double *diag, *offd;
+    size_t nd;
+    __device__ __forceinline__ double &operator[](size_t b) const { return b < nd ? diag[b] : offd[b - nd]; }
+};
+
+// the entries of `in` that other ranks hold, into their receive regions
+__global__ void __launch_bounds__(256) transpose_push_kernel(const Entries in, const TransposePush *__restrict__ runs, int n,
+                                                             const __grid_constant__ PushDst dst)
 {
     for (int e = blockIdx.x * blockDim.x + threadIdx.x; e < n; e += gridDim.x * blockDim.x) {
         const TransposePush p = runs[e];
-        dst.recv[p.rank][p.slot] = src_val[p.src];
+        dst.recv[p.rank][p.slot] = in[(size_t)p.src];
     }
 }
 
-// every merged value of the transpose: a local source value or a received one
-__global__ void __launch_bounds__(256) transpose_gather_kernel(const double *__restrict__ src_val, const double *__restrict__ recv,
-                                                               const int *__restrict__ perm, size_t n, double *__restrict__ val)
+// every entry of the transpose: a local source entry or a received one
+__global__ void __launch_bounds__(256) transpose_gather_kernel(const Entries in, const double *__restrict__ recv,
+                                                               const int *__restrict__ perm, size_t n, const OutEntries out)
 {
     for (size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) {
         const int s = perm[k];
-        val[k] = s >= 0 ? src_val[s] : recv[~s];
+        out[k] = s >= 0 ? in[(size_t)s] : recv[~s];
+    }
+}
+
+// the inverse of a gather over the entries with perm[k] >= 0: out[perm[k]] = in[k]
+__global__ void __launch_bounds__(256) transpose_scatter_kernel(const Entries in, const int *__restrict__ perm, size_t n,
+                                                                const OutEntries out)
+{
+    for (size_t k = blockIdx.x * (size_t)blockDim.x + threadIdx.x; k < n; k += (size_t)gridDim.x * blockDim.x) {
+        const int s = perm[k];
+        if (s >= 0) out[(size_t)s] = in[k];
     }
 }
 
 int grid_for(size_t n) { return (int)std::max<size_t>(1, std::min<size_t>((n + 255) / 256, (size_t)ctx().sm_count * 8)); }
 
+PushDst push_dst(const bicg_matrix *mt)
+{
+    PushDst dst{};
+    for (int p = 0; p < mt->world; ++p) dst.recv[p] = mt->peer_trecv[p];
+    return dst;
+}
+
+// with peers: `runs` (n of them) store entries of `in` into the receive regions of mt's peers, between two empty cross-GPU
+// reductions: nobody stores into a receive region its owner has not consumed yet, and then every push has landed
+void exchange(bicg_matrix *mt, const Entries &in, const TransposePush *runs, int n, cudaStream_t st)
+{
+    BICG_CUDA(cudaMemsetAsync(&mt->d_sc->done, 0, sizeof(int), st));
+    peer_barrier(mt, st);
+    if (n) {
+        transpose_push_kernel<<<grid_for((size_t)n), 256, 0, st>>>(in, runs, n, push_dst(mt));
+        BICG_CUDA(cudaGetLastError());
+    }
+    peer_barrier(mt, st);
+}
+
 // the refresh on st, behind both handles' earlier work (the caller has made st wait for it)
 void enqueue_refresh(bicg_matrix *mt, const bicg_matrix *src, cudaStream_t st)
 {
-    if (mt->world > 1) {
-        // nobody stores into a receive region its owner has not consumed yet; then every push has landed
-        BICG_CUDA(cudaMemsetAsync(&mt->d_sc->done, 0, sizeof(int), st));
-        peer_barrier(mt, st);
-        if (mt->t_npush) {
-            PushDst dst{};
-            for (int p = 0; p < mt->world; ++p) dst.recv[p] = mt->peer_trecv[p];
-            transpose_push_kernel<<<grid_for((size_t)mt->t_npush), 256, 0, st>>>(src->d_val, mt->d_tpush, mt->t_npush, dst);
-            BICG_CUDA(cudaGetLastError());
-        }
-        peer_barrier(mt, st);
-    }
+    const Entries in{src->d_val, nullptr, src->nnz};
+    if (mt->world > 1) exchange(mt, in, mt->d_tpush, mt->t_npush, st);
     if (mt->nnz) {
-        transpose_gather_kernel<<<grid_for(mt->nnz), 256, 0, st>>>(src->d_val, mt->d_trecv, mt->d_tperm, mt->nnz, mt->d_val);
+        transpose_gather_kernel<<<grid_for(mt->nnz), 256, 0, st>>>(in, mt->d_trecv, mt->d_tperm, mt->nnz,
+                                                                  OutEntries{mt->d_val, nullptr, mt->nnz});
         BICG_CUDA(cudaGetLastError());
     }
     launch_value_tables(mt, st);
+}
+
+// bicg_matrix_transpose_entries_async on st: forward, src's block order -> mt's, the refresh's traffic on entry vectors; reverse,
+// mt's block order -> src's, every entry back where the forward took it from
+void enqueue_entries(bicg_matrix *mt, const bicg_matrix *src, int reverse, const double *in_diag, const double *in_offd,
+                     double *out_diag, double *out_offd, cudaStream_t st)
+{
+    const size_t snd = src->nnz - src->nnz_offd, tnd = mt->nnz - mt->nnz_offd;
+    if (!reverse) {
+        const Entries in{in_diag, in_offd, snd};
+        if (mt->world > 1) exchange(mt, in, mt->d_tbpush, mt->t_npush, st);
+        if (mt->nnz) {
+            transpose_gather_kernel<<<grid_for(mt->nnz), 256, 0, st>>>(in, mt->d_trecv, mt->d_tbperm, mt->nnz,
+                                                                      OutEntries{out_diag, out_offd, tnd});
+            BICG_CUDA(cudaGetLastError());
+        }
+        return;
+    }
+    const Entries in{in_diag, in_offd, tnd};
+    const OutEntries out{out_diag, out_offd, snd};
+    if (mt->world > 1) exchange(mt, in, mt->d_trpush, mt->t_nrpush, st);
+    if (mt->nnz) {
+        transpose_scatter_kernel<<<grid_for(mt->nnz), 256, 0, st>>>(in, mt->d_tbperm, mt->nnz, out);
+        BICG_CUDA(cudaGetLastError());
+    }
+    if (mt->t_npush) {
+        const Entries back{mt->d_trecv + mt->t_rev_off, nullptr, (size_t)mt->t_npush};
+        transpose_scatter_kernel<<<grid_for((size_t)mt->t_npush), 256, 0, st>>>(back, mt->d_trev_src, (size_t)mt->t_npush, out);
+        BICG_CUDA(cudaGetLastError());
+    }
 }
 
 // the -1 case of both refresh calls: mt is not a transpose of src
@@ -134,6 +203,7 @@ extern "C" bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m)
     std::vector<unsigned> send(2 * max_send, 0);
     std::vector<TransposePush> push;
     push.reserve(send_off[(size_t)W]);
+    std::vector<int> rev_src(send_off[(size_t)W]);               // reverse region entry e (grouped by peer): source merged entry
     {
         std::vector<size_t> fill(send_off.begin(), send_off.end() - 1);
         for (int i = 0; i < n_loc; ++i)
@@ -144,6 +214,7 @@ extern "C" bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m)
                 const size_t e = fill[(size_t)p]++;
                 send[2 * e] = lo + (unsigned)i; send[2 * e + 1] = g;
                 push.push_back(TransposePush{(int)k, p, slot_base(me, p) + (int)(e - send_off[(size_t)p])});
+                rev_src[e] = (int)k;
             }
     }
     std::vector<unsigned> recv;
@@ -212,8 +283,51 @@ extern "C" bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m)
     memcpy(info.code, "MCRG", 4);
     info.recvcounts = recvcounts.data(); info.displs = displs.data();
 
-    bicg_matrix *mt = matrix_create(&D, &O, &info, nrecv);
+    // the receive region holds the forward entries (nrecv), then the reverse region: the entries this rank pushes forward
+    bicg_matrix *mt = matrix_create(&D, &O, &info, nrecv + push.size());
     mt->t_src_uid = m->uid;
+    mt->t_rev_off = nrecv;
+
+    // ---- the tables over block orders (bicg_matrix_transpose_entries_async) ---------------------------------------------
+    // merged entry -> block index, on either handle: row i's diag entries, then its offd entries (dev.cuh: merge_row)
+    auto block_index = [&](const std::vector<unsigned> &bp, int rows) {
+        std::vector<int> b;
+        if (bp.empty()) return b;                                   // no offd entries: the orders agree
+        const unsigned *bd = bp.data(), *bo = bp.data() + rows + 1;
+        const int nd = (int)bd[rows];
+        b.reserve((size_t)nd + bo[rows]);
+        for (int i = 0; i < rows; ++i) {
+            for (unsigned j = bd[i]; j < bd[i + 1]; ++j) b.push_back((int)j);
+            for (unsigned j = bo[i]; j < bo[i + 1]; ++j) b.push_back(nd + (int)j);
+        }
+        return b;
+    };
+    std::vector<unsigned> sbp, tbp;
+    if (m->nnz_offd) d2h(sbp, m->d_blk_ptr, 2 * ((size_t)n_loc + 1));
+    if (mt->nnz_offd) {
+        tbp.assign(dptr.begin(), dptr.end());
+        tbp.insert(tbp.end(), optr.begin(), optr.end());
+    }
+    const std::vector<int> sblk = block_index(sbp, n_loc), tblk = block_index(tbp, n_loc);
+    auto sb = [&](int k) { return sblk.empty() ? k : sblk[(size_t)k]; };
+    auto tb = [&](size_t k) { return tblk.empty() ? k : (size_t)tblk[k]; };
+    std::vector<int> bperm(perm.size());
+    for (size_t k = 0; k < perm.size(); ++k) bperm[tb(k)] = perm[k] >= 0 ? sb(perm[k]) : perm[k];
+    std::vector<TransposePush> bpush(push);
+    for (TransposePush &p : bpush) p.src = sb(p.src);
+    for (int &k : rev_src) k = sb(k);
+    // every received entry goes back to the rank q that pushed it: slot s of my region is q's t-th entry for me, which sits at
+    // t_rev_off(q) + (q's entries for lower ranks) + t in q's receive region
+    std::vector<TransposePush> rpush;
+    for (size_t k = 0; k < perm.size(); ++k) {
+        if (perm[k] >= 0) continue;
+        int s = ~perm[k], q = 0;
+        while (s >= cnt_all[(size_t)q * W + me]) s -= cnt_all[(size_t)q++ * W + me];
+        int base = 0;
+        for (int r = 0; r < W; ++r) base += cnt_all[(size_t)r * W + q];            // q's nrecv
+        for (int r = 0; r < me; ++r) base += cnt_all[(size_t)q * W + r];
+        rpush.push_back(TransposePush{(int)tb(k), q, base + s});
+    }
     if (!perm.empty()) {
         mt->d_tperm = (int *)c.dev_alloc(perm.size() * sizeof(int));
         BICG_CUDA(cudaMemcpyAsync(mt->d_tperm, perm.data(), perm.size() * sizeof(int), cudaMemcpyHostToDevice, c.stream));
@@ -223,6 +337,22 @@ extern "C" bicg_matrix *bicg_matrix_create_transpose(bicg_matrix *m)
         mt->d_tpush = (TransposePush *)c.dev_alloc(push.size() * sizeof(TransposePush));
         BICG_CUDA(cudaMemcpyAsync(mt->d_tpush, push.data(), push.size() * sizeof(TransposePush), cudaMemcpyHostToDevice, c.stream));
     }
+    auto upload = [&](auto &v, auto *alias) {
+        using T = typename std::decay_t<decltype(v)>::value_type;
+        if (v.empty()) return (T *)nullptr;
+        if (alias && std::equal(v.begin(), v.end(), alias, [](const T &a, const T &b) { return !memcmp(&a, &b, sizeof(T)); }))
+            return (T *)nullptr;
+        T *d = (T *)c.dev_alloc(v.size() * sizeof(T));
+        BICG_CUDA(cudaMemcpyAsync(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice, c.stream));
+        return d;
+    };
+    mt->d_tbperm = upload(bperm, perm.data());
+    if (!mt->d_tbperm) mt->d_tbperm = mt->d_tperm;
+    mt->d_tbpush = upload(bpush, push.data());
+    if (!mt->d_tbpush) mt->d_tbpush = mt->d_tpush;
+    mt->d_trpush = upload(rpush, (const TransposePush *)nullptr);
+    mt->t_nrpush = (int)rpush.size();
+    mt->d_trev_src = upload(rev_src, (const int *)nullptr);
     // the values: the refresh every later bicg_matrix_transpose_values runs
     enqueue_refresh(mt, m, c.stream);
     sync_checked(mt, "the creation of a transpose");
@@ -250,5 +380,25 @@ extern "C" int bicg_matrix_transpose_values_async(bicg_matrix *mt, bicg_matrix *
     ctx().ensure();
     const cudaStream_t st = (cudaStream_t)stream;
     stream_ordered({mt, src}, st, capturing(st), [&] { enqueue_refresh(mt, src, st); });
+    return 0;
+}
+
+extern "C" int bicg_matrix_transpose_entries_async(bicg_matrix *mt, bicg_matrix *src, int reverse, const double *in_diag,
+                                                   const double *in_offd, double *out_diag, double *out_offd, void *stream)
+{
+    using namespace bicg;
+    if (!mt || !src || (reverse != 0 && reverse != 1) || !in_diag || !out_diag) return -1;
+    const bicg_matrix *a = reverse ? mt : src, *b = reverse ? src : mt;         // in's handle, out's handle
+    const size_t ano = a->nnz_offd, and_ = a->nnz - ano, bno = b->nnz_offd, bnd = b->nnz - bno;
+    if ((ano && !in_offd) || (bno && !out_offd)) return -1;
+    auto hits_in = [&](const void *o, size_t n) {
+        return overlaps(o, n * sizeof(double), in_diag, and_ * sizeof(double)) ||
+               (ano && overlaps(o, n * sizeof(double), in_offd, ano * sizeof(double)));
+    };
+    if (hits_in(out_diag, bnd) || (bno && hits_in(out_offd, bno)) || transpose_bad(mt, src)) return -1;
+    ctx().ensure();
+    const cudaStream_t st = (cudaStream_t)stream;
+    stream_ordered({mt, src}, st, capturing(st),
+                   [&] { enqueue_entries(mt, src, reverse, in_diag, in_offd, out_diag, out_offd, st); });
     return 0;
 }

@@ -88,12 +88,6 @@ int launch_value_grad(int lanes, int grid, const ValueGradArgs &a, cudaStream_t 
     return (int)cudaGetLastError();
 }
 
-bool overlaps(const void *a, size_t abytes, const void *b, size_t bbytes)
-{
-    const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
-    return a0 < b0 + std::max<size_t>(bbytes, 1) && b0 < a0 + std::max<size_t>(abytes, 1);
-}
-
 // the checks both calls make before the device is touched: -1 cases of include/bicgstab_b200.h
 bool bad_args(const bicg_matrix *m, int nvec, const double *u, const double *v, const double *diag_out, const double *offd_out)
 {
